@@ -3,15 +3,15 @@
 
 Headline workload (BASELINE.json configs[1]): torchvision.ops.roi_align, 256-ch 200x272 fp32 FPN feature map, 1000 RoIs,
 7x7 output, spatial_scale 0.25, sampling_ratio 2.  A "step" = one roi_align call over one such batch through the
-reference-facing API (torchvision.ops.roi_align after vision_b200.install() -> dispatcher -> C ABI -> sm_100a kernels).
+reference-facing API (torchvision.ops.roi_align after vision_b200.install() -> dispatcher -> C ABI -> sm_90a kernels).
 The other BASELINE configurations are measured in the same run as first-class blocks under "configs" (each with its own
-`value`, `roofline`, `cpu_baseline`, `e2e`, and `gpu_reference` = the reference's own sm_100 CUDA kernels from the installed
+`value`, `roofline`, `cpu_baseline`, `e2e`, and `gpu_reference` = the reference's own CUDA kernels from the installed
 wheel, same inputs, same box):
     cfg3  batched_nms   100k boxes x 80 classes per image, fp32, 4 images per rank          boxes/s
-    cfg4  deform_conv2d 3x3, N=32 C=512->512 64x64, bf16 (tcgen05 path)                      TFLOP/s
+    cfg4  deform_conv2d 3x3, N=32 C=512->512 64x64, bf16 (wgmma path)                        TFLOP/s
     cfg5  resize        bilinear antialias, 128 x 3x2160x3840 fp16 -> 224x224 per rank       images/s
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--configs 2,3,4,5]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--configs 2,3,4,5] [--dump-outputs DIR]
   torchrun --nproc-per-node N ... bench.py --gpus N ...      (one rank per GPU, NCCL)
 
 N > 1 is weak scaling: every rank owns its own images.  Images are independent units, so the timed step has NO
@@ -22,6 +22,11 @@ pinned host memory (the e2e leg moves ~100 MB per step per rank through the host
 
 Timing: W >= 3 warm-up steps; L2 is flushed (256 MiB write) before every timed step; each step is bracketed by CUDA
 events on the launching stream and the K step times are summed; barrier + synchronize on both sides; max over ranks.
+Every config's timed loop runs exactly K steps.
+
+--dump-outputs DIR (rank 0) writes what the timed steps computed in their last step, as DIR/<name>.npy (float32 / float64):
+the full roi_align output, each cfg3 image's kept indices, and a fixed seeded sample of 2^19 elements of the cfg4 and cfg5
+outputs (about 56 MB in all).  The inputs are seeded, so two builds can be compared output for output.
 `--impl reference` times the reference's own CPU kernel of the headline op (installed torchvision wheel; the oracle port
 if it is absent) on the host cores.
 """
@@ -41,21 +46,40 @@ if ROOT not in sys.path:
 
 ALG_BYTES = 55_705_600 + 20_000 + 50_176_000      # map + rois + output (SURVEY.md §8d cfg2)
 K_ROIS = 1000
-# dram__bytes_read.sum + dram__bytes_write.sum of the headline kernel, one launch of this workload (profiles/, ncu --set full)
-NCU_TRAFFIC = {"bytes": 67_071_744 + 9_524_224, "source": "profiles/r2_roi_align.ncu-rep / r2_roi_align_ncu.txt (ncu --set full, one launch; most of "
-                                                          "the 50 MB output is still dirty in L2 when the capture ends)"}
-# per-launch DRAM traffic of the dominant kernel of the other configs, same kind of capture (profiles/r2_*_ncu.txt)
-NCU_TRAFFIC_CFG = {
-    "cfg3": {"bytes": 1_622_784 + 8_721_664, "source": "profiles/r2_bnms_mask_ncu.txt + r2_bnms_scan_ncu.txt (one image)"},
-    "cfg4": {"bytes": 146_062_848 + 97_087_488, "source": "profiles/r2_deform_bf16.ncu-rep / r2_deform_bf16_ncu.txt (deform_conv2d_tc_kernel, N=32)"},
-    "cfg5": {"bytes": 6_426_276_000 + 42_117_888, "source": "profiles/r2_resize128.ncu-rep / r2_resize128_ncu.txt (resize_aa_stream_kernel, 128 images)"},
-}
 WORKLOAD = "roi_align fp32 1x256x200x272, 1000 RoIs, 7x7, scale 0.25, sampling_ratio 2, aligned=False (BASELINE configs[1])"
 CFG3_IMAGES = 4
 CFG3_BOXES = 100_000
 CFG4_FLOPS = 2 * 32 * 64 * 64 * 512 * 512 * 9          # SURVEY.md §8d cfg4: 618,475,290,624
 CFG5_BATCH = 128
 CFG5_BYTES_PER_IMAGE = 3 * 2160 * 3840 * 2 + 3 * 224 * 224 * 2
+NVLINK_BYTES_PER_S = 450e9          # H100 SXM NVLink 4, one direction
+SAMPLE_ELEMS = 1 << 19              # --dump-outputs: elements kept of a large output
+# the shared-memory gather floor of the headline op (DESIGN.md 4.1): 12.5 M bins x 16 taps x 4 B through
+# 132 SMs x 128 B/clk at the H100 SXM's 1.98 GHz maximum SM clock
+SMEM_FLOOR_US = 12_544_000 * 16 * 4 / (132 * 128 * 1.98e9) * 1e6
+
+
+def sample(t, seed: int, n: int = SAMPLE_ELEMS):
+    """A fixed, seeded sample of n elements of `t` (all of it when smaller), flattened, on the host."""
+    import torch
+
+    flat = t.detach().reshape(-1)
+    if flat.numel() > n:
+        idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(seed))[:n].sort().values
+        flat = flat[idx.to(flat.device)]
+    return flat.cpu()
+
+
+def dump_outputs(dirname: str, outputs: dict) -> None:
+    """DIR/<name>.npy per output: floating values as float32 (float64 stays float64), integer indices as float64."""
+    import numpy as np
+    import torch
+
+    os.makedirs(dirname, exist_ok=True)
+    for name, t in outputs.items():
+        t = t.detach().cpu()
+        dt = torch.float64 if t.dtype in (torch.float64, torch.int64, torch.int32) else torch.float32
+        np.save(os.path.join(dirname, f"{name}.npy"), t.to(dt).numpy())
 
 
 def _peaks_json() -> dict:
@@ -72,18 +96,19 @@ def peaks():
     d = _peaks_json()
     if "hbm_gbs" in d:
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 def tensor_peaks():
     d = _peaks_json()
     if "bf16_tflops" in d:
         return float(d["bf16_tflops"]), float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "measured (MEASURED_PEAKS.json)"
-    return 1680.0, 1460.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 989.0, "H100 SXM data sheet (dense BF16 at 700 W), not measured"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region.  start() returns once the first sample has arrived, so that
+    nvidia-smi's start-up (NVML initialisation, which can delay the driver) does not fall inside a timed step."""
 
     def __init__(self, index: int):
         self.index, self.proc, self.lines = index, None, []
@@ -97,6 +122,10 @@ class ClockSampler:
             threading.Thread(target=self._read, daemon=True).start()
         except Exception:
             self.proc = None
+            return
+        deadline = time.perf_counter() + 10.0
+        while not self.lines and self.proc.poll() is None and time.perf_counter() < deadline:
+            time.sleep(0.01)
 
     def _read(self):
         for line in self.proc.stdout:
@@ -232,6 +261,7 @@ class Ctx:
     def __init__(self, torch, dist, dev, rank, world, args):
         self.torch, self.dist, self.dev, self.rank, self.world, self.args = torch, dist, dev, rank, world, args
         self.flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
+        self.outputs = {}               # name -> what a timed path returned in its last step (--dump-outputs)
 
     def barrier(self):
         self.torch.cuda.synchronize()
@@ -334,15 +364,19 @@ def block_cfg3(ctx: Ctx, vb, tv, sharded) -> dict:
 
     imgs = [workloads.cfg3_batched_nms(seed=ctx.rank * CFG3_IMAGES + j) for j in range(CFG3_IMAGES)]
     dimgs = [tuple(t.to(ctx.dev) for t in im) for im in imgs]
-    steps = max(20, min(ctx.args.steps, 50))
-    kept = [0]
+    steps = ctx.args.steps
+    keeps = []
 
     def step():
-        kept[0] = sum(int(tv.ops.batched_nms(b, s, i, 0.5).numel()) for (b, s, i) in dimgs)
+        keeps.clear()                   # the previous step's outputs are freed before this one allocates
+        keeps.extend(tv.ops.batched_nms(b, s, i, 0.5) for (b, s, i) in dimgs)
 
     ms = ctx.device_ms(step, steps)
+    for j, k in enumerate(keeps):
+        ctx.outputs[f"cfg3_batched_nms_keep_image{j}"] = k
+    kept = sum(int(k.numel()) for k in keeps)
     boxes = ctx.world * CFG3_IMAGES * CFG3_BOXES
-    alg = CFG3_IMAGES * (CFG3_BOXES * (16 + 4 + 8)) + 8 * kept[0]
+    alg = CFG3_IMAGES * (CFG3_BOXES * (16 + 4 + 8)) + 8 * kept
     peak, src = peaks()
     cl = workloads.cfg3_batched_nms(seed=1000 + ctx.rank, clustered=True)
     cld = tuple(t.to(ctx.dev) for t in cl)
@@ -355,8 +389,7 @@ def block_cfg3(ctx: Ctx, vb, tv, sharded) -> dict:
                    "l2": "flushed before every timed step"},
         "ms_per_image": ms / CFG3_IMAGES, "clustered_ms_per_image": ms_cl,
         "roofline": {"bound": "hbm", "achieved": alg / (ms / 1e3) / 1e9, "peak": peak, "unit": "GB/s",
-                     "frac": alg / (ms / 1e3) / 1e9 / peak, "traffic": NCU_TRAFFIC_CFG["cfg3"]["bytes"] * CFG3_IMAGES,
-                     "traffic_source": NCU_TRAFFIC_CFG["cfg3"]["source"], "algorithmic_bytes": alg, "peak_source": src,
+                     "frac": alg / (ms / 1e3) / 1e9 / peak, "algorithmic_bytes": alg, "peak_source": src,
                      "note": "HBM-nominal only: 2.8 MB per image is < 1 us of HBM time; the real bound is the per-class greedy chain plus "
                              "sum n_c^2/2 = 62.5 M IoU tests per image (DESIGN.md 4.3)",
                      "iou_pairs_per_s": ctx.world * CFG3_IMAGES * 62.5e6 / (ms / 1e3)},
@@ -375,7 +408,7 @@ def block_cfg3(ctx: Ctx, vb, tv, sharded) -> dict:
         g = gpu_reference_ms(ctx, vb, lambda: tv.ops.batched_nms(*dimgs[0], 0.5), 3, 1)
         out["gpu_reference"] = {"ms_per_image": g, "value": CFG3_BOXES / (g / 1e3), "unit": "boxes/s",
                                 "ours_over_reference": g / (ms / CFG3_IMAGES),
-                                "what": "torchvision.ops.batched_nms on the wheel's sm_100 kernels (per-class Python loop + nms_kernel_impl), same boxes"}
+                                "what": "torchvision.ops.batched_nms on the wheel's CUDA kernels (per-class Python loop + nms_kernel_impl), same boxes"}
         from concurrent.futures import ThreadPoolExecutor
         torch.set_num_threads(1)
         nthr = min(len(os.sched_getaffinity(0)), 16)
@@ -393,19 +426,26 @@ def block_cfg4(ctx: Ctx, vb, tv, sharded) -> dict:
     from vision_b200 import workloads
 
     x, off, w, b, m = workloads.cfg4_deform_conv2d(device=ctx.dev, seed=ctx.rank)
-    steps = max(20, min(ctx.args.steps, 50))
+    steps = ctx.args.steps
     op = lambda: tv.ops.deform_conv2d(x, off, w, b, 1, 1, 1, m)
-    ms = ctx.device_ms(op, steps)
+    last = [None]
+
+    def step():
+        last[0] = None                  # the previous step's output is freed before this one allocates
+        last[0] = op()
+
+    ms = ctx.device_ms(step, steps)
+    ctx.outputs["cfg4_deform_conv2d_sample"] = sample(last[0], seed=4)
+    last[0] = None
     tf = CFG4_FLOPS / (ms / 1e3) / 1e12
     burst, sustained, src = tensor_peaks()
     out = {
         "metric": "deform_conv2d TFLOP/s", "value": ctx.world * tf, "unit": "TFLOP/s", "ms_per_step": ms, "steps": steps, "dtype": "bf16",
         "config": {"workload": "deform_conv2d 3x3 DCNv2, N=32 C=512->512 64x64, stride 1 pad 1, bf16 in / fp32 accumulate (BASELINE configs[3])",
                    "api": "torchvision.ops.deform_conv2d after vision_b200.install()", "l2": "flushed before every timed step",
-                   "includes": "NCHW->NHWC staging of the input and weight packing (re-done every call) + the tcgen05 kernel"},
+                   "includes": "NCHW->NHWC staging of the input and weight packing (re-done every call) + the wgmma kernel"},
         "roofline": {"bound": "tensor", "achieved": tf, "peak": burst, "unit": "TFLOP/s", "frac": tf / burst,
-                     "frac_of_sustained": tf / sustained, "peak_sustained": sustained, "traffic": NCU_TRAFFIC_CFG["cfg4"]["bytes"],
-                     "traffic_source": NCU_TRAFFIC_CFG["cfg4"]["source"], "tensor_pipe_active_pct_ncu": 52.7,
+                     "frac_of_sustained": tf / sustained, "peak_sustained": sustained,
                      "algorithmic_flops": CFG4_FLOPS, "peak_source": src + " (burst: the op is timed alone between L2 flushes)"},
     }
     hx, hoff, hw_, hb, hm = [t.cpu() for t in (x, off, w, b, m)]
@@ -432,10 +472,10 @@ def block_cfg4(ctx: Ctx, vb, tv, sharded) -> dict:
                 out["with_allgather"] = {
                     "ms_per_step": fms, "value": ctx.world * CFG4_FLOPS / (fms / 1e3) / 1e12, "unit": "TFLOP/s",
                     "bytes_gathered_per_rank": ctx.world * x.numel() * 2, "identical_to_nccl_gather": True,
-                    "nvlink_ingress_floor_ms": ingress / 900e9 * 1e3,
-                    "note": "all-gather fused into the tcgen05 kernel's epilogue: each output element is stored to every rank's gathered buffer "
-                            "(torch symmetric memory, NVLink peer stores of 256-byte runs), one device-side barrier per step (double-buffered); "
-                            "no NCCL call.  nvlink_ingress_floor_ms = (world-1) x 134 MB received per rank per step at 900 GB/s",
+                    "nvlink_ingress_floor_ms": ingress / NVLINK_BYTES_PER_S * 1e3,
+                    "note": "all-gather fused into the wgmma kernel's epilogue: each output element is stored to every rank's gathered buffer "
+                            "(torch symmetric memory, NVLink peer stores of 16-byte runs), one device-side barrier per step (double-buffered); "
+                            "no NCCL call.  nvlink_ingress_floor_ms = (world-1) x 134 MB received per rank per step at 450 GB/s",
                     "nccl_overlapped": nccl}
             else:
                 nccl["fused_peer_stores"] = {"ms_per_step": fms, "identical_to_nccl_gather": False}
@@ -457,7 +497,7 @@ def block_cfg4(ctx: Ctx, vb, tv, sharded) -> dict:
         del xh, oh, wh, bh, mh
         out["gpu_reference"] = {"fp32_ms": g32, "fp16_ms": g16, "value": CFG4_FLOPS / (g16 / 1e3) / 1e12, "unit": "TFLOP/s",
                                 "ours_over_reference": g16 / ms, "ours_over_reference_fp32": g32 / ms,
-                                "what": "torchvision.ops.deform_conv2d on the wheel's sm_100 kernels (im2col + cuBLAS), same values; the reference "
+                                "what": "torchvision.ops.deform_conv2d on the wheel's CUDA kernels (im2col + cuBLAS), same values; the reference "
                                         "has no bf16 kernel, so its fastest 16-bit option (fp16, inputs pre-cast) and its fp32 default are both timed"}
         torch.set_num_threads(len(os.sched_getaffinity(0)))
         cx, coff, cw, cb, cm = [t[:2].float().cpu() if t.dim() == 4 and t.shape[0] == 32 else t.float().cpu() for t in (x, off, w, b, m)]
@@ -473,8 +513,16 @@ def block_cfg5(ctx: Ctx, vb, tv, sharded) -> dict:
     from vision_b200 import workloads
 
     x = workloads.cfg5_resize(device=ctx.dev, batch=CFG5_BATCH, seed=ctx.rank)
-    steps = max(20, min(ctx.args.steps, 50))
-    ms = ctx.device_ms(lambda: TF.resize(x, [224, 224]), steps)
+    steps = ctx.args.steps
+    last = [None]
+
+    def step():
+        last[0] = None
+        last[0] = TF.resize(x, [224, 224])
+
+    ms = ctx.device_ms(step, steps)
+    ctx.outputs["cfg5_resize_sample"] = sample(last[0], seed=5)
+    last[0] = None
     nbytes = CFG5_BATCH * CFG5_BYTES_PER_IMAGE
     peak, src = peaks()
     out = {
@@ -484,8 +532,7 @@ def block_cfg5(ctx: Ctx, vb, tv, sharded) -> dict:
                                f"configs[4] at 8 GPUs; 1024 images = 8 such shards)",
                    "api": "torchvision.transforms.v2.functional.resize after vision_b200.install()", "l2": "input (6.4 GB) exceeds L2; flushed anyway"},
         "roofline": {"bound": "hbm", "achieved": nbytes / (ms / 1e3) / 1e9, "peak": peak, "unit": "GB/s",
-                     "frac": nbytes / (ms / 1e3) / 1e9 / peak, "traffic": NCU_TRAFFIC_CFG["cfg5"]["bytes"],
-                     "traffic_source": NCU_TRAFFIC_CFG["cfg5"]["source"], "algorithmic_bytes": nbytes, "peak_source": src},
+                     "frac": nbytes / (ms / 1e3) / 1e9 / peak, "algorithmic_bytes": nbytes, "peak_source": src},
     }
     sub = 32
     hx = x[:sub].cpu()
@@ -553,6 +600,8 @@ def main():
     ap.add_argument("--no-secondary", action="store_true", help="headline (cfg2) only")
     ap.add_argument("--configs", default="2,3,4,5", help="which BASELINE configs to measure (2 is always measured)")
     ap.add_argument("--cpu-calls", type=int, default=10, help="CPU-baseline sample size (full-size calls)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of every timed path's last step as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -590,24 +639,29 @@ def main():
     def step():
         return torchvision.ops.roi_align(xd, rd, **kw)
 
+    sampler = ClockSampler(local_rank)
+    if rank == 0:
+        sampler.start()                     # before the warm-up: its start-up must not overlap the timed steps
     for _ in range(args.warmup):
         flush.zero_()
         step()
     ctx.barrier()
 
-    sampler = ClockSampler(local_rank)
-    if rank == 0:
-        sampler.start()
     starts = [torch.cuda.Event(enable_timing=True) for _ in range(args.steps)]
     ends = [torch.cuda.Event(enable_timing=True) for _ in range(args.steps)]
     launches0 = vb.launch_count()
     wall0 = time.perf_counter()
+    last = None
     for i in range(args.steps):
+        last = None                         # free the previous output first: no step may allocate a new buffer
         flush.zero_()                       # L2 flush between timed iterations (not timed)
         starts[i].record(stream)
-        step()
+        last = step()
         ends[i].record(stream)
     ctx.barrier()
+    if last is not None:
+        ctx.outputs["roi_align"] = last
+    del last
     wall = time.perf_counter() - wall0
     launches = vb.launch_count() - launches0
     ms_per_step = ctx.max_over_ranks(sum(s.elapsed_time(e) for s, e in zip(starts, ends))) / args.steps
@@ -655,7 +709,7 @@ def main():
                     fused[name] = {"error": repr(ex)[:200]}
             ok = {k_: v for k_, v in fused.items() if v.get("identical_to_nccl_gather")}
             ingress = (world - 1) * K_ROIS * 256 * 49 * 4
-            gather["nvlink_ingress_floor_ms"] = ingress / 900e9 * 1e3
+            gather["nvlink_ingress_floor_ms"] = ingress / NVLINK_BYTES_PER_S * 1e3
             gather["fused_variants"] = fused
             gather["transport"] = "nccl"
             if ok:
@@ -665,7 +719,7 @@ def main():
             gather["note"] += (".  fused_variants: the exchange done by the roi_align kernel's own stores into every rank's gathered buffer (torch symmetric "
                                "memory; multicast = one multimem.st replicated by the NVSwitch, peer_stores = one NVLink store per rank; 28-byte runs, "
                                "so the links carry partial sectors), one device-side barrier per step; ms_per_step / value = the fastest "
-                               "transport.  Every rank RECEIVES (world-1) x 50 MB per step: nvlink_ingress_floor_ms is that volume at 900 GB/s, the "
+                               "transport.  Every rank RECEIVES (world-1) x 50 MB per step: nvlink_ingress_floor_ms is that volume at 450 GB/s, the "
                                "bound of this exchange whatever the transport")
             del ref
         else:
@@ -693,14 +747,12 @@ def main():
         if world == 1:
             g = gpu_reference_ms(ctx, vb, lambda: torchvision.ops.roi_align(xd, rd, **kw), 10)
             gpu_ref = {"ms_per_step": g, "value": K_ROIS / (g / 1e3), "unit": "RoIs/s", "ours_over_reference": g / ms_per_step,
-                       "what": "torchvision.ops.roi_align on the wheel's sm_100 kernel (roi_align_forward_kernel_impl), same inputs, L2 flushed"}
+                       "what": "torchvision.ops.roi_align on the wheel's CUDA kernel (roi_align_forward_kernel_impl), same inputs, L2 flushed"}
             torch.set_num_threads(1)      # the pool supplies the parallelism
             fn, kind, desc, threads = cpu_reference_fn()
             sec = time_cpu(fn, args.cpu_calls)
             cpu = {"value": K_ROIS / sec, "unit": "RoIs/s", "cores": threads, "host_cores": os.cpu_count(), "kind": kind,
                    "sample": f"{args.cpu_calls} full-size calls ({sec * 1e3:.0f} ms each); {desc}"}
-        # the shared-memory gather floor of the op (DESIGN.md 4.1): 12.5 M bins x 16 taps x 4 B through 148 SMs x 128 B/clk
-        smem_floor_us = 12_544_000 * 16 * 4 / (148 * 128 * 1.965e9) * 1e6
         line = {
             "metric": "roi_align RoIs/s", "value": world * K_ROIS / (ms_per_step / 1e3), "unit": "RoIs/s", "n_gpus": world,
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True,
@@ -709,11 +761,10 @@ def main():
                        "parallelism": f"dp{world}: one image per rank, no data-path collective in the timed step",
                        "api": "torchvision.ops.roi_align after vision_b200.install()", "numa": numa},
             "roofline": {
-                "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": NCU_TRAFFIC["bytes"],
-                "traffic_source": NCU_TRAFFIC["source"],
+                "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                 "kernel": "roi_align_line_kernel<7, 2> (+ roi_align_line_geometry_kernel inside the same event pair)",
                 "algorithmic_bytes": ALG_BYTES, "peak_source": peak_src,
-                "smem_gather_floor_us": smem_floor_us, "frac_of_smem_gather_floor": smem_floor_us / (ms_per_step * 1e3),
+                "smem_gather_floor_us": SMEM_FLOOR_US, "frac_of_smem_gather_floor": SMEM_FLOOR_US / (ms_per_step * 1e3),
                 "note": "the op is a shared-memory gather (200 M tap reads): its conflict-free floor is above the HBM time (DESIGN.md 4.1)"},
             "cpu_baseline": cpu, "gpu_reference": gpu_ref,
             "e2e": {"value": world * K_ROIS / (e2e_ms / 1e3), "unit": "RoIs/s", "ms_per_step": e2e_ms,
@@ -725,6 +776,8 @@ def main():
             line["with_allgather"] = gather
         if configs:
             line["configs"] = configs
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, ctx.outputs)
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.barrier()

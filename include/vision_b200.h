@@ -1,5 +1,5 @@
 /*
- * vision_b200.h — C ABI of libvision_b200.so (sm_100a CUDA kernels for the
+ * vision_b200.h — C ABI of libvision_b200.so (sm_90a CUDA kernels for the
  * torchvision custom-op hot path).  No torch types cross this boundary: plain
  * device pointers, sizes and a CUDA stream handle.  Every entry point names
  * the reference interface it replaces (paths relative to pytorch/vision).
@@ -230,7 +230,7 @@ VB200_API int vb200_detection_postprocess(const void* boxes, const void* scores,
  * offset [batch, offset_groups*2*kh*kw, out_h, out_w],
  * mask [batch, offset_groups*kh*kw, out_h, out_w] (ignored if !use_mask),
  * bias [c_out] (may be NULL), out [batch,c_out,out_h,out_w].
- * dtype: BF16 / F16 (tcgen05 tensor-core path, fp32 accumulate), F32 (tcgen05 with a three-way bf16 split of both
+ * dtype: BF16 / F16 (wgmma tensor-core path, fp32 accumulate), F32 (wgmma with a three-way bf16 split of both
  * operands, six MMAs per K step: fp32-level accuracy; SIMT kernel for shapes the tensor-core tiling does not cover),
  * F64 (plain double kernel - the reference's gradcheck tests run in double).
  * workspace: vb200_deform_conv2d_workspace_bytes() bytes (may be 0). */
@@ -260,7 +260,7 @@ VB200_API int vb200_deform_conv2d_forward_ex(const void* input, const void* weig
                                    void* workspace, size_t workspace_bytes, vb200_stream stream);
 /* deform_conv2d fused with the all-gather of its output over the GPUs of one box (SURVEY.md 8e: the batch shards, one
  * all-gather of the per-shard outputs): outs[0] is the caller's slot of its own gathered buffer, outs[1..n_outs) the SAME slot
- * of every peer's buffer (peer-mapped device pointers); the tcgen05 kernel's epilogue stores each output element to all of
+ * of every peer's buffer (peer-mapped device pointers); the wgmma kernel's epilogue stores each output element to all of
  * them.  Other arguments as vb200_deform_conv2d_forward_ex.  The caller synchronises the ranks before anyone reads. */
 VB200_API int vb200_deform_conv2d_forward_gather(const void* input, const void* weight, const void* packed_weight, int input_is_nhwc,
                                        const void* offset, const void* mask, const void* bias, void* const* outs, int n_outs,

@@ -64,7 +64,7 @@ ORC_API void orc_argsort_desc_stable_f32(const float* key, int64_t n, int64_t* o
 /* mode 0 ("cpu"):  areas rounded separately, den = (iarea + area_j) - inter,*/
 /*                  compare (double)ovr > iou_threshold(double).            */
 /* mode 1 ("cuda"): what nvcc makes of devIoU<float> in the reference build  */
-/*                  (SURVEY.md §2.2, SASS of the installed sm_100 cubin):   */
+/*                  (SURVEY.md §2.2, SASS of the installed wheel's cubin):  */
 /*                  Sa = fmul(a2-a0, a3-a1); t = fma(b2-b0, b3-b1, Sa);      */
 /*                  den = t - inter; compare ovr > (float)iou_threshold.    */
 /* mode 2 ("cuda half"): what nvcc makes of devIoU<Half> (SASS of the same   */
@@ -235,7 +235,7 @@ ORC_API void orc_argsort_desc_stable_f64(const double* key, int64_t n, int64_t* 
 /* mode 0 ("cpu"):  areas rounded separately, den = (iarea + area_j) - inter,*/
 /*                  compare (double)ovr > iou_threshold(double).            */
 /* mode 1 ("cuda"): what nvcc makes of devIoU<float> in the reference build  */
-/*                  (SURVEY.md §2.2, SASS of the installed sm_100 cubin):   */
+/*                  (SURVEY.md §2.2, SASS of the installed wheel's cubin):  */
 /*                  Sa = fmul(a2-a0, a3-a1); t = fma(b2-b0, b3-b1, Sa);      */
 /*                  den = t - inter; compare ovr > (float)iou_threshold.    */
 /* Returns the number kept; keep[] holds original indices in descending-    */

@@ -10,13 +10,17 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")
 def golden():
-    path = os.path.join(ROOT, "tests", "golden", "reference_cpu.npz")
-    return np.load(path)
+    # one fixture set stored in two files (each under 1 MB)
+    out = {}
+    for name in ("reference_cpu.npz", "reference_cpu_resize.npz"):
+        with np.load(os.path.join(ROOT, "tests", "golden", name)) as z:
+            out.update({k: z[k] for k in z.files})
+    return out
 
 
 @pytest.fixture(scope="session")

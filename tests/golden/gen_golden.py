@@ -3,7 +3,7 @@ kernels (torch.ops.torchvision.*, CPU dispatch key) and ATen's CPU interpolate, 
 build container (torchvision 0.26.0+cu128 / torch 2.11.0 wheel = release build of the kernels
 under /root/reference/torchvision/csrc/ops/cpu).  The fixtures pin oracle/ and the CUDA kernels.
 
-    python tests/golden/gen_golden.py        # rewrites the .npz files next to this script
+    python tests/golden/gen_golden.py        # rewrites reference_cpu.npz and reference_cpu_resize.npz next to this script
 """
 import os
 
@@ -106,8 +106,11 @@ def main():
                 out[f"rs_{mode}_aa{aa}_{size[0]}x{size[1]}"] = F.interpolate(
                     img, size=list(size), mode=mode, align_corners=False, antialias=bool(aa)).numpy()
     out["versions"] = np.array([torch.__version__, torchvision.__version__])
-    np.savez_compressed(os.path.join(HERE, "reference_cpu.npz"), **out)
-    print("wrote", os.path.join(HERE, "reference_cpu.npz"), len(out), "arrays")
+    # the resize arrays go to a file of their own, so that no fixture file exceeds 1 MB (tests/conftest.py merges the two)
+    for name, keep in (("reference_cpu.npz", lambda k: not k.startswith("rs_")), ("reference_cpu_resize.npz", lambda k: k.startswith("rs_"))):
+        part = {k: v for k, v in out.items() if keep(k)}
+        np.savez_compressed(os.path.join(HERE, name), **part)
+        print("wrote", os.path.join(HERE, name), len(part), "arrays")
 
 
 if __name__ == "__main__":

@@ -507,7 +507,7 @@ def test_deform_conv2d_cfg4_reduced_vs_oracle(vb, oracle, dtype, tol):
 
     x, off, w, b, m = workloads.cfg4_deform_conv2d(batch=2, c_in=64, c_out=128, hw=32, dtype=dtype)
     if dtype != torch.float32:
-        # one accumulator (BN 128/256, 3 stages) and two accumulators (BN 512, 2 stages) of the tcgen05 kernel
+        # one CTA per 256 output channels, and two CTAs along the output channels, of the wgmma kernel
         for c_out, hw in ((256, 16), (512, 12)):
             x2, off2, w2, b2, m2 = workloads.cfg4_deform_conv2d(seed=c_out, batch=1, c_in=128, c_out=c_out, hw=hw, dtype=dtype)
             want2 = oracle.deform_conv2d(x2.float().numpy(), off2.float().numpy(), w2.float().numpy(), b2.float().numpy(),
@@ -518,23 +518,6 @@ def test_deform_conv2d_cfg4_reduced_vs_oracle(vb, oracle, dtype, tol):
                                 m.float().numpy())
     got = vb.ops.deform_conv2d(x.to(DEV), off.to(DEV), w.to(DEV), b.to(DEV), 1, 1, 1, m.to(DEV))
     np.testing.assert_allclose(npy(got), want, rtol=tol, atol=tol)
-
-
-def test_deform_conv2d_cta_pair_variant_matches(vb, oracle):
-    """The cta_group::2 (CTA-pair, M = 256) tcgen05 kernel, enabled by VB200_DCN_CTA2=1: same bits as the
-    single-CTA kernel, incl. an odd tile count (padded cluster) and ragged pixel tiles; oracle parity."""
-    from vision_b200 import workloads
-
-    for batch, cin, cout, hw in ((1, 64, 512, 12), (3, 128, 512, 20)):
-        x, off, w, b, m = workloads.cfg4_deform_conv2d(seed=hw, batch=batch, c_in=cin, c_out=cout, hw=hw, dtype=torch.bfloat16)
-        args = (x.to(DEV), off.to(DEV), w.to(DEV), b.to(DEV), 1, 1, 1, m.to(DEV))
-        one = vb.ops.deform_conv2d(*args)
-        with force_env("VB200_DCN_CTA2", "1"):
-            two = vb.ops.deform_conv2d(*args)
-        assert torch.equal(one, two)
-        want = oracle.deform_conv2d(x.float().numpy(), off.float().numpy(), w.float().numpy(), b.float().numpy(), (1, 1), (1, 1), (1, 1),
-                                    m.float().numpy())
-        np.testing.assert_allclose(npy(two), want, rtol=1e-2, atol=1e-2)
 
 
 @pytest.mark.parametrize("dtype,tol", [(torch.float32, 1e-5), (torch.bfloat16, 1e-2)])
@@ -657,7 +640,7 @@ def test_dropin_through_torchvision_api(vb, oracle):
 
     x, rois, kw = workloads.cfg2_roi_align(channels=32, k=100)
     xd, rd = x.to(DEV), rois.to(DEV)
-    ref_cuda = tv.ops.roi_align(xd, rd, **kw)                                   # reference CUDA kernel (sm_100 SASS)
+    ref_cuda = tv.ops.roi_align(xd, rd, **kw)                                   # reference CUDA kernel (the wheel's SASS)
     vb.install()
     try:
         before = vb.launch_count()
@@ -695,7 +678,7 @@ def test_dropin_through_torchvision_api(vb, oracle):
 
 
 def test_against_reference_cuda_kernels_same_box(vb):
-    """Extra: our kernels vs the reference's own CUDA kernels (wheel, sm_100 SASS) on this GPU."""
+    """Extra: our kernels vs the reference's own CUDA kernels (the wheel's SASS) on this GPU."""
     tv = pytest.importorskip("torchvision")
     from vision_b200 import workloads
 

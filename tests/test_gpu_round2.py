@@ -1,4 +1,4 @@
-"""GPU parity tests added in round 2 (run on the B200 box: `pytest -m gpu`).
+"""GPU parity tests added in round 2 (run on an H100: `pytest -m gpu`).
 
 * fp16 nms / batched_nms: bit-exact against the reference's own CUDA kernel (devIoU<Half>,
   csrc/ops/cuda/nms_kernel.cu:42-54; the in-half coordinate trick, ops/boxes.py:92-109) and the oracle's half mode;
@@ -109,7 +109,7 @@ def test_nms_score_order_edge_cases_vs_reference_cuda(vb, dtype):
 
 @pytest.mark.parametrize("variant", ["mask", "nomask", "zero_offset"])
 def test_deform_conv2d_cfg4_full_size_vs_reference_cuda(vb, oracle, variant):
-    """BASELINE configs[3] at FULL size through the tcgen05 kernel the bench times (BN=512, 4 stages, two gather groups):
+    """BASELINE configs[3] at FULL size through the wgmma kernel the bench times (BN=256, 3 stages, two consumer warpgroups):
     N=32, 512->512, 64x64, 3x3, bf16.  Reference = torchvision's CUDA deform_conv2d in fp32 on the bf16-rounded values
     (the reference has no bf16 kernel on any backend), tolerance 1e-2 (north_star).  One image is also checked
     against the CPU oracle."""
@@ -748,7 +748,7 @@ def test_roi_align_gather_writes_every_destination(vb):
 
 @pytest.mark.gpu
 def test_deform_conv2d_gather_writes_every_destination(vb):
-    """vision_b200::deform_conv2d_gather: the tcgen05 epilogue stores each output element to all destinations (peer slots on a
+    """vision_b200::deform_conv2d_gather: the wgmma epilogue stores each output element to all destinations (peer slots on a
     multi-GPU box; three local buffers here); shapes on the SIMT kernel are computed once and copied."""
     from vision_b200 import workloads
 

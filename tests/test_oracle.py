@@ -267,9 +267,11 @@ def test_box_iou_rotated_golden_and_ref(oracle):
     rng = np.random.default_rng(7)
     c = rng.uniform(0, 100, (150, 2)); wh = np.exp(rng.uniform(0, 4, (150, 2))); a = rng.uniform(-360, 360, (150, 1))
     b = np.concatenate([c, wh, a], 1).astype(np.float32)
+    assert np.array_equal(b, g["rev_boxes"])
+    assert np.array_equal(oracle.box_iou_rotated(b, b[::-1].copy()), g["rev_ious"])   # the reference's own result, stored
     ref = oracle.box_iou_rotated_ref(b, b[::-1].copy())
-    if ref is not None:                                     # build container: the reference's own code, live
-        assert np.array_equal(oracle.box_iou_rotated(b, b[::-1].copy()), ref)
+    if ref is not None:                                     # oracle/_ref built: the reference's own code, live
+        assert np.array_equal(ref, g["rev_ious"])
     iou = oracle.box_iou_rotated(b, b)
     assert np.allclose(np.diag(iou), 1.0, atol=1e-5) and np.all(iou >= 0) and np.all(iou <= 1)
     np.testing.assert_allclose(iou, iou.T, atol=2e-5)       # symmetric up to the order of operations

@@ -1,4 +1,4 @@
-"""A/B of the tcgen05 deform_conv2d corner blend: fp32 FFMA2 (default) vs the packed 16-bit HFMA2 blend (VB200_DCN_BLEND=16).
+"""A/B of the tensor-core deform_conv2d corner blend: fp32 FMA (default) vs the packed 16-bit HFMA2 blend (VB200_DCN_BLEND=16).
 Prints, per dtype and blend, the device time of BASELINE configs[3] and the worst |err| / (1e-2 + 1e-2 |ref|) against
 torchvision's CUDA fp32 kernel on the same 16-bit-rounded values.   python tools/dcn_blend_ab.py"""
 import os

@@ -1,5 +1,5 @@
 """Round-2 diagnostics (GPU): (1) headroom of the 16-bit deform_conv2d tests at 1e-2, (2) timings of the reference's own
-sm_100 CUDA kernels (the wheel) next to ours on the five BASELINE configs.  Prints plain lines; not a test."""
+CUDA kernels (the wheel) next to ours on the five BASELINE configs.  Prints plain lines; not a test."""
 import os
 import sys
 

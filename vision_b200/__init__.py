@@ -1,4 +1,4 @@
-"""vision_b200 — Blackwell-native (sm_100a) kernels behind torchvision's custom-op hot path.
+"""vision_b200 — Hopper-native (sm_90a) kernels behind torchvision's custom-op hot path.
 
     import torchvision, vision_b200
     vision_b200.install()        # torchvision.ops.{nms, roi_align, roi_pool, ps_roi_align, deform_conv2d}

@@ -23,7 +23,7 @@ class ExtensionMissing(RuntimeError):
 def _missing(path: str) -> ExtensionMissing:
     return ExtensionMissing(
         f"vision_b200 native library not found: {path}. Build it in-tree with "
-        f"`python -m vision_b200.build` (needs nvcc, -gencode arch=compute_100a,code=sm_100a). "
+        f"`python -m vision_b200.build` (needs nvcc, -gencode arch=compute_90a,code=sm_90a). "
         f"There is deliberately no CPU fallback."
     )
 

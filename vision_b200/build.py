@@ -1,6 +1,6 @@
 """In-tree build of the two shared libraries (no JIT cache: the .so files travel with the repo).
 
-  vision_b200/lib/libvision_b200.so    C-ABI CUDA kernels, nvcc -gencode arch=compute_100a,code=sm_100a
+  vision_b200/lib/libvision_b200.so    C-ABI CUDA kernels, nvcc -gencode arch=compute_90a,code=sm_90a
   vision_b200/lib/libvision_b200_torch.so   torch dispatcher shim (g++, links the above)
 
 `python -m vision_b200.build [--force]`
@@ -24,7 +24,7 @@ CU_SOURCES = ["runtime.cu", "box_iou_rotated.cu", "roi_ops.cu", "roi_backward.cu
 CORE_LIB = os.path.join(LIBDIR, "libvision_b200.so")
 SHIM_LIB = os.path.join(LIBDIR, "libvision_b200_torch.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr", "-Wno-deprecated-declarations",
               "-I", INCLUDE]
 
@@ -70,7 +70,7 @@ def build_core(force: bool = False, verbose: bool = False) -> str:
     if force or not _newer(CORE_LIB, objs):
         # default (static) cudart: the library carries its own runtime and attaches to the
         # primary context torch already created; streams are plain CUstream handles.
-        cmd = [nvcc, "-shared", "-o", CORE_LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [nvcc, "-shared", "-o", CORE_LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         if verbose:
             print(" ".join(cmd), flush=True)
         subprocess.check_call(cmd)

@@ -1,4 +1,4 @@
-// box_iou_rotated.cu — IoU of rotated boxes (x_ctr, y_ctr, w, h, angle in degrees), all pairs, for sm_100a.
+// box_iou_rotated.cu — IoU of rotated boxes (x_ctr, y_ctr, w, h, angle in degrees), all pairs, for sm_90a.
 //
 // Reference: csrc/ops/cuda/box_iou_rotated_kernel.cu:42-90 driving csrc/ops/box_iou_rotated_utils.h:67-383 (per pair: all
 // 16 edge/edge intersections + contained vertices -> up to 24 points -> Graham scan with an O(n^2) sort -> fan area; the

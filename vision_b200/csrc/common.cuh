@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for the sm_100a kernels behind include/vision_b200.h.
+// common.cuh — shared helpers for the sm_90a kernels behind include/vision_b200.h.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -12,8 +12,6 @@
 #include "../../include/vision_b200.h"
 
 namespace vb200 {
-
-constexpr int kNumSMsB200 = 148;
 
 // ---- error plumbing -------------------------------------------------------
 char* last_error_buf();
@@ -54,7 +52,7 @@ int max_smem_optin();
 // VB200_* path overrides (testing / profiling): read from the environment ONCE when the library first needs them
 // (no getenv on the per-call path); vb200_reload_env() re-reads them.  nullptr when unset.
 enum EnvKey { ENV_ROI_ALIGN_PATH, ENV_ROI_LINE_AXIS, ENV_NMS_PATH, ENV_BNMS_PATH, ENV_BNMS_WARPS, ENV_RESIZE_PATH, ENV_DCN_PATH,
-              ENV_DCN_CTA2, ENV_DCN_STAGES, ENV_DCN_BN, ENV_ROI_BWD_PATH, ENV_BNMS_GRAPH, ENV_DCN_BLEND, ENV_ROI_BAND_OVH, ENV_COUNT };
+              ENV_DCN_BN, ENV_ROI_BWD_PATH, ENV_BNMS_GRAPH, ENV_DCN_BLEND, ENV_ROI_BAND_OVH, ENV_COUNT };
 const char* env_override(EnvKey k);
 int env_generation();     // bumped by every (re)load of the overrides: caches keyed on it forget their entries
 
@@ -97,16 +95,14 @@ __device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(
 __device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
 __device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
 
-// packed fp32 pairs for FFMA2 (fma.rn.f32x2, new on sm_100): two FMAs per issue slot
+// fp32 pairs carried in one 64-bit value; fma2 is two round-to-nearest FMAs, one per element
 __device__ __forceinline__ unsigned long long pack2(float x, float y) {
   return (unsigned long long)__float_as_uint(x) | ((unsigned long long)__float_as_uint(y) << 32);
 }
 __device__ __forceinline__ float lo32(unsigned long long v) { return __uint_as_float((uint32_t)v); }
 __device__ __forceinline__ float hi32(unsigned long long v) { return __uint_as_float((uint32_t)(v >> 32)); }
 __device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  return pack2(__fmaf_rn(lo32(a), lo32(b), lo32(c)), __fmaf_rn(hi32(a), hi32(b), hi32(c)));
 }
 
 __host__ __device__ inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }

@@ -1,4 +1,4 @@
-// deform_conv2d.cu — deformable convolution forward (DCNv1/v2), sm_100a.
+// deform_conv2d.cu — deformable convolution forward (DCNv1/v2), sm_90a.
 //
 // Reference: csrc/ops/cuda/deform_conv2d_kernel.cu:97-209 (bilinear + deformable_im2col),
 // :1035-1255 (host: materialised `columns` buffer + per-group cuBLAS addmm + transpose/copy/bias);
@@ -14,8 +14,8 @@
 //     col element costs 4 loads + 4 FMAs.  K is walked in slabs of 16; A (weights) and
 //     B (sampled columns) slabs live in shared memory, each thread accumulates an 8x4
 //     register tile.  Bias is fused into the epilogue; output is written once, NCHW.
-//   * tcgen05 kernel (deform_conv2d_tc.cu): same decomposition with the B slab written
-//     as a swizzled bf16 K-major tile and the contraction on the 5th-gen tensor cores.
+//   * wgmma kernel (deform_conv2d_tc.cu): same decomposition with the B slab written
+//     as a swizzled bf16 K-major tile and the contraction on the Hopper tensor cores.
 #include "common.cuh"
 #include "dcn_params.h"
 
@@ -285,7 +285,7 @@ extern "C" int vb200_deform_conv2d_forward_ex(const void* input, const void* wei
 }
 
 // deform_conv2d fused with the all-gather of its output: outs[0] is the caller's slot of its own gathered buffer, outs[1..n) the
-// same slot of the peers' buffers (peer-mapped).  The tcgen05 kernel's epilogue stores each element to all of them; shapes that
+// same slot of the peers' buffers (peer-mapped).  The wgmma kernel's epilogue stores each element to all of them; shapes that
 // take another kernel are computed into outs[0] and copied to the peers on the same stream.
 extern "C" int vb200_deform_conv2d_forward_gather(const void* input, const void* weight, const void* packed_weight, int input_is_nhwc,
                                                   const void* offset, const void* mask, const void* bias, void* const* outs, int n_outs,

@@ -1,4 +1,4 @@
-// deform_conv2d_bwd.cu — backward of deform_conv2d for sm_100a (SURVEY.md §8f1).
+// deform_conv2d_bwd.cu — backward of deform_conv2d for sm_90a (SURVEY.md §8f1).
 //
 // Reference: csrc/ops/cuda/deform_conv2d_kernel.cu:319-1033 — backward_gradient_inputs (GEMM weight^T x grad_out into a
 // columns buffer, then deformable_col2im_coord_kernel for grad_offset / grad_mask and deformable_col2im_kernel for

@@ -1,4 +1,4 @@
-// resize.cu — bilinear / bicubic resize (antialias on/off) with fused dtype casts, sm_100a.
+// resize.cu — bilinear / bicubic resize (antialias on/off) with fused dtype casts, sm_90a.
 //
 // Replaces the interpolate leg of torchvision.transforms.v2.functional.resize_image
 // (torchvision/transforms/v2/functional/_geometry.py:340-360): the reference casts

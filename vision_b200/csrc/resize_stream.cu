@@ -202,8 +202,7 @@ resize_aa_stream_kernel(const T* __restrict__ in, StreamParams p, int n_cwarps) 
   constexpr int PPW = Px<T>::PPW;
   constexpr int ALIGN = PPW > 2 ? PPW : 2;        // the slot starts on a 32-bit word AND on a pixel pair
   const int e = lo & ~(ALIGN - 1);
-  // weights kept as packed fp32 pairs: the inner loop is FFMA2 (fma.rn.f32x2, sm_100) — one issue slot
-  // for two pixels
+  // weights kept as fp32 pairs: each step of the inner loop is two FMAs, one per pixel
   unsigned long long wA2[NP], wB2[NP];
 #pragma unroll
   for (int t = 0; t < NP; ++t) {

@@ -1,4 +1,4 @@
-// roi_backward.cu — deterministic backward kernels of roi_align / roi_pool / ps_roi_align for sm_100a.
+// roi_backward.cu — deterministic backward kernels of roi_align / roi_pool / ps_roi_align for sm_90a.
 //
 // Reference semantics (pytorch/vision; all three scatter with fastAtomicAdd into a zeroed grad_input and call
 // alertNotDeterministic):
@@ -307,8 +307,8 @@ roi_align_bwd_plane_fast_kernel(const float* __restrict__ grad, const BwdHdr* __
 
 // Non-deterministic sibling of the two kernels above (the default unless the caller asks for determinism): the plane is
 // still resident, but RoIs are dealt to the warps round-robin and every tap is a shared-memory atomic add, so no work is
-// repeated per band (the ownership scheme pays ~10 band hits per RoI).  fp32 shared atomics are a CAS loop on sm_100
-// (ATOMS.CAST.SPIN), cheap while contention is low - a warp's 28 taps of one line hit distinct columns.  The result differs
+// repeated per band (the ownership scheme pays ~10 band hits per RoI).  The shared-memory atomics are cheap while contention
+// is low - a warp's 28 taps of one line hit distinct columns.  The result differs
 // from run to run only in the summation order, as the reference's own atomic kernel does.
 __global__ void __launch_bounds__(kBwdThreads, 1)
 roi_align_bwd_plane_atomic_kernel(const float* __restrict__ grad, const BwdHdr* __restrict__ hdr, const uint2* __restrict__ ys,

@@ -1,4 +1,4 @@
-// roi_ops.cu — roi_align / roi_pool / ps_roi_align forward for sm_100a.
+// roi_ops.cu — roi_align / roi_pool / ps_roi_align forward for sm_90a.
 //
 // Reference semantics (pytorch/vision):
 //   roi_align     csrc/ops/cuda/roi_align_kernel.cu:14-143   (CPU: cpu/roi_align_kernel.cpp:18-115,
@@ -1365,8 +1365,8 @@ int roi_align_path(int dtype, const void* input, int batch, int channels, int he
   const bool line_ok = shape7 && line_bytes + 1024 <= (size_t)max_smem_optin();
   const bool band_ok = shape7 && band_config(batch, channels, height, width, num_rois).ok;
   const int64_t pairs = (int64_t)batch * channels * num_rois;
-  // measured on cfg2 (profiles/roi_align_r2.md): line 101 us, band 131 us - the band kernel is conflict-free but spends more
-  // instructions per output (per-bin-row folds, item prologues, transposing tile loads), so it is opt-in only
+  // the band kernel is conflict-free but spends more instructions per output (per-bin-row folds, item prologues, transposing
+  // tile loads) and measured slower than the line kernel on cfg2, so it is opt-in only
   int path = pairs >= 4096 ? (line_ok ? 2 : plane_ok ? 1 : 0) : 0;
   const char* force = env_override(ENV_ROI_ALIGN_PATH);   // "generic" | "plane" | "line" | "band" (testing / profiling)
   if (force && force[0] == 'g') path = 0;

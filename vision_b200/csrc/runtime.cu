@@ -32,7 +32,7 @@ DevAttr& attr() {
   if (!a.init) {
     cudaDeviceGetAttribute(&a.sms, cudaDevAttrMultiProcessorCount, dev);
     cudaDeviceGetAttribute(&a.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    if (a.sms <= 0) a.sms = kNumSMsB200;
+    if (a.sms <= 0) a.sms = 132;                // H100 SXM
     if (a.smem_optin <= 0) a.smem_optin = 232448;
     a.init = true;
   }
@@ -42,8 +42,8 @@ DevAttr& attr() {
 
 namespace {
 const char* const kEnvNames[ENV_COUNT] = {"VB200_ROI_ALIGN_PATH", "VB200_ROI_LINE_AXIS", "VB200_NMS_PATH", "VB200_BNMS_PATH",
-                                          "VB200_BNMS_WARPS", "VB200_RESIZE_PATH", "VB200_DCN_PATH", "VB200_DCN_CTA2",
-                                          "VB200_DCN_STAGES", "VB200_DCN_BN", "VB200_ROI_BWD_PATH", "VB200_BNMS_GRAPH", "VB200_DCN_BLEND", "VB200_ROI_BAND_OVH"};
+                                          "VB200_BNMS_WARPS", "VB200_RESIZE_PATH", "VB200_DCN_PATH",
+                                          "VB200_DCN_BN", "VB200_ROI_BWD_PATH", "VB200_BNMS_GRAPH", "VB200_DCN_BLEND", "VB200_ROI_BAND_OVH"};
 std::atomic<int> g_env_gen{0};
 char g_env_val[ENV_COUNT][32];
 std::atomic<int> g_env_set[ENV_COUNT];

@@ -413,7 +413,7 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> detection_postprocess(const at::T
 // ---- deform_conv2d ---------------------------------------------------------
 // Packed weights are cached per weight tensor: the key is the TensorImpl (held weakly, so a recycled address cannot
 // alias) plus its version counter (an in-place update of the parameter invalidates the entry) plus the generation of the
-// VB200_* overrides (VB200_DCN_CTA2 / VB200_DCN_BN change the packed layout).
+// VB200_* overrides (VB200_DCN_BN changes the packed layout).
 struct PackedWeight {
   c10::weak_intrusive_ptr<c10::TensorImpl> impl;
   uint32_t version;

@@ -1,6 +1,6 @@
 """Host-side mirror of ``torchvision.ops`` for the hot path: same names, arguments and errors
 (torchvision/ops/boxes.py:20-126, roi_align.py:204-285, roi_pool.py:15-53, ps_roi_align.py:11-59,
-deform_conv.py:14-107), routed to the sm_100a kernels through ``torch.ops.vision_b200``.
+deform_conv.py:14-107), routed to the sm_90a kernels through ``torch.ops.vision_b200``.
 
 These functions accept CUDA tensors only — there is no CPU path in this package (the reference's
 CPU kernels keep serving CPU tensors through ``torchvision.ops`` itself, untouched by install()).

@@ -346,7 +346,7 @@ def deform_conv2d_gather(input: torch.Tensor, offset: torch.Tensor, weight: torc
                          stride=(1, 1), padding=(0, 0), dilation=(1, 1), mask=None, group=None):
     """``deform_conv2d`` on this rank's images + all-gather of the ``[n, C_out, H, W]`` outputs over the ranks, rank-major.
 
-    With a `PeerGather` buffer the tcgen05 kernel's epilogue stores every output element to all ranks' buffers (NVLink peer
+    With a `PeerGather` buffer the wgmma kernel's epilogue stores every output element to all ranks' buffers (NVLink peer
     stores); without one: the op followed by the NCCL exchange."""
     from . import _lib, ops as _ops
 

@@ -2,7 +2,7 @@
 (torchvision/transforms/v2/functional/_geometry.py:236-362, transforms/functional.py:353-384).
 
 Output-size rules, interpolation checks and the "same size -> return input" shortcut are the
-reference's; the compute is ONE fused sm_100a kernel (storage dtype in, fp32 math, storage dtype
+reference's; the compute is ONE fused sm_90a kernel (storage dtype in, fp32 math, storage dtype
 out) instead of cast -> aten::upsample_* -> cast.
 """
 from __future__ import annotations
