@@ -74,8 +74,8 @@ VB200_API uint64_t vb200_launch_count(void);
 /* The VB200_* path overrides (DESIGN.md, testing / profiling only) are read from the environment once, the first
  * time a launcher needs them; this re-reads them (tests switch paths inside one process). */
 VB200_API void vb200_reload_env(void);
-/* Generation counter of those overrides (bumped by every (re)load): callers that cache layout-dependent artefacts, e.g.
- * packed deform_conv2d weights, key them on it. */
+/* Generation counter of those overrides (bumped by every (re)load): callers that cache work recorded under one setting
+ * of them, e.g. captured CUDA graphs (as the library's own batched_nms graph cache does), key the cache on it. */
 VB200_API int vb200_env_generation(void);
 
 /* ---- roi_align ---------------------------------------------------------

@@ -82,17 +82,13 @@ def dcn():
         env("VB200_DCN_PATH", None)
 
 
-def band():
-    """round 2: the band-resident roi_align kernel (several bands, split bin rows -> RED) and the multi-destination stores"""
+def gather():
+    """the multi-destination stores of the fused all-gather (roi_align, resize, deform_conv2d)"""
     x, r, kw = workloads.cfg2_roi_align(seed=3, k=200, batch=2, channels=8, height=80, width=200)
     r = r.clone()
     r[::7, 1:3] -= 90.0
     r[1::11, 3:] += 400.0
     x, r = x.to(dev), r.to(dev)
-    env("VB200_ROI_ALIGN_PATH", "band")
-    vb.ops.roi_align(x, r, 7, 0.25, 2, False)
-    vb.ops.roi_align(x, r, 7, 0.25, 2, True)
-    env("VB200_ROI_ALIGN_PATH", None)
     want = vb.ops.roi_align(x, r, 7, 0.25, 2, False)
     bufs = [torch.empty_like(want) for _ in range(3)]
     torch.ops.vision_b200.roi_align_gather(x, r, [b.data_ptr() for b in bufs], 0, 0.25, 7, 7, 2, False)
@@ -108,7 +104,7 @@ def band():
     torch.ops.vision_b200.deform_conv2d_gather(xi, w, off, m, bias, [t.data_ptr() for t in d], 1, 1, 1, 1, 1, 1, 1, 1, True)
 
 
-for name, fn in (("roi", roi), ("nms", nms), ("resize", resize), ("dcn", dcn), ("band", band)):
+for name, fn in (("roi", roi), ("nms", nms), ("resize", resize), ("dcn", dcn), ("gather", gather)):
     if only in ("all", name):
         fn()
         torch.cuda.synchronize()

@@ -51,8 +51,8 @@ int max_smem_optin();
 
 // VB200_* path overrides (testing / profiling): read from the environment ONCE when the library first needs them
 // (no getenv on the per-call path); vb200_reload_env() re-reads them.  nullptr when unset.
-enum EnvKey { ENV_ROI_ALIGN_PATH, ENV_ROI_LINE_AXIS, ENV_NMS_PATH, ENV_BNMS_PATH, ENV_BNMS_WARPS, ENV_RESIZE_PATH, ENV_DCN_PATH,
-              ENV_DCN_BN, ENV_ROI_BWD_PATH, ENV_BNMS_GRAPH, ENV_DCN_BLEND, ENV_ROI_BAND_OVH, ENV_COUNT };
+enum EnvKey { ENV_ROI_ALIGN_PATH, ENV_NMS_PATH, ENV_BNMS_PATH, ENV_RESIZE_PATH, ENV_DCN_PATH, ENV_ROI_BWD_PATH, ENV_BNMS_GRAPH,
+              ENV_COUNT };
 const char* env_override(EnvKey k);
 int env_generation();     // bumped by every (re)load of the overrides: caches keyed on it forget their entries
 

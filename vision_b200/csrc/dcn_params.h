@@ -4,7 +4,6 @@ namespace vb200 {
 struct DcnParams {
   int batch, c_in, in_h, in_w, c_out, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w;
   int groups, offset_groups, use_mask, out_h, out_w;
-  int blend16;   // tensor-core 16-bit path: blend the four corners in the storage format (HFMA2) instead of fp32
   // fused all-gather (vb200_deform_conv2d_forward_gather): the epilogue also stores every output element to the same slot of
   // the peers' gathered buffers (peer-mapped device pointers; NVLink stores)
   void* peer_out[7];

@@ -177,13 +177,6 @@ template <> struct Wgmma<256> {
 template <typename T> struct Elem;
 template <> struct Elem<__nv_bfloat16> {
   static constexpr uint32_t kFmt = 1;
-  // packed 16-bit blend (HFMA2.BF16): weight pair x value pair + accumulator pair, one rounding to bf16 per step
-  static __device__ __forceinline__ uint32_t dup(float w) { __nv_bfloat162 v = __float2bfloat162_rn(w); return *reinterpret_cast<uint32_t*>(&v); }
-  static __device__ __forceinline__ uint32_t mul2(uint32_t w, uint32_t a) {
-    __nv_bfloat162 r = __hmul2(*reinterpret_cast<__nv_bfloat162*>(&w), *reinterpret_cast<__nv_bfloat162*>(&a)); return *reinterpret_cast<uint32_t*>(&r); }
-  static __device__ __forceinline__ uint32_t fma2p(uint32_t w, uint32_t a, uint32_t c) {
-    __nv_bfloat162 r = __hfma2(*reinterpret_cast<__nv_bfloat162*>(&w), *reinterpret_cast<__nv_bfloat162*>(&a), *reinterpret_cast<__nv_bfloat162*>(&c));
-    return *reinterpret_cast<uint32_t*>(&r); }
   static __device__ __forceinline__ float2 up(uint32_t u) { return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u)); }
   static __device__ __forceinline__ uint32_t pk(float a, float b) { __nv_bfloat162 v = __floats2bfloat162_rn(a, b); return *reinterpret_cast<uint32_t*>(&v); }
 };
@@ -360,9 +353,10 @@ deform_conv2d_tc_kernel(const T* __restrict__ nhwc, const T* __restrict__ wpacke
       for (int i = 0; i < 4; ++i) {
         const float wv[4] = {wq[i].x, wq[i].y, wq[i].z, wq[i].w};
         uint4 o;
-        if (p.blend16) {
-          // blend in the storage format (HFMA2): 16 instructions per 8 channels instead of 52 (unpack + FFMA + pack).  Every
-          // step rounds to 16 bits - the A operand is rounded to that format anyway; the whole op stays inside its 1e-2 bound.
+        if constexpr (std::is_same<T, __half>::value) {
+          // fp16: blend in the storage format (HFMA2): 16 instructions per 8 channels instead of 52 (unpack + FFMA + pack).
+          // Every step rounds to 16 bits - the A operand is rounded to that format anyway; the whole op stays inside its 1e-2
+          // bound.  bf16 keeps the fp32 blend: packed in bf16 the blend exceeds that bound (DESIGN §4.5).
           const uint32_t w0 = Elem<T>::dup(wv[0]), w1 = Elem<T>::dup(wv[1]), w2_ = Elem<T>::dup(wv[2]), w3 = Elem<T>::dup(wv[3]);
           o.x = Elem<T>::fma2p(w3, v[i][3].x, Elem<T>::fma2p(w2_, v[i][2].x, Elem<T>::fma2p(w1, v[i][1].x, Elem<T>::mul2(w0, v[i][0].x))));
           o.y = Elem<T>::fma2p(w3, v[i][3].y, Elem<T>::fma2p(w2_, v[i][2].y, Elem<T>::fma2p(w1, v[i][1].y, Elem<T>::mul2(w0, v[i][0].y))));
@@ -644,16 +638,9 @@ size_t tc_smem_bytes(int BN, int KK) {
   return (size_t)tc_stages(BN) * (TC_BM + BN) * 128 + 64 + (size_t)KK * TC_BM * sizeof(TcEnt) + 1024;
 }
 int tc_pick_bn(const DcnParams& p) {
-  const char* env = env_override(ENV_DCN_BN);           // profiling override: 128 / 256
   const int KK = p.kh * p.kw;
-  const int cands[2] = {256, 128};
-  for (int c = 0; c < 2; ++c) {
-    const int bn = cands[c];
-    if (env && atoi(env) != bn) continue;
+  for (const int bn : {256, 128})
     if (p.c_out % bn == 0 && tc_smem_bytes(bn, KK) <= (size_t)max_smem_optin()) return bn;
-  }
-  for (int c = 0; c < 2; ++c)
-    if (p.c_out % cands[c] == 0 && tc_smem_bytes(cands[c], KK) <= (size_t)max_smem_optin()) return cands[c];
   return 0;
 }
 
@@ -681,12 +668,6 @@ template <typename T>
 int launch_tc(const void* input, const void* weight, const void* offset, const void* mask, const void* bias, void* out,
               const DcnParams& p_in, void* workspace, size_t workspace_bytes, cudaStream_t st, const DcnHints& hints) {
   DcnParams p = p_in;
-  {
-    // corner blend: fp32 FMA, or packed in the storage format (HFMA2).  Default: packed for fp16 (worst error 0.13 of the 1e-2
-    // bound on cfg4), fp32 for bf16 (the packed bf16 blend reaches 1.06 of the bound); VB200_DCN_BLEND=16|32 overrides.
-    const char* env = env_override(ENV_DCN_BLEND);
-    p.blend16 = env ? (env[0] == '1' && env[1] == '6') : (sizeof(T) == 2 && std::is_same<T, __half>::value);
-  }
   const int KK = p.kh * p.kw, HWi = p.in_h * p.in_w, HWo = p.out_h * p.out_w;
   const size_t nhwc_bytes = hints.input_is_nhwc ? 0 : align256((size_t)p.batch * HWi * p.c_in * sizeof(T));
   const size_t w_bytes = hints.packed_weight ? 0 : align256((size_t)p.c_out * p.c_in * KK * sizeof(T));

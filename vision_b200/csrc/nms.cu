@@ -281,12 +281,13 @@ __device__ __forceinline__ bool iou_gt_filter(const double4a, const double, cons
   return false;
 }
 
-// CTA = one block of 64 rows (positions), 2 warps (small CTAs: a row block has 1..33 tiles, and a CTA lives as
-// long as its busiest warp); a warp owns whole 64x64 tiles (column block kb = i + warp, i + warp + 2, ...): its
-// lanes hold two column boxes each, the rows are broadcast from shared memory, and one vote per 32 IoU tests
-// delivers the bits.  min/max, compares and votes share the half-rate ALU pipe, which is what bounds this
-// kernel, so everything else (result capture, unsure flags, column validity) is kept off it or out of the loop.
-template <typename Box, int SEM, int kMaskWarps>
+// CTA = one block of 64 rows (positions), kMaskWarps warps; a warp owns whole 64x64 tiles (column block
+// kb = i + warp, i + warp + kMaskWarps, ...): its lanes hold two column boxes each, the rows are broadcast from
+// shared memory, and one vote per 32 IoU tests delivers the bits.  min/max, compares and votes share the
+// half-rate ALU pipe, which is what bounds this kernel, so everything else (result capture, unsure flags, column
+// validity) is kept off it or out of the loop.
+constexpr int kMaskWarps = 8;
+template <typename Box, int SEM>
 __global__ void __launch_bounds__(kMaskWarps * 32)
 bnms_mask_kernel(const Box* __restrict__ boxes, const int* __restrict__ seg_start, const int* __restrict__ num_seg_ptr,
                  int n, int wpr, int max_len, IouParams prm, unsigned long long* __restrict__ mask) {
@@ -699,9 +700,9 @@ int run_single_segment(const Box* boxes_sorted, int64_t n, IouParams prm, uint8_
   // IoU bit matrix on every SM (row pitch = the number of 64-position blocks), then one CTA walks the chain
   const int cb = (int)ceil_div64(n, 64);
   if (prm.semantics == VB200_NMS_CUDA)
-    bnms_mask_kernel<Box, VB200_NMS_CUDA, 8><<<cb, 256, 0, st>>>(boxes_sorted, nullptr, nullptr, (int)n, cb, (int)n, prm, mask);
+    bnms_mask_kernel<Box, VB200_NMS_CUDA><<<cb, kMaskWarps * 32, 0, st>>>(boxes_sorted, nullptr, nullptr, (int)n, cb, (int)n, prm, mask);
   else
-    bnms_mask_kernel<Box, VB200_NMS_CPU, 8><<<cb, 256, 0, st>>>(boxes_sorted, nullptr, nullptr, (int)n, cb, (int)n, prm, mask);
+    bnms_mask_kernel<Box, VB200_NMS_CPU><<<cb, kMaskWarps * 32, 0, st>>>(boxes_sorted, nullptr, nullptr, (int)n, cb, (int)n, prm, mask);
   int rc = check_launch("bnms_mask_kernel");
   if (rc) return rc;
   const size_t smem = 2 * (size_t)(cb + 4) * sizeof(unsigned long long);
@@ -894,17 +895,12 @@ int bnms_core(const void* boxes, const void* scores, const int64_t* idxs, int64_
   const char* mp = env_override(ENV_BNMS_PATH);       // "chain": per-class sequential kernel only (testing / profiling)
   const bool use_mask = !(mp && mp[0] == 'c');
   if (use_mask) {
-    const char* mw = env_override(ENV_BNMS_WARPS);     // tuning: warps per mask CTA (2 | 4 | 8)
-    const int warps = mw ? atoi(mw) : 8;
-#define VB200_LAUNCH_MASK(SEMV, WV)                                                                        \
-  bnms_mask_kernel<Box, SEMV, WV><<<ceil_div(ni, 64), WV * 32, 0, st>>>((const Box*)w.boxes_cm, w.seg_start, \
-                                                                        w.num_seg, ni, kBnmsWpr, kBnmsMaxLen, prm, w.mask)
-    if (semantics == VB200_NMS_CUDA) {
-      if (warps == 2) VB200_LAUNCH_MASK(VB200_NMS_CUDA, 2); else if (warps == 8) VB200_LAUNCH_MASK(VB200_NMS_CUDA, 8); else VB200_LAUNCH_MASK(VB200_NMS_CUDA, 4);
-    } else {
-      if (warps == 2) VB200_LAUNCH_MASK(VB200_NMS_CPU, 2); else if (warps == 8) VB200_LAUNCH_MASK(VB200_NMS_CPU, 8); else VB200_LAUNCH_MASK(VB200_NMS_CPU, 4);
-    }
-#undef VB200_LAUNCH_MASK
+    if (semantics == VB200_NMS_CUDA)
+      bnms_mask_kernel<Box, VB200_NMS_CUDA><<<ceil_div(ni, 64), kMaskWarps * 32, 0, st>>>(
+          (const Box*)w.boxes_cm, w.seg_start, w.num_seg, ni, kBnmsWpr, kBnmsMaxLen, prm, w.mask);
+    else
+      bnms_mask_kernel<Box, VB200_NMS_CPU><<<ceil_div(ni, 64), kMaskWarps * 32, 0, st>>>(
+          (const Box*)w.boxes_cm, w.seg_start, w.num_seg, ni, kBnmsWpr, kBnmsMaxLen, prm, w.mask);
     rc = check_launch("bnms_mask_kernel");
     if (rc) return rc;
   }

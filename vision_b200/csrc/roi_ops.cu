@@ -368,7 +368,7 @@ __device__ __forceinline__ int map_level(const float* __restrict__ box /* x1 y1 
 template <int P, int SR, bool MULTI>
 __global__ void __launch_bounds__(256)
 roi_align_line_geometry_kernel(const float* __restrict__ rois, LineTab* __restrict__ tab, int K, int H, int W,
-                               float scale, int aligned, int pitch, int force_axis, int B, LevelSet L,
+                               float scale, int aligned, int pitch, int B, LevelSet L,
                                int* __restrict__ lvl_count, int* __restrict__ bucket, int32_t* __restrict__ lvl_out) {
   constexpr int NS = P * SR, NL = NS * 2;
   asm volatile("griddepcontrol.launch_dependents;");   // the gather kernel may start staging its first plane
@@ -393,7 +393,7 @@ roi_align_line_geometry_kernel(const float* __restrict__ rois, LineTab* __restri
   packed_axis(axis_entry<float>(sample_coord<float>(g.start_h, g.bin_h, j / SR, j % SR, SR), H), H, ylo, yl);
   const uint32_t ax = (uint32_t)(xlo + c), ay = (uint32_t)((ylo + c) * pitch);
   const int mx = bank_multiplicity(ax, act, lane), my = bank_multiplicity(ay, act, lane);
-  const bool lane_is_y = force_axis ? force_axis == 2 : my < mx;
+  const bool lane_is_y = my < mx;
   LineTab* t = tab + n;
   const float l = lane_is_y ? yl : xl;
   // lanes beyond the taps repeat lane 0's address with weight 0: a broadcast, never an extra bank conflict
@@ -621,329 +621,6 @@ roi_align_line_kernel(const float* __restrict__ input, const LineTab* __restrict
       id_next = id_next2;
     }
     w += span;
-  }
-}
-
-// ---------------------------------------------------------------------------
-// Band-resident path, channel-interleaved lanes (7 x 7 bins, sampling_ratio 2, C % 8 == 0).
-// ---------------------------------------------------------------------------
-// The line kernel above keeps ONE channel plane per CTA, so every lane of a gather has its own tap address: ~1.45
-// bank conflicts per LDS and per-lane geometry.  Here a CTA keeps EIGHT channels of a band of R image rows,
-// interleaved [row][column][channel], and a warp's lanes are (tap row r, tap column c, channel) of ONE bilinear
-// sample: lane = r * 16 + c * 8 + channel.  With a row pitch of 8 * px words, px % 4 == 2, the word address
-// (y + r) * 8 px + (x + c) * 8 + ch falls in bank 16 * ((y + r) & 1) + 8 * ((x + c) & 3) + ch: the four taps of any
-// sample always occupy the four different 8-bank groups, so EVERY gather is one conflict-free 128-byte wavefront
-// with all 32 lanes busy, and the whole sample geometry is warp-uniform (one (ylo, ly) per sample row, 14 (xlo, lx)
-// per RoI).  Bands overlap by one row (the high tap); a RoI is cut into "items" = its sample rows that start in a
-// band.  A bin row (two sample rows) that straddles two bands gets two partial sums: both are added with RED into a
-// row the geometry kernel zeroed - a + b is commutative, so the result stays bit-reproducible.
-struct BandTab {            // per RoI, 256 B
-  uint2 x[14];              // per x sample: (BYTE offset of column xlo inside a band row = xlo * 32, lx)
-  uint32_t pad0[4];
-  uint2 y[14];              // per y sample: (ylo, ly); ylo = 0xffffffff when the sample row lies outside the map
-  uint32_t pad1[4];
-};
-static_assert(sizeof(BandTab) == 256, "BandTab layout");
-
-constexpr int kBandThreads = 512, kBandWarps = kBandThreads / 32;
-constexpr int kBandMaxGroups = 512;            // (image, band) pairs of one call
-constexpr int kBandSlotBytes = 512;            // per warp: two 256-byte table slots
-constexpr int kBandAuxBytes = kBandWarps * kBandSlotBytes + (kBandMaxGroups + 1) * 4 + 60;
-constexpr uint32_t kBandRoiMask = (1u << 22) - 1u;
-
-__host__ __device__ inline int band_pitch(int W) {   // columns per band row: >= W + 2 zero columns, == 2 (mod 4)
-  int p = W + 2;
-  while ((p & 3) != 2) ++p;
-  return p;
-}
-
-constexpr int kBandGeoThreads = 512;      // 16 RoIs per CTA: their item appends are aggregated per (image, band) group
-
-template <int P, int SR>
-__global__ void __launch_bounds__(kBandGeoThreads)
-roi_align_band_geometry_kernel(const float* __restrict__ rois, BandTab* __restrict__ tab, int* __restrict__ cnt,
-                               uint32_t* __restrict__ items, float* __restrict__ output, int K, int C, int H, int W,
-                               float scale, int aligned, int B, int S, int NB, int px) {
-  constexpr int NS = P * SR, NBIN = P * P;
-  static_assert(NS == 14, "item words carry 4-bit sample-row indices");
-  __shared__ int lcount[kBandMaxGroups], gbase[kBandMaxGroups];
-  asm volatile("griddepcontrol.launch_dependents;");
-  const int NG = B * NB;
-  for (int i = threadIdx.x; i < NG; i += blockDim.x) lcount[i] = 0;
-  __syncthreads();
-  const int n = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  const bool live = n < K;
-  RoiGeom<float> g = {};
-  if (live) g = roi_geometry<float, float>(rois + (int64_t)n * 5, scale, P, P, SR, aligned != 0, false);
-  const bool dead = !live || g.batch < 0 || g.batch >= B;      // bad batch index: the reference would read out of bounds, zeros here
-  const bool act = lane < NS;
-  const int j = act ? lane : 0;
-  const AxisEnt<float> ax = axis_entry<float>(sample_coord<float>(g.start_w, g.bin_w, j / SR, j % SR, SR), W);
-  const AxisEnt<float> ay = axis_entry<float>(sample_coord<float>(g.start_h, g.bin_h, j / SR, j % SR, SR), H);
-  const bool yvalid = act && !dead && ay.lo >= 0;
-  if (act && live) {
-    // outside in x: the two zero columns W, W + 1.  Border (lo == hi == size - 1, l == 0): the high tap is the zero
-    // column / zero row with weight 0.  y entries carry the BYTE offset of image row ylo in a band that starts at row 0.
-    tab[n].x[lane] = ax.lo < 0 ? make_uint2((uint32_t)W * 32u, 0u) : make_uint2((uint32_t)ax.lo * 32u, __float_as_uint(ax.l));
-    tab[n].y[lane] = make_uint2(yvalid ? (uint32_t)ay.lo * (uint32_t)px * 32u : 0xffffffffu, __float_as_uint(ay.l));
-  }
-  // items: maximal runs of consecutive valid sample rows that start in the same band.  A run start reserves a slot in
-  // its group's list: first inside the CTA (shared-memory counter), then one global atomic per (CTA, group) - the
-  // per-group counters would otherwise serialise ~3 atomics per RoI on a handful of addresses.
-  const int band = yvalid ? ay.lo / S : -1;
-  const int band_prev = __shfl_up_sync(0xffffffffu, band, 1);
-  const bool start = yvalid && (lane == 0 || band_prev != band);
-  const unsigned vmask = __ballot_sync(0xffffffffu, yvalid);
-  const unsigned smask = __ballot_sync(0xffffffffu, start);
-  int grp = 0, local = 0;
-  uint32_t item = 0;
-  if (start) {
-    // the run ends before the next run start or the first invalid row after `lane`
-    const unsigned after = ~((2u << lane) - 1u);
-    const unsigned stop = (smask | ~vmask) & after;                 // bits NS.. of ~vmask are set: a stop always exists
-    const int len = __ffs(stop) - 1 - lane;
-    const int last = lane + len - 1;
-    const unsigned fr = ((lane & 1) && ((vmask >> (lane - 1)) & 1u)) ? 1u : 0u;      // first bin row shared with another item
-    const unsigned lr = (!(last & 1) && ((vmask >> (last + 1)) & 1u)) ? 1u : 0u;     // last bin row shared
-    grp = g.batch * NB + band;
-    local = atomicAdd(lcount + grp, 1);
-    item = (uint32_t)n | ((uint32_t)lane << 22) | ((uint32_t)(len - 1) << 26) | (fr << 30) | (lr << 31);
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < NG; i += blockDim.x) {
-    const int c = lcount[i];
-    if (c > 0) gbase[i] = atomicAdd(cnt + i, c);
-  }
-  __syncthreads();
-  if (start) items[(int64_t)grp * K + gbase[grp] + local] = item;
-  // bin rows nobody writes (both sample rows outside) or two items add into: zero them here
-  bool z = false;
-  {
-    const int b0 = __shfl_sync(0xffffffffu, band, (2 * lane) & 31), b1 = __shfl_sync(0xffffffffu, band, (2 * lane + 1) & 31);
-    if (lane < P && live) {
-      const bool s0 = (vmask >> (2 * lane)) & 1u, s1 = (vmask >> (2 * lane + 1)) & 1u;
-      z = (!s0 && !s1) || (s0 && s1 && b0 != b1);
-    }
-  }
-  unsigned zmask = __ballot_sync(0xffffffffu, z);
-  if (zmask && lane < 4 * P) {
-    const int pw = lane % P, cl = lane / P;
-    float* __restrict__ o = output + (int64_t)n * C * NBIN + pw;
-    while (zmask) {
-      const int ph = __ffs(zmask) - 1;
-      zmask &= zmask - 1;
-#pragma unroll 4
-      for (int c = cl; c < C; c += 4) o[c * NBIN + ph * P] = 0.f;
-    }
-  }
-}
-
-__device__ __forceinline__ uint2 lds_u64(uint32_t addr) {
-  uint2 v;
-  asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
-  return v;
-}
-
-// x geometry of one item as a lane sees it: tap addresses (relative to the row) and x weights of its tap column.
-struct BandX {
-  uint32_t xo[14];
-  float wx[14];
-};
-
-template <int P, int SR>
-__global__ void __launch_bounds__(kBandThreads, 1)
-roi_align_band_kernel(const float* __restrict__ input, const BandTab* __restrict__ tab, const int* __restrict__ cnt,
-                      const uint32_t* __restrict__ items, float* __restrict__ output, int B, int C, int H, int W, int K,
-                      int px, int R, int S, int NB, int ovh) {
-  constexpr int NS = P * SR, NBIN = P * P;
-  static_assert(P == 7 && SR == 2, "lane mapping and fold are written for 7 x 7 bins, 2 x 2 samples");
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  float* tile = reinterpret_cast<float*>(smem_raw);
-  const uint32_t tile_s = smem_u32(tile);
-  const uint32_t row_bytes = (uint32_t)px * 32u;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const uint32_t slot_s = tile_s + (uint32_t)R * row_bytes + (uint32_t)warp * kBandSlotBytes;
-  int* pre = reinterpret_cast<int*>(smem_raw + (size_t)R * row_bytes + kBandWarps * kBandSlotBytes);
-
-  const int tr = lane >> 4, tc = (lane >> 3) & 1, ch = lane & 7;
-  const uint32_t lane_off = (uint32_t)tr * row_bytes + (uint32_t)tc * 32u + (uint32_t)ch * 4u;
-  const int G = C >> 3, NG = B * NB;
-  // store mapping after the fold (see emit below): bin st_pw = 2 * (lane >> 3) + (ch >> 2), channels (ch & 3) and (ch & 3) + 4
-  const int st_pw = 2 * (lane >> 3) + (ch >> 2);
-  const bool st_ok = st_pw < P;
-  const bool odd = (ch >> 2) != 0;
-
-  asm volatile("griddepcontrol.wait;" ::: "memory");      // tables, item lists and the zeroed rows come from the geometry kernel
-  if (warp == 0) {
-    int running = 0;
-    for (int base = 0; base < NG; base += 32) {
-      const int i = base + lane;
-      int v = 0;
-      if (i < NG) { const int c = __ldg(cnt + i); v = c > 0 ? c + ovh : 0; }
-      int inc = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-      if (i < NG) pre[i + 1] = running + inc;
-      running += __shfl_sync(0xffffffffu, inc, 31);
-    }
-    if (lane == 0) pre[0] = 0;
-  }
-  __syncthreads();
-  const int64_t total = (int64_t)G * pre[NG];
-  const int64_t per = (total + gridDim.x - 1) / gridDim.x;
-  const int64_t w0 = (int64_t)blockIdx.x * per;
-  const int64_t w1 = min(total, w0 + per);
-  const int nch = (px + 31) >> 5;
-  const int64_t plane = (int64_t)H * W;
-
-  // fold the four tap lanes of a bin row (xor 16, xor 8), trade halves across channel bit 2 so that each store
-  // instruction covers 4 channels x 7 bins (4 lines instead of 8), scale by 1 / count and store (or RED when a second
-  // item adds the other sample row of this bin row)
-  auto emit = [&](const float (&acc)[8], float* __restrict__ o, bool red) {
-    float r4[4];
-#pragma unroll
-    for (int m = 0; m < 4; ++m) {
-      const float send = tr ? acc[m] : acc[4 + m], keep = tr ? acc[4 + m] : acc[m];
-      r4[m] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-    }
-    float s2[2];
-#pragma unroll
-    for (int m = 0; m < 2; ++m) {
-      const float send = tc ? r4[m] : r4[2 + m], keep = tc ? r4[2 + m] : r4[m];
-      s2[m] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-    }
-    const float got = __shfl_xor_sync(0xffffffffu, odd ? s2[0] : s2[1], 4);
-    const float va = (odd ? got : s2[0]) * 0.25f;        // channel (ch & 3),     bin st_pw
-    const float vb = (odd ? s2[1] : got) * 0.25f;        // channel (ch & 3) + 4, bin st_pw
-    if (st_ok) {
-      if (red) { atomicAdd(o, va); atomicAdd(o + 4 * NBIN, vb); }
-      else { o[0] = va; o[4 * NBIN] = vb; }
-    }
-  };
-
-  int64_t w = w0;
-  while (w < w1) {
-    // ---- locate (image, band) group j, channel group g and the item range of work position w ----
-    const int u = (int)(w / G);
-    int lo_ = 0, hi_ = NG;                       // largest j with pre[j] <= u
-    while (hi_ - lo_ > 1) { const int mid = (lo_ + hi_) >> 1; if (pre[mid] <= u) lo_ = mid; else hi_ = mid; }
-    const int j = lo_;
-    const int cj = pre[j + 1] - pre[j];
-    const int64_t wl = w - (int64_t)G * pre[j];
-    const int g = (int)(wl / cj);
-    const int f = (int)(wl - (int64_t)g * cj);
-    const int span = (int)min((int64_t)(cj - f), w1 - w);
-    const int r0 = max(0, f - ovh), r1 = min(cj - ovh, f + span - ovh);
-    w += span;
-    if (r1 <= r0) continue;                      // this CTA's share of the tile is load cost only
-    const int b = j / NB, band = j - b * NB;
-    const int y0 = band * S;
-    __syncthreads();                             // everyone is done with the previous tile
-    // ---- stage the tile: rows [y0, y0 + R) x 8 channels, transposed to [row][column][channel]; rows >= H and
-    //      columns >= W are written as zeros (every word of the tile is rewritten) ----
-    {
-      // one base pointer per channel, kept in registers; a load address is base + 4 * (32-bit offset): one IMAD.WIDE
-      unsigned long long pc[8];
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        pc[c] = (unsigned long long)(input + ((int64_t)b * C + (int64_t)g * 8 + c) * plane + lane);
-        asm volatile("" : "+l"(pc[c]));          // keep it live (ptxas otherwise re-derives it from the parameters per load)
-      }
-      constexpr int U = 6;                       // 48 independent loads per thread in flight
-      int rr = 0, k = warp;                      // task = (band row rr, 32-column chunk k); tasks are dealt round-robin to the warps
-      while (k >= nch) { k -= nch; ++rr; }
-      while (rr < R) {
-        float v[U][8];
-        int trow[U], tx[U];
-#pragma unroll
-        for (int q = 0; q < U; ++q) {
-          trow[q] = rr; tx[q] = k * 32 + lane;
-          const int y = y0 + rr;
-          const bool ok = rr < R && y < H && tx[q] < W;
-          const unsigned off = (unsigned)(y * W + k * 32);
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            v[q][c] = 0.f;
-            if (ok) asm volatile("{\n\t.reg .b64 a;\n\tmad.wide.u32 a, %1, 4, %2;\n\tld.global.nc.f32 %0, [a];\n\t}" : "=f"(v[q][c]) : "r"(off), "l"(pc[c]));
-          }
-          k += kBandWarps;
-          while (k >= nch) { k -= nch; ++rr; }
-        }
-#pragma unroll
-        for (int q = 0; q < U; ++q) {
-          if (trow[q] < R && tx[q] < px) {
-            float4* d = reinterpret_cast<float4*>(tile + ((size_t)trow[q] * px + tx[q]) * 8);
-            d[0] = make_float4(v[q][0], v[q][1], v[q][2], v[q][3]);
-            d[1] = make_float4(v[q][4], v[q][5], v[q][6], v[q][7]);
-          }
-        }
-      }
-    }
-    // ---- items: the table of the next item travels one iteration ahead (cp.async into the warp's other slot) ----
-    const uint32_t* __restrict__ il = items + (int64_t)j * K;
-    int e = r0 + warp;
-    uint32_t word = 0, word_next = 0;
-    if (e < r1) {
-      word = __ldg(il + e);
-      if (e + kBandWarps < r1) word_next = __ldg(il + e + kBandWarps);
-      if (lane < 16) cp_async16(slot_s + lane * 16u, reinterpret_cast<const uint4*>(tab + (word & kBandRoiMask)) + lane);
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    __syncthreads();                             // the tile is complete
-    uint32_t buf = 0;
-    const uint32_t band_base = tile_s - (uint32_t)y0 * row_bytes;     // address of image row 0 if the band started there
-    float* __restrict__ const out_g = output + ((int64_t)g * 8 + (ch & 3)) * NBIN + st_pw;
-    for (; e < r1; e += kBandWarps) {
-      uint32_t word_n2 = 0;
-      if (e + 2 * kBandWarps < r1) word_n2 = __ldg(il + e + 2 * kBandWarps);
-      if (e + kBandWarps < r1 && lane < 16)
-        cp_async16(slot_s + (buf ^ 256u) + lane * 16u, reinterpret_cast<const uint4*>(tab + (word_next & kBandRoiMask)) + lane);
-      asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 1;" ::: "memory");
-      __syncwarp();
-      const uint32_t st = slot_s + buf;
-      BandX X;
-#pragma unroll
-      for (int q = 0; q < NS / 2; ++q) {
-        const uint4 xe = lds_u128(st + q * 16u);
-        X.xo[2 * q] = xe.x + lane_off;
-        X.xo[2 * q + 1] = xe.z + lane_off;
-        const float l0 = __uint_as_float(xe.y), l1 = __uint_as_float(xe.w);
-        X.wx[2 * q] = tc ? l0 : 1.f - l0;
-        X.wx[2 * q + 1] = tc ? l1 : 1.f - l1;
-      }
-      const uint32_t uw = word;
-      const int iy0 = (int)((uw >> 22) & 15u), iy1 = iy0 + (int)((uw >> 26) & 15u);   // inclusive
-      const bool fr = (uw >> 30) & 1u, lr = (uw >> 31) & 1u;
-      float* __restrict__ ob = out_g + (int64_t)(uw & kBandRoiMask) * C * NBIN;
-      float acc[8];
-      acc[7] = 0.f;
-      // One loop over the item's sample rows.  (A variant that gathers both rows of a bin row at once lost the
-      // [register + uniform register] addressing in ptxas 12.9 and paid 28 address adds per bin row.)
-      for (int iy = iy0; iy <= iy1; ++iy) {
-        const uint2 ye = lds_u64(st + 128u + (uint32_t)iy * 8u);
-        // every lane read the same word: the warp reduction (CREDUX) returns it in a uniform register, so the 14 gathers
-        // below are LDS [lane register + uniform register] with no per-lane address arithmetic
-        const uint32_t rowb = __reduce_max_sync(0xffffffffu, band_base + ye.x);
-        const float la = __uint_as_float(ye.y);
-        const float wy = tr ? la : 1.f - la;
-        if (iy == iy0 || !(iy & 1)) {
-#pragma unroll
-          for (int p = 0; p < P; ++p) acc[p] = 0.f;
-        }
-#pragma unroll
-        for (int p = 0; p < P; ++p) {
-          const float v0 = lds_f32(rowb + X.xo[2 * p]), v1 = lds_f32(rowb + X.xo[2 * p + 1]);
-          const float t = fmaf(X.wx[2 * p + 1], v1, X.wx[2 * p] * v0);
-          acc[p] = fmaf(wy, t, acc[p]);
-        }
-        // the leading odd row / trailing even row of an item share their bin row with another item: RED
-        if ((iy & 1) || iy == iy1) emit(acc, ob + (iy >> 1) * P, (iy & 1) ? (iy == iy0 && fr) : lr);
-      }
-      __syncwarp();                               // all lanes are done with this slot before it is refilled
-      buf ^= 256u;
-      word = word_next;
-      word_next = word_n2;
-    }
   }
 }
 
@@ -1330,26 +1007,7 @@ using namespace vb200;
 namespace {
 // Path selection shared by the workspace query and the launcher.
 //   0 generic, 1 plane-resident thread-per-bin (any pooled size, sampling_ratio 1..4),
-//   2 plane-resident line-wise lanes (7x7 bins, sampling_ratio 2: the detection-head shape),
-//   3 band-resident channel-interleaved lanes (same shape, channels % 8 == 0): opt-in (VB200_ROI_ALIGN_PATH=band).
-struct BandCfg { int px, R, S, NB; size_t smem; bool ok; };
-BandCfg band_config(int batch, int channels, int height, int width, int num_rois) {
-  BandCfg c = {};
-  c.px = band_pitch(width);
-  const size_t row_bytes = (size_t)c.px * 32;
-  const size_t budget = (size_t)max_smem_optin() > (size_t)kBandAuxBytes ? (size_t)max_smem_optin() - kBandAuxBytes : 0;
-  int R = (int)(budget / row_bytes);
-  if (R > height + 1) R = height + 1;
-  c.R = R;
-  c.S = R - 1;
-  if (c.S < 1) return c;
-  c.NB = ceil_div(height, c.S);
-  c.smem = (size_t)R * row_bytes + kBandAuxBytes;
-  // a band must hold enough rows for the halo row to be cheap (or the whole map), and the group table is bounded
-  c.ok = (c.S >= 8 || c.NB == 1) && (int64_t)batch * c.NB <= kBandMaxGroups && channels % 8 == 0 && channels >= 8 &&
-         num_rois < (1 << 22);
-  return c;
-}
+//   2 plane-resident line-wise lanes (7x7 bins, sampling_ratio 2: the detection-head shape).
 int roi_align_path(int dtype, const void* input, int batch, int channels, int height, int width, int num_rois,
                    int pooled_h, int pooled_w, int sampling_ratio) {
   if (dtype != VB200_F32) return 0;
@@ -1363,42 +1021,21 @@ int roi_align_path(int dtype, const void* input, int batch, int channels, int he
   const size_t line_bytes = line_plane_bytes(height, line_pitch(width)) + kLineStageBytes;
   const bool shape7 = pooled_h == 7 && pooled_w == 7 && sampling_ratio == 2;
   const bool line_ok = shape7 && line_bytes + 1024 <= (size_t)max_smem_optin();
-  const bool band_ok = shape7 && band_config(batch, channels, height, width, num_rois).ok;
   const int64_t pairs = (int64_t)batch * channels * num_rois;
-  // the band kernel is conflict-free but spends more instructions per output (per-bin-row folds, item prologues, transposing
-  // tile loads) and measured slower than the line kernel on cfg2, so it is opt-in only
   int path = pairs >= 4096 ? (line_ok ? 2 : plane_ok ? 1 : 0) : 0;
-  const char* force = env_override(ENV_ROI_ALIGN_PATH);   // "generic" | "plane" | "line" | "band" (testing / profiling)
+  const char* force = env_override(ENV_ROI_ALIGN_PATH);   // "generic" | "plane" | "line" (testing / profiling)
   if (force && force[0] == 'g') path = 0;
   if (force && force[0] == 'p') path = plane_ok ? 1 : 0;
   if (force && force[0] == 'l') path = line_ok ? 2 : 0;
-  if (force && force[0] == 'b') path = band_ok ? 3 : 0;
   return path;
 }
 size_t roi_align_geo_bytes(int num_rois, int pooled_h, int pooled_w, int sampling_ratio) {
   const size_t geo = (size_t)num_rois * (pooled_h + pooled_w) * sampling_ratio * sizeof(PackedEnt);
   return (geo + 255) & ~(size_t)255;
 }
-struct BandWs { BandTab* tab; int* cnt; uint32_t* items; size_t total; };
-BandWs carve_band(void* base, int batch, int num_rois, int NB) {
-  char* p = (char*)base;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { void* q = base ? (void*)(p + off) : nullptr; off += (bytes + 255) & ~(size_t)255; return q; };
-  BandWs w;
-  w.tab = (BandTab*)take((size_t)num_rois * sizeof(BandTab));
-  w.cnt = (int*)take((size_t)batch * NB * sizeof(int));
-  w.items = (uint32_t*)take((size_t)batch * NB * num_rois * sizeof(uint32_t));
-  w.total = off;
-  return w;
-}
-size_t roi_align_ws_bytes(int path, int batch, int channels, int height, int width, int num_rois, int pooled_h, int pooled_w,
-                          int sampling_ratio) {
+size_t roi_align_ws_bytes(int path, int num_rois, int pooled_h, int pooled_w, int sampling_ratio) {
   if (path == 1) return roi_align_geo_bytes(num_rois, pooled_h, pooled_w, sampling_ratio) + (size_t)num_rois * 4;
   if (path == 2) return (size_t)num_rois * sizeof(LineTab);
-  if (path == 3) {
-    const BandCfg c = band_config(batch, channels, height, width, num_rois);
-    return c.ok ? carve_band(nullptr, batch, num_rois, c.NB).total : 0;
-  }
   return 0;
 }
 }  // namespace
@@ -1407,10 +1044,10 @@ extern "C" size_t vb200_roi_align_workspace_bytes(int dtype, int batch, int chan
                                                   int num_rois, int pooled_h, int pooled_w,
                                                   int sampling_ratio) {
   if (num_rois <= 0 || channels <= 0) return 0;
-  // the largest of the table-driven paths, so the answer does not depend on the environment override
+  // the larger of the two table-driven paths, so the answer does not depend on the environment override
   size_t a = 0;
-  for (int path = 1; path <= 3; ++path) {
-    const size_t b = roi_align_ws_bytes(path, batch, channels, height, width, num_rois, pooled_h, pooled_w, sampling_ratio);
+  for (int path = 1; path <= 2; ++path) {
+    const size_t b = roi_align_ws_bytes(path, num_rois, pooled_h, pooled_w, sampling_ratio);
     a = b > a ? b : a;
   }
   return roi_align_path(dtype, nullptr, batch, channels, height, width, num_rois, pooled_h, pooled_w, sampling_ratio) ? a : 0;
@@ -1431,46 +1068,16 @@ static int roi_align_forward_impl(const void* input, const void* rois, void* out
   if (dtype == VB200_F32) {
     const size_t geo_pad = roi_align_geo_bytes(num_rois, pooled_h, pooled_w, sampling_ratio);
     int path = roi_align_path(dtype, input, batch, channels, height, width, num_rois, pooled_h, pooled_w, sampling_ratio);
-    const bool want_peers = peers.n > 0 || peers.mc != nullptr;
-    if (want_peers && path == 3)                 // the band kernel's RED protocol is local-only: the line kernel where it fits, else generic + copies
-      path = line_plane_bytes(height, line_pitch(width)) + kLineStageBytes + 1024 <= (size_t)max_smem_optin() ? 2 : 0;
     if (path && (workspace == nullptr || ((uintptr_t)workspace % 16) != 0 ||
-                 workspace_bytes < roi_align_ws_bytes(path, batch, channels, height, width, num_rois, pooled_h, pooled_w, sampling_ratio)))
+                 workspace_bytes < roi_align_ws_bytes(path, num_rois, pooled_h, pooled_w, sampling_ratio)))
       path = 0;
-    if (path == 3) {
-      const BandCfg bc = band_config(batch, channels, height, width, num_rois);
-      const BandWs ws = carve_band(workspace, batch, num_rois, bc.NB);
-      const char* ov = env_override(ENV_ROI_BAND_OVH);   // tuning: price of a tile load in items
-      const int ovh = ov ? atoi(ov) : 56;
-      VB200_CUDA_TRY(cudaMemsetAsync(ws.cnt, 0, (size_t)batch * bc.NB * sizeof(int), st));
-      roi_align_band_geometry_kernel<7, 2><<<ceil_div(num_rois * 32, kBandGeoThreads), kBandGeoThreads, 0, st>>>(
-          (const float*)rois, ws.tab, ws.cnt, ws.items, (float*)output, num_rois, channels, height, width, (float)spatial_scale,
-          aligned, batch, bc.S, bc.NB, bc.px);
-      int rc = check_launch("roi_align_band_geometry_kernel");
-      if (rc) return rc;
-      VB200_CUDA_TRY(ensure_dyn_smem<roi_align_band_kernel<7, 2>>(bc.smem));
-      // programmatic dependent launch: the gather kernel's CTAs are resident (shared memory carved out) while the
-      // geometry kernel still runs; they wait (griddepcontrol.wait) before reading its tables
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(sm_count()); cfg.blockDim = dim3(kBandThreads); cfg.dynamicSmemBytes = bc.smem; cfg.stream = st;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[0].val.programmaticStreamSerializationAllowed = 1;
-      cfg.attrs = attr; cfg.numAttrs = 1;
-      VB200_CUDA_TRY(cudaLaunchKernelEx(&cfg, roi_align_band_kernel<7, 2>, (const float*)input, (const BandTab*)ws.tab,
-                                        (const int*)ws.cnt, (const uint32_t*)ws.items, (float*)output, batch, channels, height,
-                                        width, num_rois, bc.px, bc.R, bc.S, bc.NB, ovh));
-      return check_launch("roi_align_band_kernel");
-    }
     if (path == 2) {
       const int pitch = line_pitch(width);
       const size_t smem = line_plane_bytes(height, pitch) + kLineStageBytes;
       LineTab* tab = (LineTab*)workspace;
-      const char* fa = env_override(ENV_ROI_LINE_AXIS);   // diagnosis: "x" | "y" pins the lane axis
-      const int force_axis = fa ? (fa[0] == 'y' ? 2 : fa[0] == 'x' ? 1 : 0) : 0;
       LevelSet none = {};
       roi_align_line_geometry_kernel<7, 2, false><<<ceil_div(num_rois * 32, 256), 256, 0, st>>>(
-          (const float*)rois, tab, num_rois, height, width, (float)spatial_scale, aligned, pitch, force_axis, batch, none, nullptr,
+          (const float*)rois, tab, num_rois, height, width, (float)spatial_scale, aligned, pitch, batch, none, nullptr,
           nullptr, nullptr);
       int rc = check_launch("roi_align_line_geometry_kernel");
       if (rc) return rc;
@@ -1635,7 +1242,7 @@ extern "C" int vb200_multiscale_roi_align_forward(const void* const* level_ptrs,
   VB200_REQUIRE((int64_t)num_rois * channels * 49 < (1ll << 31), "multiscale_roi_align: output too large for 32-bit indexing");
   VB200_CUDA_TRY(cudaMemsetAsync(ws.lvl_count, 0, kMaxLevels * sizeof(int), st));
   roi_align_line_geometry_kernel<7, 2, true><<<ceil_div(num_rois * 32, 256), 256, 0, st>>>(
-      (const float*)rois, ws.tab, num_rois, 0, 0, 0.f, 0, 0, 0, batch, L, ws.lvl_count, ws.bucket, levels_out);
+      (const float*)rois, ws.tab, num_rois, 0, 0, 0.f, 0, 0, batch, L, ws.lvl_count, ws.bucket, levels_out);
   int rc = check_launch("roi_align_line_geometry_kernel");
   if (rc) return rc;
   const int64_t pairs = (int64_t)batch * channels * num_rois;

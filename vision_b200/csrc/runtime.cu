@@ -41,9 +41,8 @@ DevAttr& attr() {
 }  // namespace
 
 namespace {
-const char* const kEnvNames[ENV_COUNT] = {"VB200_ROI_ALIGN_PATH", "VB200_ROI_LINE_AXIS", "VB200_NMS_PATH", "VB200_BNMS_PATH",
-                                          "VB200_BNMS_WARPS", "VB200_RESIZE_PATH", "VB200_DCN_PATH",
-                                          "VB200_DCN_BN", "VB200_ROI_BWD_PATH", "VB200_BNMS_GRAPH", "VB200_DCN_BLEND", "VB200_ROI_BAND_OVH"};
+const char* const kEnvNames[ENV_COUNT] = {"VB200_ROI_ALIGN_PATH", "VB200_NMS_PATH", "VB200_BNMS_PATH", "VB200_RESIZE_PATH",
+                                          "VB200_DCN_PATH", "VB200_ROI_BWD_PATH", "VB200_BNMS_GRAPH"};
 std::atomic<int> g_env_gen{0};
 char g_env_val[ENV_COUNT][32];
 std::atomic<int> g_env_set[ENV_COUNT];

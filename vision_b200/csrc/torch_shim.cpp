@@ -412,13 +412,12 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> detection_postprocess(const at::T
 
 // ---- deform_conv2d ---------------------------------------------------------
 // Packed weights are cached per weight tensor: the key is the TensorImpl (held weakly, so a recycled address cannot
-// alias) plus its version counter (an in-place update of the parameter invalidates the entry) plus the generation of the
-// VB200_* overrides (VB200_DCN_BN changes the packed layout).
+// alias) plus its version counter (an in-place update of the parameter invalidates the entry).  The packed layout follows
+// from the dtype and the shape alone; VB200_DCN_PATH=simt makes the packed size 0, so that call never reaches the cache.
 struct PackedWeight {
   c10::weak_intrusive_ptr<c10::TensorImpl> impl;
   uint32_t version;
   int dtype;
-  int env_gen;
   at::Tensor packed;
 };
 std::mutex g_pack_mu;
@@ -429,13 +428,12 @@ at::Tensor packed_weight_for(const at::Tensor& weight_c, int dt, int c_in, int c
   if (bytes == 0 || weight_c.is_inference()) return at::Tensor();
   c10::TensorImpl* impl = weight_c.unsafeGetTensorImpl();
   const uint32_t version = (uint32_t)weight_c._version();
-  const int env_gen = vb200_env_generation();
   std::lock_guard<std::mutex> lk(g_pack_mu);
   for (size_t i = 0; i < g_pack_cache.size(); ++i) {
     auto locked = g_pack_cache[i].impl.lock();
     if (!locked) { g_pack_cache.erase(g_pack_cache.begin() + i); --i; continue; }      // the weight died
     if (locked.get() == impl && g_pack_cache[i].dtype == dt) {
-      if (g_pack_cache[i].version == version && g_pack_cache[i].env_gen == env_gen) return g_pack_cache[i].packed;
+      if (g_pack_cache[i].version == version) return g_pack_cache[i].packed;
       g_pack_cache.erase(g_pack_cache.begin() + i);                                     // updated in place: re-pack
       break;
     }
@@ -446,7 +444,7 @@ at::Tensor packed_weight_for(const at::Tensor& weight_c, int dt, int c_in, int c
            "deform_conv2d");
   if (g_pack_cache.size() >= 32) g_pack_cache.erase(g_pack_cache.begin());
   g_pack_cache.push_back(PackedWeight{c10::weak_intrusive_ptr<c10::TensorImpl>(c10::intrusive_ptr<c10::TensorImpl>::reclaim_copy(impl)),
-                                      version, dt, env_gen, packed});
+                                      version, dt, packed});
   return packed;
 }
 
