@@ -108,4 +108,26 @@ __device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigne
 __host__ __device__ inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// atomicAdd of an accumulator-type value into a T element, rounded to T first.
+template <typename T> __device__ __forceinline__ void atomic_add(T* p, typename Acc<T>::type v) { atomicAdd(p, (T)v); }
+template <> __device__ __forceinline__ void atomic_add<__half>(__half* p, float v) { atomicAdd(p, __float2half_rn(v)); }
+template <> __device__ __forceinline__ void atomic_add<__nv_bfloat16>(__nv_bfloat16* p, float v) {
+  atomicAdd(p, __float2bfloat16_rn(v));
+}
+
+// ---- workspaces ---------------------------------------------------------------
+inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// Carves a workspace into 256-byte aligned arrays; with base == nullptr only sizes are accumulated.
+struct Carver {
+  char* base;
+  size_t off = 0;
+  explicit Carver(void* b) : base((char*)b) {}
+  template <typename T> T* take(size_t count) {
+    T* p = base ? (T*)(base + off) : nullptr;
+    off += align256(count * sizeof(T));
+    return p;
+  }
+};
+
 }  // namespace vb200

@@ -21,10 +21,6 @@
 namespace vb200 {
 namespace {
 
-template <typename T> __device__ __forceinline__ void atomic_add_acc(T* p, typename Acc<T>::type v) { atomicAdd(p, (T)v); }
-template <> __device__ __forceinline__ void atomic_add_acc<__half>(__half* p, float v) { atomicAdd(p, __float2half_rn(v)); }
-template <> __device__ __forceinline__ void atomic_add_acc<__nv_bfloat16>(__nv_bfloat16* p, float v) { atomicAdd(p, __float2bfloat16_rn(v)); }
-
 template <typename A>
 struct Sample {
   int o[4];          // y*W + x of the four corners (clamped into the image)
@@ -124,10 +120,10 @@ dcn_backward_inputs_kernel(const T* __restrict__ dcol, const T* __restrict__ inp
         gm += d * (w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4);
         const A md = m * d;
         T* __restrict__ gi = grad_input + plane_off;
-        if (s.ok[0] && w1 != (A)0) atomic_add_acc<T>(gi + s.o[0], md * w1);
-        if (s.ok[1] && w2 != (A)0) atomic_add_acc<T>(gi + s.o[1], md * w2);
-        if (s.ok[2] && w3 != (A)0) atomic_add_acc<T>(gi + s.o[2], md * w3);
-        if (s.ok[3] && w4 != (A)0) atomic_add_acc<T>(gi + s.o[3], md * w4);
+        if (s.ok[0] && w1 != (A)0) atomic_add<T>(gi + s.o[0], md * w1);
+        if (s.ok[1] && w2 != (A)0) atomic_add<T>(gi + s.o[1], md * w2);
+        if (s.ok[2] && w3 != (A)0) atomic_add<T>(gi + s.o[2], md * w3);
+        if (s.ok[3] && w4 != (A)0) atomic_add<T>(gi + s.o[3], md * w4);
       }
     }
     grad_offset[(ob + 2 * tap) * HWo + pix] = from_acc<T, A>(gy);

@@ -656,8 +656,6 @@ bool tc_eligible(int dtype, const DcnParams& p) {
   return true;
 }
 
-size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 template <typename T>
 int pack_tc_weights(const void* weight, T* wpacked, const DcnParams& p, cudaStream_t st) {
   pack_weights_kernel<T, 64><<<sm_count() * 4, 256, 0, st>>>((const T*)weight, wpacked, p.c_out, p.c_in, p.kh * p.kw, tc_pick_bn(p));

@@ -622,20 +622,6 @@ struct ToI64 {
   __host__ __device__ __forceinline__ int64_t operator()(const int v) const { return (int64_t)v; }
 };
 
-inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
-// Carves a workspace; with base == nullptr only sizes are accumulated.
-struct Carver {
-  char* base;
-  size_t off = 0;
-  explicit Carver(void* b) : base((char*)b) {}
-  template <typename T> T* take(size_t count) {
-    T* p = base ? (T*)(base + off) : nullptr;
-    off += align256(count * sizeof(T));
-    return p;
-  }
-};
-
 size_t cub_temp_bytes(int64_t n) {
   // upper bound over every cub call below (queried with null storage); memoised per thread
   static thread_local int64_t cached_n = -1;
