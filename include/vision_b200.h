@@ -223,6 +223,40 @@ VB200_API int vb200_detection_postprocess(const void* boxes, const void* scores,
                                 size_t workspace_bytes, void* boxes_out, void* scores_out, int64_t* labels_out,
                                 int64_t* count_host, vb200_stream stream);
 
+/* ---- single-stage detector post-processing --------------------------------------------------------------------
+ * Replaces postprocess_detections of RetinaNet (torchvision/models/detection/retinanet.py:509-571), FCOS
+ * (fcos.py:489-556) and SSD / SSDLite (ssd.py:414-463): per image, per FPN level (or per foreground class) score,
+ * `score > score_thresh`, topk(topk_candidates), decode (BoxCoder.decode_single, _utils.py:183-224, or
+ * BoxLinearCoder.decode, _utils.py:275-310) and clip_boxes_to_image of the selected items, then batched_nms ->
+ * keep[:detections_per_img] -> gather, for every image of the call in one device pipeline.
+ *   kind VB200_SS_RETINANET: score = sigmoid(logit), segment = (image, level) slice of [A_l, C] logits, flattened;
+ *        VB200_SS_FCOS:      score = sqrt(sigmoid(logit) * sigmoid(ctrness)), BoxLinearCoder(normalize_by_size=True);
+ *        VB200_SS_SSD:       score = the [A, C] softmax probabilities (num_levels = 1), segment = (image, class >= 1).
+ * Within a segment the top min(topk_candidates, n_pass) items are ordered by score descending, then flat index
+ * ascending; labels are flat index % C (RetinaNet, FCOS) or the class (SSD).
+ * HOST arrays (one entry per level unless noted): level_anchors (A_l); logits / ctrness / regression device pointers
+ * of [N, A_l, C] / [N, A_l, 1] / [N, A_l, 4] fp32 tensors whose last dimension is dense, with (image, row) strides in
+ * elements; anchors: N * L device pointers (image-major) of [A_l, 4] fp32 with their row strides; image_hw: 2N sizes;
+ * weights: the BoxCoder's 4 weights (ignored by FCOS).  topk_candidates <= VB200_SS_MAX_TOPK.
+ * Output: boxes_out [N * detections_per_img, 4] / scores_out / labels_out (int64) receive the detections of every
+ * image, concatenated; counts_host [N] (host) their per-image numbers.
+ * SYNCHRONOUS: reads the candidate counts of all images (they decide each image's batched_nms strategy,
+ * boxes.py:86) and then the kept counts of all images - two synchronisations of `stream` per call. */
+enum { VB200_SS_RETINANET = 0, VB200_SS_FCOS = 1, VB200_SS_SSD = 2 };
+#define VB200_SS_MAX_TOPK 2048
+VB200_API size_t vb200_single_stage_postprocess_workspace_bytes(int kind, int num_images, int num_levels,
+                                                      const int64_t* level_anchors, int num_classes,
+                                                      int64_t topk_candidates, int64_t detections_per_img);
+VB200_API int vb200_single_stage_postprocess(int kind, int num_images, int num_levels, const int64_t* level_anchors,
+                                   int num_classes, const void* const* logits, const int64_t* logit_strides,
+                                   const void* const* ctrness, const int64_t* ctrness_strides,
+                                   const void* const* regression, const int64_t* regression_strides,
+                                   const void* const* anchors, const int64_t* anchor_strides, const double* image_hw,
+                                   double score_thresh, int64_t topk_candidates, double nms_thresh,
+                                   int64_t detections_per_img, const double* weights, double bbox_xform_clip,
+                                   int semantics, void* workspace, size_t workspace_bytes, void* boxes_out,
+                                   void* scores_out, int64_t* labels_out, int64_t* counts_host, vb200_stream stream);
+
 /* ---- deform_conv2d -----------------------------------------------------
  * Replaces deform_conv2d_forward_kernel, csrc/ops/cuda/deform_conv2d_kernel.cu:1035-1255
  * (schema torchvision::deform_conv2d, csrc/ops/deform_conv2d.cpp:101-102).

@@ -1,6 +1,8 @@
 """Small driver for ncu captures: runs one op of the hot path a few times at its BASELINE shape.
     python tools/prof_ops.py roi_align|roi_pool|ps_roi_align|ps_roi_pool|batched_nms|nms|resize|resize128|resize_noaa|deform|deform_f32|
-                             roi_align_bwd|roi_align_bwd_det|multiscale|postprocess|preprocess [iters]"""
+                             roi_align_bwd|roi_align_bwd_det|multiscale|postprocess|preprocess [iters]
+    python tools/prof_ops.py retinanet_post|fcos_post|ssd_post [iters]     fused vs. reference postprocess_detections,
+                             batch 1 and 8, logits N(-4.595, 1) and N(-4.595, 0.5); select-kernel time from torch.profiler"""
 import os
 import sys
 
@@ -16,6 +18,103 @@ vb._lib.load_ops()
 op = sys.argv[1]
 iters = int(sys.argv[2]) if len(sys.argv) > 2 else 3
 dev = "cuda"
+
+
+def single_stage_post(kind: str, iters: int) -> None:
+    """RetinaNet / FCOS at 800x1088 with 91 classes, SSD300: the fused method against the uninstalled one."""
+    import math
+    import subprocess
+
+    from torch.profiler import ProfilerActivity, profile
+    from torchvision.models.detection import _utils as det_utils
+    from torchvision.models.detection.fcos import FCOS
+    from torchvision.models.detection.retinanet import RetinaNet
+    from torchvision.models.detection.ssd import SSD
+
+    def bare(cls, coder, **a):
+        m = cls.__new__(cls)
+        m.box_coder = coder
+        for k, v in a.items():
+            setattr(m, k, v)
+        return m
+
+    if kind == "retinanet_post":
+        model = bare(RetinaNet, det_utils.BoxCoder(weights=(1.0, 1.0, 1.0, 1.0)), score_thresh=0.05, topk_candidates=1000, nms_thresh=0.5,
+                     detections_per_img=300)
+    elif kind == "fcos_post":
+        model = bare(FCOS, det_utils.BoxLinearCoder(normalize_by_size=True), score_thresh=0.2, topk_candidates=1000, nms_thresh=0.6,
+                     detections_per_img=100)
+    else:
+        model = bare(SSD, det_utils.BoxCoder(weights=(10.0, 10.0, 5.0, 5.0)), score_thresh=0.01, topk_candidates=400, nms_thresh=0.45,
+                     detections_per_img=200)
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+    print(f"{kind}: {gpu.strip().splitlines()[0] if gpu.strip() else 'unknown GPU'}")
+    prior = -math.log((1 - 0.01) / 0.01)
+    for batch in (1, 8):
+        for sd in (1.0, 0.5):
+            gen = torch.Generator(device=dev).manual_seed(0)
+            if kind == "ssd_post":
+                A, C, shapes = 8732, 91, [(300, 300)] * batch
+                levels = [A]
+                head = {"cls_logits": torch.randn(batch, A, C, generator=gen, device=dev) * sd + prior,
+                        "bbox_regression": torch.randn(batch, A, 4, generator=gen, device=dev) * 0.5}
+                anchors = [torch.rand(A, 4, generator=gen, device=dev).cumsum(1) * 100 for _ in shapes]
+                logit_bytes = batch * A * C * 4
+            else:
+                a_loc = 9 if kind == "retinanet_post" else 1
+                levels = [math.ceil(800 / s) * math.ceil(1088 / s) * a_loc for s in (8, 16, 32, 64, 128)]
+                total, C, shapes = sum(levels), 91, [(800, 1088)] * batch
+                cls = torch.randn(batch, total, C, generator=gen, device=dev) * sd + prior
+                reg = torch.randn(batch, total, 4, generator=gen, device=dev) * 0.5
+                head = {"cls_logits": list(cls.split(levels, 1)), "bbox_regression": list(reg.split(levels, 1))}
+                if kind == "fcos_post":
+                    head["bbox_ctrness"] = list(torch.randn(batch, total, 1, generator=gen, device=dev).split(levels, 1))
+                anchors = [list((torch.rand(total, 4, generator=gen, device=dev).cumsum(1) * 200).split(levels)) for _ in shapes]
+                logit_bytes = batch * total * C * 4
+            fn = lambda: type(model).postprocess_detections(model, head, anchors, shapes)
+
+            def timed(n):
+                for _ in range(2):
+                    fn()
+                torch.cuda.synchronize()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for _ in range(n):
+                    fn()
+                e1.record()
+                torch.cuda.synchronize()
+                return e0.elapsed_time(e1) / n
+
+            vb.uninstall()
+            ref_out = fn()
+            t_ref = timed(max(1, iters // 4))
+            vb.install()
+            try:
+                got = fn()
+                t_ours = timed(iters)
+                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                    for _ in range(iters):
+                        fn()
+                    torch.cuda.synchronize()
+            finally:
+                vb.uninstall()
+            sel_us = {}
+            for e in prof.key_averages():
+                for name in ("ss_hist_kernel", "ss_collect_kernel", "ss_final_kernel", "ss_decode_kernel"):
+                    if name in e.key:
+                        sel_us[name] = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / iters
+            passes = sel_us.get("ss_hist_kernel", 0.0) + sel_us.get("ss_collect_kernel", 0.0)
+            bound_us = logit_bytes / 3.35e12 * 1e6
+            same = all(torch.equal(a[k], b[k]) for a, b in zip(ref_out, got) for k in a)
+            kernels = ", ".join(f"{k} {v:.1f} us" for k, v in sel_us.items())
+            print(f"  batch {batch} N({prior:.3f}, {sd}): reference {t_ref:.3f} ms, fused {t_ours:.3f} ms ({t_ref / t_ours:.1f}x); "
+                  f"{kernels}; two logit passes {passes:.1f} us vs one-read HBM bound {bound_us:.1f} us "
+                  f"({bound_us / passes if passes else 0:.0%}); outputs identical: {same}")
+
+
+if op in ("retinanet_post", "fcos_post", "ssd_post"):
+    single_stage_post(op, iters)
+    raise SystemExit(0)
 if op == "roi_align":
     x, r, kw = workloads.cfg2_roi_align()
     x, r = x.to(dev), r.to(dev)

@@ -9,7 +9,8 @@
 3. ``MultiScaleRoIAlign`` (torchvision/ops/poolers.py:147-228): the module-level ``_multiscale_roi_align`` is rebound
    to the fused kernel (device-side LevelMapper + one gather launch over all FPN levels) when the shape is covered.
 4. detection post-processing: ``RoIHeads.postprocess_detections`` and ``RegionProposalNetwork.filter_proposals`` keep their
-   tensor prologue and run the per-image tail (clip, filters, batched_nms, top-k, gathers) as one fused call.
+   tensor prologue and run the per-image tail (clip, filters, batched_nms, top-k, gathers) as one fused call;
+   ``RetinaNet``, ``FCOS`` and ``SSD`` (and so SSDLite) ``postprocess_detections`` run as one fused call for all images.
 5. ``resize`` has no torchvision kernel (transforms/v2/functional/_geometry.py:283-362 calls
    F.interpolate): the entries of ``_KERNEL_REGISTRY[resize]`` for Tensor / Image / Video are swapped.
 CPU tensors and unsupported dtypes/modes keep flowing to the reference implementation.
@@ -90,6 +91,21 @@ def install() -> None:
     tv_roi_heads.RoIHeads.postprocess_detections = postprocess_detections
     tv_rpn.RegionProposalNetwork.filter_proposals = filter_proposals
 
+    # ---- single-stage detectors (retinanet.py:509-571, fcos.py:489-556, ssd.py:414-463) ----
+    from torchvision.models.detection import fcos as tv_fcos, retinanet as tv_retinanet, ssd as tv_ssd
+
+    single_stage = {}
+    for cls, body in ((tv_retinanet.RetinaNet, _det.retinanet_postprocess_detections), (tv_fcos.FCOS, _det.fcos_postprocess_detections),
+                      (tv_ssd.SSD, _det.ssd_postprocess_detections)):
+        orig = cls.postprocess_detections
+
+        def fused(self, head_outputs, anchors, image_shapes, _body=body, _orig=orig):
+            return _body(self, head_outputs, anchors, image_shapes, _orig=_orig)
+
+        functools.update_wrapper(fused, orig)
+        single_stage[cls] = orig
+        cls.postprocess_detections = fused
+
     # ---- ImageClassification preset (transforms/_presets.py:57-64): resize + center_crop + to float + normalize fused ----
     from torchvision.transforms import _presets as tv_presets
 
@@ -123,7 +139,7 @@ def install() -> None:
     _state.update(dict(tv_boxes=tv_boxes, torchvision=torchvision, orig_batched_nms=orig_batched_nms,
                        registry=registry, saved_registry=saved, tv_poolers=tv_poolers, orig_msra=orig_msra,
                        tv_roi_heads=tv_roi_heads, tv_rpn=tv_rpn, orig_pp=orig_pp, orig_fp=orig_fp,
-                       tv_presets=tv_presets, orig_preset_forward=orig_preset_forward))
+                       tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage))
 
 
 def uninstall() -> None:
@@ -136,6 +152,8 @@ def uninstall() -> None:
     _state["tv_presets"].ImageClassification.forward = _state["orig_preset_forward"]
     _state["tv_roi_heads"].RoIHeads.postprocess_detections = _state["orig_pp"]
     _state["tv_rpn"].RegionProposalNetwork.filter_proposals = _state["orig_fp"]
+    for cls, orig in _state["single_stage"].items():
+        cls.postprocess_detections = orig
     reg = _state["registry"]
     reg.clear()
     reg.update(_state["saved_registry"])

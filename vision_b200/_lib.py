@@ -42,7 +42,8 @@ def core() -> ctypes.CDLL:
             for name in ("vb200_nms_workspace_bytes", "vb200_batched_nms_workspace_bytes",
                          "vb200_roi_align_workspace_bytes", "vb200_deform_conv2d_workspace_bytes",
                          "vb200_roi_backward_workspace_bytes", "vb200_multiscale_roi_align_workspace_bytes",
-                         "vb200_detection_postprocess_workspace_bytes", "vb200_deform_conv2d_packed_weight_bytes"):
+                         "vb200_detection_postprocess_workspace_bytes", "vb200_deform_conv2d_packed_weight_bytes",
+                         "vb200_single_stage_postprocess_workspace_bytes"):
                 getattr(lib, name).restype = ctypes.c_size_t
             _core = lib
         return _core
@@ -77,4 +78,5 @@ ABI_SYMBOLS = (
     "vb200_deform_conv2d_sample_columns", "vb200_deform_conv2d_backward_inputs", "vb200_ps_roi_pool_forward", "vb200_ps_roi_pool_backward", "vb200_box_iou_rotated", "vb200_resize_crop_normalize", "vb200_detection_postprocess_workspace_bytes", "vb200_detection_postprocess",
     "vb200_multiscale_roi_align_workspace_bytes", "vb200_multiscale_roi_align_supported", "vb200_multiscale_roi_align_forward",
     "vb200_roi_backward_workspace_bytes", "vb200_roi_align_backward", "vb200_roi_pool_backward", "vb200_ps_roi_align_backward",
+    "vb200_single_stage_postprocess_workspace_bytes", "vb200_single_stage_postprocess",
 )

@@ -25,6 +25,7 @@
 #include <cmath>
 #include <cstring>
 #include <mutex>
+#include <vector>
 
 #include "common.cuh"
 
@@ -1185,4 +1186,531 @@ extern "C" int vb200_detection_postprocess(const void* boxes, const void* scores
   }
   set_error("detection_postprocess: internal error (negative kept count)");
   return VB200_EINVAL;
+}
+
+// =====================================================================================================================
+// Single-stage detector post-processing: RetinaNet (retinanet.py:509-571), FCOS (fcos.py:489-556), SSD / SSDLite
+// (ssd.py:414-463).  The reference loops over images and FPN levels (or foreground classes), writes a full score tensor
+// and a full mask per level, compacts them and takes a topk - ~180 host synchronisations per SSD image.  Here every
+// segment - an (image, level) slice of logits or an (image, class) column of probabilities - of every image is
+// selected by one radix-select pipeline over the logits, read twice:
+//   ss_hist_kernel     (read 1) per-segment histogram of the top 12 bits of key = bits(score) - bits(next float above
+//                      the threshold).  Scores lie in [0, 1], so the key orders them and spans exactly the passing range
+//                      (threshold, 1]: at a threshold of 0.05 the 4096 bins cover 2^14 ulps each (the top bits of the raw
+//                      pattern would put all of (0.05, 1] into 37 bins);
+//   ss_bound_kernel    boundary bucket B of each segment: fewer than k items lie above it, at least k at or above it;
+//   ss_collect_kernel  (read 2) items above B are in the result; items in B are kept as (key, reversed index) pairs;
+//   ss_final_kernel    one CTA per segment sorts the <= 4096 pairs (their significant bits only) by (score desc,
+//                      index asc) and keeps the first k.
+//                      When bucket B alone holds more items than fit, this CTA narrows it 12 bits at a time by
+//                      re-reading its segment (the pairs are unique, so this ends) - only for such degenerate segments;
+//   ss_decode_kernel   decode + clip of the selected items into each image's candidate list, in the reference's order.
+// The per-image tail is bnms_core + det_gather_topk_kernel above; one concatenation kernel packs the images' results.
+// Host synchronisations: two per call (candidate counts of all images, kept counts of all images).
+// =====================================================================================================================
+namespace vb200 {
+namespace {
+
+constexpr int kSelThreads = 256;
+constexpr int kSelTile = 8192;                  // elements of one segment per CTA of the two passes over the logits
+constexpr int kSelBits = 12;
+constexpr int kSelBins = 1 << kSelBits;
+constexpr int kSelSortThreads = 512, kSelSortItems = 8;
+constexpr int kSelSortCap = kSelSortThreads * kSelSortItems;     // pairs sorted by one CTA
+static_assert(2 * VB200_SS_MAX_TOPK <= kSelSortCap, "the boundary list needs at least as much room as the top-k");
+
+struct SsSeg {                 // one segment
+  const float* logit;          // element i: logit[(i / C) * lstride + i % C] (RetinaNet, FCOS), logit[i * lstride] (SSD)
+  const float* ctr;            // FCOS: ctrness of anchor row a at ctr[a * cstride]
+  const float* reg;            // regression row a at reg[a * rstride .. + 3]
+  const float* anc;            // anchor row a at anc[a * astride .. + 3]
+  int64_t n, lstride, cstride, rstride, astride;
+  int label;                   // SSD: the class of this column
+  float img_h, img_w;
+};
+
+struct SsParams {
+  int kind, C;
+  float thr;                   // float(score_thresh): the reference compares `scores > score_thresh` in fp32
+  uint32_t base;               // bit pattern of the smallest passing score: key = bits(score) - base
+  int shift0;                  // first digit = key >> shift0
+  int ib;                      // pair = key << ib | (imask - index): ib bits hold any index of the largest segment
+  unsigned long long imask;
+  int sort_bits;               // significant bits of a pair
+  int k, cap, spi, nmax;       // per-segment top-k, boundary-list capacity, segments per image, candidates per image
+  float inv_w[4], clip;        // 1.0f / weight (torch divides a tensor by a Python float as a multiply by its reciprocal)
+};
+
+__device__ __forceinline__ float ss_sigmoid(float x) { return div_rn(1.f, add_rn(1.f, expf(-x))); }   // torch.sigmoid (fp32)
+
+// Sigmoid, its square root and softmax probabilities lie in [+0, 1]; the clamp (NaN kept) only guarantees that every key
+// of a passing score is at most bits(1.0f) - base, whatever the input holds.
+__device__ __forceinline__ float ss_unit(float s) { return s > 1.f ? 1.f : (s <= 0.f ? 0.f : s); }
+
+// Calls f(i, score) for i = i0 + t, i0 + t + stride, ... < i1 of segment g; four loads are issued before any use.
+template <typename F>
+__device__ __forceinline__ void ss_walk(const SsSeg& g, const SsParams& p, int64_t i0, int64_t i1, int t, int stride, F&& f) {
+  constexpr int U = 4;
+  if (p.kind == VB200_SS_SSD) {
+    for (int64_t ib = i0 + t; ib < i1; ib += (int64_t)U * stride) {
+      float x[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int64_t i = ib + (int64_t)u * stride;
+        x[u] = i < i1 ? __ldg(g.logit + i * g.lstride) : 0.f;
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u)
+        if (ib + (int64_t)u * stride < i1) f(ib + (int64_t)u * stride, ss_unit(x[u]));
+    }
+    return;
+  }
+  // (anchor row, class) of the current index, advanced by `stride` elements per step
+  const int C = p.C, sa = stride / C, sc = stride % C;
+  int64_t a = (i0 + t) / C;
+  int c = (int)(i0 + t - a * C);
+  for (int64_t ib = i0 + t; ib < i1; ib += (int64_t)U * stride) {
+    float x[U], y[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const bool in = ib + (int64_t)u * stride < i1;
+      x[u] = in ? __ldg(g.logit + a * g.lstride + c) : 0.f;
+      y[u] = (in && p.kind == VB200_SS_FCOS) ? __ldg(g.ctr + a * g.cstride) : 0.f;
+      a += sa; c += sc;
+      if (c >= C) { c -= C; ++a; }
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      if (ib + (int64_t)u * stride >= i1) break;
+      float s = ss_sigmoid(x[u]);
+      if (p.kind == VB200_SS_FCOS) s = __fsqrt_rn(mul_rn(s, ss_sigmoid(y[u])));    // fcos.py:516-518
+      f(ib + (int64_t)u * stride, ss_unit(s));
+    }
+  }
+}
+
+// key of a passing score (s > thr, so bits(s) >= base)
+__device__ __forceinline__ uint32_t ss_key(float s, const SsParams& p) { return __float_as_uint(s) - p.base; }
+// (key, reversed index): descending order of the pair is score descending, then index ascending
+__device__ __forceinline__ unsigned long long ss_pair(float s, int64_t i, const SsParams& p) {
+  return ((unsigned long long)ss_key(s, p) << p.ib) | (p.imask - (unsigned long long)i);
+}
+
+__device__ __forceinline__ int ss_tile_segment(const int* __restrict__ tile_off, int nseg, int b, int64_t& i0) {
+  const int g = find_segment(tile_off, nseg, b);
+  i0 = (int64_t)(b - __ldg(tile_off + g)) * kSelTile;
+  return g;
+}
+
+__global__ void __launch_bounds__(kSelThreads) ss_hist_kernel(const SsSeg* __restrict__ segs, const int* __restrict__ tile_off,
+                                                             int nseg, SsParams p, int* __restrict__ hist) {
+  __shared__ int h[kSelBins];
+  for (int b = threadIdx.x; b < kSelBins; b += kSelThreads) h[b] = 0;
+  int64_t i0;
+  const int g = ss_tile_segment(tile_off, nseg, blockIdx.x, i0);
+  const SsSeg sg = segs[g];
+  __syncthreads();
+  ss_walk(sg, p, i0, min(sg.n, i0 + kSelTile), threadIdx.x, kSelThreads, [&](int64_t, float s) {
+    if (s > p.thr) atomicAdd(&h[ss_key(s, p) >> p.shift0], 1);
+  });
+  __syncthreads();
+  int* gh = hist + (size_t)g * kSelBins;
+  for (int b = threadIdx.x; b < kSelBins; b += kSelThreads)
+    if (h[b]) atomicAdd(gh + b, h[b]);
+}
+
+struct SsState {
+  int B;           // boundary bucket, -1: every passing item is selected
+  int n_bnd;       // items in bucket B
+  int total;       // passing items
+  int n_sure, n_list;   // pairs collected above B / in B
+  int pad[3];
+};
+
+__global__ void __launch_bounds__(kSelThreads) ss_bound_kernel(const int* __restrict__ hist, SsParams p, SsState* __restrict__ st) {
+  constexpr int per = kSelBins / kSelThreads;
+  using Scan = cub::BlockScan<int, kSelThreads>;
+  __shared__ typename Scan::TempStorage ts;
+  const int g = blockIdx.x, hi = kSelBins - (int)threadIdx.x * per;     // thread 0 owns the top bins
+  const int* h = hist + (size_t)g * kSelBins;
+  int v[per], sum = 0;
+#pragma unroll
+  for (int j = 0; j < per; ++j) { v[j] = h[hi - 1 - j]; sum += v[j]; }
+  int above, total;
+  Scan(ts).ExclusiveSum(sum, above, total);
+  if (threadIdx.x == 0) {
+    st[g].total = total; st[g].n_sure = 0; st[g].n_list = 0;
+    if (total <= p.k) { st[g].B = -1; st[g].n_bnd = 0; }
+  }
+  if (total > p.k) {
+#pragma unroll
+    for (int j = 0; j < per; ++j) {
+      if (above < p.k && above + v[j] >= p.k) { st[g].B = hi - 1 - j; st[g].n_bnd = v[j]; }
+      above += v[j];
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kSelThreads) ss_collect_kernel(const SsSeg* __restrict__ segs, const int* __restrict__ tile_off,
+                                                                int nseg, SsParams p, SsState* __restrict__ st,
+                                                                unsigned long long* __restrict__ sure, unsigned long long* __restrict__ list) {
+  int64_t i0;
+  const int g = ss_tile_segment(tile_off, nseg, blockIdx.x, i0);
+  const SsSeg sg = segs[g];
+  const int B = st[g].B;
+  const bool take_list = B >= 0 && st[g].n_bnd <= p.cap;       // otherwise ss_final_kernel narrows the bucket
+  ss_walk(sg, p, i0, min(sg.n, i0 + kSelTile), threadIdx.x, kSelThreads, [&](int64_t i, float s) {
+    if (!(s > p.thr)) return;
+    const int d = (int)(ss_key(s, p) >> p.shift0);
+    if (d > B) sure[(size_t)g * p.k + atomicAdd(&st[g].n_sure, 1)] = ss_pair(s, i, p);
+    else if (d == B && take_list) list[(size_t)g * p.cap + atomicAdd(&st[g].n_list, 1)] = ss_pair(s, i, p);
+  });
+}
+
+__global__ void __launch_bounds__(kSelSortThreads) ss_final_kernel(const SsSeg* __restrict__ segs, SsParams p, SsState* __restrict__ st,
+                                                                  unsigned long long* __restrict__ sure, unsigned long long* __restrict__ list,
+                                                                  unsigned long long* __restrict__ sel, int* __restrict__ sel_n) {
+  using Sort = cub::BlockRadixSort<unsigned long long, kSelSortThreads, kSelSortItems>;
+  __shared__ union { typename Sort::TempStorage sort; int hist[kSelBins]; } sm;
+  __shared__ int s_sure, s_list, s_digit, s_above, s_count;
+  const int g = blockIdx.x, t = threadIdx.x;
+  const SsState S = st[g];
+  unsigned long long* gs = sure + (size_t)g * p.k;
+  unsigned long long* gl = list + (size_t)g * p.cap;
+  if (t == 0) { s_sure = S.n_sure; s_list = S.n_list; }
+  if (S.B >= 0 && S.n_bnd > p.cap) {
+    // degenerate segment: narrow the boundary prefix 12 bits at a time over the (key, ~index) pair
+    const SsSeg sg = segs[g];
+    unsigned long long P = (unsigned long long)S.B;
+    int pos = p.ib + p.shift0, need = p.k - S.n_sure, count = S.n_bnd;
+    __syncthreads();
+    while (count > p.cap) {
+      const int npos = max(pos - kSelBits, 0), w = pos - npos;
+      const unsigned long long mask = (1ull << w) - 1ull;
+      for (int b = t; b < kSelBins; b += kSelSortThreads) sm.hist[b] = 0;
+      __syncthreads();
+      ss_walk(sg, p, 0, sg.n, t, kSelSortThreads, [&](int64_t i, float s) {
+        if (!(s > p.thr)) return;
+        const unsigned long long q = ss_pair(s, i, p);
+        if ((q >> pos) == P) atomicAdd(&sm.hist[(q >> npos) & mask], 1);
+      });
+      __syncthreads();
+      if (t == 0) {
+        int run = 0;
+        for (int b = (int)mask; b >= 0; --b) {
+          if (run + sm.hist[b] >= need) { s_digit = b; s_above = run; s_count = sm.hist[b]; break; }
+          run += sm.hist[b];
+        }
+      }
+      __syncthreads();
+      const unsigned long long D = (unsigned long long)s_digit;
+      ss_walk(sg, p, 0, sg.n, t, kSelSortThreads, [&](int64_t i, float s) {
+        if (!(s > p.thr)) return;
+        const unsigned long long q = ss_pair(s, i, p);
+        if ((q >> pos) == P && ((q >> npos) & mask) > D) gs[atomicAdd(&s_sure, 1)] = q;
+      });
+      need -= s_above;
+      count = s_count;
+      P = (P << w) | D;
+      pos = npos;
+      __syncthreads();
+    }
+    ss_walk(sg, p, 0, sg.n, t, kSelSortThreads, [&](int64_t i, float s) {
+      if (!(s > p.thr)) return;
+      const unsigned long long q = ss_pair(s, i, p);
+      if ((q >> pos) == P) gl[atomicAdd(&s_list, 1)] = q;
+    });
+  }
+  __syncthreads();
+  const int ns = s_sure, nl = s_list;
+  unsigned long long keys[kSelSortItems];
+#pragma unroll
+  for (int j = 0; j < kSelSortItems; ++j) {
+    const int r = t * kSelSortItems + j;
+    keys[j] = r < ns ? gs[r] : (r - ns < nl ? gl[r - ns] : 0ull);      // 0 sorts after every real pair
+  }
+  __syncthreads();
+  Sort(sm.sort).SortDescending(keys, 0, p.sort_bits);
+  const int m = min(p.k, S.total);
+#pragma unroll
+  for (int j = 0; j < kSelSortItems; ++j) {
+    const int r = t * kSelSortItems + j;
+    if (r < m) sel[(size_t)g * p.k + r] = keys[j];
+  }
+  if (t == 0) sel_n[g] = m;
+}
+
+// Decode + clip of the selected items.  Segment g of image g / spi lands after the items of the image's earlier segments
+// (retinanet.py:555-557 concatenates the levels in order; ssd.py:448-450 the classes).
+__global__ void ss_decode_kernel(const SsSeg* __restrict__ segs, SsParams p, const unsigned long long* __restrict__ sel,
+                                 const int* __restrict__ sel_n, float4* __restrict__ cb, float* __restrict__ cs, int64_t* __restrict__ cl,
+                                 int* __restrict__ n_img) {
+  const int per = ceil_div(p.k, (int)blockDim.x);          // blocks per segment
+  const int g = blockIdx.x / per, j = (blockIdx.x % per) * blockDim.x + threadIdx.x;
+  const int img = g / p.spi, g0 = img * p.spi;
+  const int m = sel_n[g];
+  const bool last = g == g0 + p.spi - 1 && j == 0;
+  if (j >= m && !last) return;
+  int off = 0;
+  for (int q = g0; q < g; ++q) off += sel_n[q];
+  if (last) n_img[img] = off + m;
+  if (j >= m) return;
+  const unsigned long long q = sel[(size_t)g * p.k + j];
+  const float s = __uint_as_float((uint32_t)(q >> p.ib) + p.base);
+  const uint32_t i = (uint32_t)(p.imask - (q & p.imask));
+  const SsSeg sg = segs[g];
+  int64_t a, label;
+  if (p.kind == VB200_SS_SSD) { a = i; label = sg.label; }
+  else { a = i / (uint32_t)p.C; label = i % (uint32_t)p.C; }     // retinanet.py:543-544
+  const float* r = sg.reg + a * sg.rstride;
+  const float* an = sg.anc + a * sg.astride;
+  const float x0 = an[0], y0 = an[1], x1 = an[2], y1 = an[3];
+  const float r0 = r[0], r1 = r[1], r2 = r[2], r3 = r[3];
+  float4 b;
+  if (p.kind == VB200_SS_FCOS) {
+    // BoxLinearCoder.decode, normalize_by_size=True (_utils.py:292-310)
+    const float cx = mul_rn(0.5f, add_rn(x0, x1)), cy = mul_rn(0.5f, add_rn(y0, y1));
+    const float w = sub_rn(x1, x0), h = sub_rn(y1, y0);
+    b = make_float4(sub_rn(cx, mul_rn(r0, w)), sub_rn(cy, mul_rn(r1, h)), add_rn(cx, mul_rn(r2, w)), add_rn(cy, mul_rn(r3, h)));
+  } else {
+    // BoxCoder.decode_single (_utils.py:193-224): every tensor op rounded on its own
+    const float w = sub_rn(x1, x0), h = sub_rn(y1, y0);
+    const float cx = add_rn(x0, mul_rn(0.5f, w)), cy = add_rn(y0, mul_rn(0.5f, h));
+    const float dx = mul_rn(r0, p.inv_w[0]), dy = mul_rn(r1, p.inv_w[1]);
+    float dw = mul_rn(r2, p.inv_w[2]), dh = mul_rn(r3, p.inv_w[3]);
+    dw = isnan(dw) ? dw : fminf(dw, p.clip);                      // torch.clamp(max=...) propagates NaN
+    dh = isnan(dh) ? dh : fminf(dh, p.clip);
+    const float pcx = add_rn(mul_rn(dx, w), cx), pcy = add_rn(mul_rn(dy, h), cy);
+    const float hw = mul_rn(0.5f, mul_rn(expf(dw), w)), hh = mul_rn(0.5f, mul_rn(expf(dh), h));
+    b = make_float4(sub_rn(pcx, hw), sub_rn(pcy, hh), add_rn(pcx, hw), add_rn(pcy, hh));
+  }
+  // clip_boxes_to_image, as det_clip_filter_kernel
+  b.x = fminf(fmaxf(b.x, 0.f), sg.img_w); b.z = fminf(fmaxf(b.z, 0.f), sg.img_w);
+  b.y = fminf(fmaxf(b.y, 0.f), sg.img_h); b.w = fminf(fmaxf(b.w, 0.f), sg.img_h);
+  const size_t o = (size_t)img * p.nmax + off + j;
+  cb[o] = b; cs[o] = s; cl[o] = label;
+}
+
+// image results at slot img * D -> packed one after another
+__global__ void ss_concat_kernel(const float4* __restrict__ pb, const float* __restrict__ ps, const int64_t* __restrict__ pl,
+                                 const int64_t* __restrict__ counts, int64_t D, float4* __restrict__ ob, float* __restrict__ os,
+                                 int64_t* __restrict__ ol, int per) {
+  const int img = blockIdx.x / per;
+  const int64_t j = (int64_t)(blockIdx.x % per) * blockDim.x + threadIdx.x;
+  if (j >= counts[img]) return;
+  int64_t off = 0;
+  for (int q = 0; q < img; ++q) off += counts[q];
+  const int64_t src = (int64_t)img * D + j;
+  ob[off + j] = pb[src]; os[off + j] = ps[src]; ol[off + j] = pl[src];
+}
+
+struct SsWs {
+  SsSeg* segs; int* tile_off; int* hist; SsState* st; unsigned long long* sure; unsigned long long* list;
+  unsigned long long* sel; int* sel_n; float4* cb; float* cs; int64_t* cl; int* n_img; int64_t* keep; int64_t* num_keep;
+  float4* pb; float* ps; int64_t* pl; int64_t* counts; size_t bnms_off; size_t total;
+};
+
+// nmax candidates per image; the batched_nms workspace must hold any n <= nmax, and it shrinks where the plain-nms
+// matrix leaves it (n above the coordinate-trick range), so both ends of that range are considered.
+SsWs carve_ss(void* base, int N, int nseg, int k, int cap, int64_t nmax, int64_t D) {
+  Carver c(base);
+  SsWs w;
+  w.segs = c.take<SsSeg>(nseg);
+  w.tile_off = c.take<int>(nseg + 1);
+  w.hist = c.take<int>((size_t)nseg * kSelBins);
+  w.st = c.take<SsState>(nseg);
+  w.sure = c.take<unsigned long long>((size_t)nseg * k);
+  w.list = c.take<unsigned long long>((size_t)nseg * cap);
+  w.sel = c.take<unsigned long long>((size_t)nseg * k);
+  w.sel_n = c.take<int>(nseg);
+  w.cb = c.take<float4>((size_t)N * nmax);
+  w.cs = c.take<float>((size_t)N * nmax);
+  w.cl = c.take<int64_t>((size_t)N * nmax);
+  w.n_img = c.take<int>(N);
+  w.keep = c.take<int64_t>(nmax);
+  w.num_keep = c.take<int64_t>(32);
+  w.pb = c.take<float4>((size_t)N * D);
+  w.ps = c.take<float>((size_t)N * D);
+  w.pl = c.take<int64_t>((size_t)N * D);
+  w.counts = c.take<int64_t>(N);
+  w.bnms_off = c.off;
+  size_t bn = 0;
+  if (nmax > 0) {
+    bn = carve_bnms(nullptr, nmax).total;
+    const int64_t n_trick = nmax < 25000 ? nmax : 25000;
+    const size_t bt = carve_bnms(nullptr, n_trick).total;
+    bn = bt > bn ? bt : bn;
+  }
+  c.off += bn;
+  w.total = c.off;
+  return w;
+}
+
+struct SsShape { int nseg, spi; int64_t tiles; int k, cap; int64_t nmax; };
+SsShape ss_shape(int kind, int N, int L, const int64_t* level_anchors, int C, int64_t topk) {
+  SsShape s;
+  s.spi = kind == VB200_SS_SSD ? C - 1 : L;
+  s.nseg = N * s.spi;
+  s.k = (int)topk;
+  s.cap = kSelSortCap - s.k;
+  s.nmax = (int64_t)s.spi * s.k;
+  int64_t per_image = 0;
+  if (kind == VB200_SS_SSD) per_image = (int64_t)(C - 1) * ceil_div64(level_anchors[0], kSelTile);
+  else for (int l = 0; l < L; ++l) per_image += ceil_div64(level_anchors[l] * C, kSelTile);
+  s.tiles = per_image * N;
+  return s;
+}
+}  // namespace
+}  // namespace vb200
+
+extern "C" size_t vb200_single_stage_postprocess_workspace_bytes(int kind, int num_images, int num_levels, const int64_t* level_anchors,
+                                                                 int num_classes, int64_t topk_candidates, int64_t detections_per_img) {
+  if (num_images <= 0 || num_levels <= 0 || !level_anchors || num_classes < 1 || topk_candidates <= 0 ||
+      topk_candidates > VB200_SS_MAX_TOPK || detections_per_img <= 0)
+    return 0;
+  const SsShape s = ss_shape(kind, num_images, num_levels, level_anchors, num_classes, topk_candidates);
+  if (s.nseg <= 0) return 0;
+  return carve_ss(nullptr, num_images, s.nseg, s.k, s.cap, s.nmax, detections_per_img).total;
+}
+
+extern "C" int vb200_single_stage_postprocess(int kind, int num_images, int num_levels, const int64_t* level_anchors, int num_classes,
+                                              const void* const* logits, const int64_t* logit_strides, const void* const* ctrness,
+                                              const int64_t* ctrness_strides, const void* const* regression,
+                                              const int64_t* regression_strides, const void* const* anchors, const int64_t* anchor_strides,
+                                              const double* image_hw, double score_thresh, int64_t topk_candidates, double nms_thresh,
+                                              int64_t detections_per_img, const double* weights, double bbox_xform_clip, int semantics,
+                                              void* workspace, size_t workspace_bytes, void* boxes_out, void* scores_out,
+                                              int64_t* labels_out, int64_t* counts_host, vb200_stream stream) {
+  VB200_REQUIRE(kind == VB200_SS_RETINANET || kind == VB200_SS_FCOS || kind == VB200_SS_SSD, "single_stage_postprocess: bad kind %d", kind);
+  VB200_REQUIRE(num_images >= 0 && num_levels >= 1 && num_levels <= 64 && (kind != VB200_SS_SSD || num_levels == 1),
+                "single_stage_postprocess: bad image / level count");
+  VB200_REQUIRE(num_classes >= 1 && topk_candidates >= 0 && topk_candidates <= VB200_SS_MAX_TOPK && detections_per_img >= 0,
+                "single_stage_postprocess: bad sizes (topk_candidates must be <= %d)", VB200_SS_MAX_TOPK);
+  VB200_REQUIRE(semantics == VB200_NMS_CPU || semantics == VB200_NMS_CUDA, "single_stage_postprocess: bad semantics selector");
+  VB200_REQUIRE(counts_host != nullptr, "single_stage_postprocess: null counts_host");
+  for (int i = 0; i < num_images; ++i) counts_host[i] = 0;
+  if (num_images == 0 || topk_candidates == 0 || detections_per_img == 0 || (kind == VB200_SS_SSD && num_classes < 2)) return 0;
+  VB200_REQUIRE(level_anchors && logits && logit_strides && regression && regression_strides && anchors && anchor_strides && image_hw &&
+                    weights && workspace && boxes_out && scores_out && labels_out,
+                "single_stage_postprocess: null pointer");
+  VB200_REQUIRE(kind != VB200_SS_FCOS || (ctrness && ctrness_strides), "single_stage_postprocess: FCOS needs ctrness");
+  const int N = num_images, L = num_levels, C = num_classes;
+  const SsShape sh = ss_shape(kind, N, L, level_anchors, C, topk_candidates);
+  VB200_REQUIRE(sh.tiles < (1ll << 31) && (int64_t)sh.nseg * ceil_div(sh.k, 128) < (1ll << 31), "single_stage_postprocess: too many segments");
+  const SsWs w = carve_ss(workspace, N, sh.nseg, sh.k, sh.cap, sh.nmax, detections_per_img);
+  if (workspace_bytes < w.total) {
+    set_error("single_stage_postprocess: workspace too small (%zu < %zu)", workspace_bytes, w.total);
+    return VB200_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+
+  // segment table (image-major) and the first tile of every segment
+  std::vector<SsSeg> segs((size_t)sh.nseg);
+  std::vector<int> tile_off((size_t)sh.nseg + 1);
+  int64_t tiles = 0, widest_seg = 1;
+  for (int img = 0; img < N; ++img) {
+    for (int q = 0; q < sh.spi; ++q) {
+      const int l = kind == VB200_SS_SSD ? 0 : q;
+      const int64_t A = level_anchors[l];
+      VB200_REQUIRE(A >= 0 && A * C < (1ll << 31), "single_stage_postprocess: a segment must have fewer than 2^31 elements");
+      SsSeg g;
+      const float* lg = (const float*)logits[l] + img * logit_strides[2 * l];
+      g.logit = kind == VB200_SS_SSD ? lg + (q + 1) : lg;
+      g.lstride = logit_strides[2 * l + 1];
+      g.ctr = kind == VB200_SS_FCOS ? (const float*)ctrness[l] + img * ctrness_strides[2 * l] : nullptr;
+      g.cstride = kind == VB200_SS_FCOS ? ctrness_strides[2 * l + 1] : 0;
+      g.reg = (const float*)regression[l] + img * regression_strides[2 * l];
+      g.rstride = regression_strides[2 * l + 1];
+      g.anc = (const float*)anchors[(size_t)img * L + l];
+      g.astride = anchor_strides[(size_t)img * L + l];
+      g.n = kind == VB200_SS_SSD ? A : A * C;
+      g.label = q + 1;
+      g.img_h = (float)image_hw[2 * img];
+      g.img_w = (float)image_hw[2 * img + 1];
+      segs[(size_t)img * sh.spi + q] = g;
+      tile_off[(size_t)img * sh.spi + q] = (int)tiles;
+      tiles += ceil_div64(g.n, kSelTile);
+      widest_seg = g.n > widest_seg ? g.n : widest_seg;
+    }
+  }
+  tile_off[sh.nseg] = (int)tiles;
+
+  SsParams p;
+  p.kind = kind;
+  p.C = C;
+  p.thr = (float)score_thresh;
+  // Smallest passing bit pattern.  Scores lie in [+0, 1] (ss_unit), so for thr < 0 every score passes (base 0), and a
+  // threshold of +0 or -0 passes every positive score (base = bits(+0) + 1).  A NaN threshold passes nothing.
+  const float athr = fabsf(p.thr);
+  uint32_t tb;
+  memcpy(&tb, &athr, 4);
+  p.base = (p.thr != p.thr || p.thr < 0.f) ? 0u : tb + 1u;
+  const uint32_t one = 0x3f800000u;                       // bits(1.0f): keys of passing scores are <= one - base
+  const uint32_t max_key = p.base <= one ? one - p.base : 0u;
+  int bits = 0;
+  while (bits < 32 && (max_key >> bits) != 0u) ++bits;
+  p.shift0 = bits > kSelBits ? bits - kSelBits : 0;
+  p.ib = 1;
+  while ((1ll << p.ib) < widest_seg) ++p.ib;
+  p.imask = (1ull << p.ib) - 1ull;
+  p.sort_bits = bits + p.ib;
+  p.k = sh.k;
+  p.cap = sh.cap;
+  p.spi = sh.spi;
+  p.nmax = (int)sh.nmax;
+  for (int j = 0; j < 4; ++j) p.inv_w[j] = 1.0f / (float)weights[j];
+  p.clip = (float)bbox_xform_clip;
+
+  VB200_CUDA_TRY(cudaMemcpyAsync(w.segs, segs.data(), segs.size() * sizeof(SsSeg), cudaMemcpyHostToDevice, st));
+  VB200_CUDA_TRY(cudaMemcpyAsync(w.tile_off, tile_off.data(), tile_off.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  VB200_CUDA_TRY(cudaMemsetAsync(w.hist, 0, (size_t)sh.nseg * kSelBins * sizeof(int), st));
+  VB200_CUDA_TRY(cudaMemsetAsync(w.counts, 0, (size_t)N * sizeof(int64_t), st));
+  int rc = 0;
+  if (tiles > 0) {
+    ss_hist_kernel<<<(unsigned)tiles, kSelThreads, 0, st>>>(w.segs, w.tile_off, sh.nseg, p, w.hist);
+    if ((rc = check_launch("ss_hist_kernel"))) return rc;
+  }
+  ss_bound_kernel<<<sh.nseg, kSelThreads, 0, st>>>(w.hist, p, w.st);
+  if ((rc = check_launch("ss_bound_kernel"))) return rc;
+  if (tiles > 0) {
+    ss_collect_kernel<<<(unsigned)tiles, kSelThreads, 0, st>>>(w.segs, w.tile_off, sh.nseg, p, w.st, w.sure, w.list);
+    if ((rc = check_launch("ss_collect_kernel"))) return rc;
+  }
+  ss_final_kernel<<<sh.nseg, kSelSortThreads, 0, st>>>(w.segs, p, w.st, w.sure, w.list, w.sel, w.sel_n);
+  if ((rc = check_launch("ss_final_kernel"))) return rc;
+  ss_decode_kernel<<<sh.nseg * ceil_div(sh.k, 128), 128, 0, st>>>(w.segs, p, w.sel, w.sel_n, w.cb, w.cs, w.cl, w.n_img);
+  if ((rc = check_launch("ss_decode_kernel"))) return rc;
+
+  // host read 1: every image's candidate count (the batched_nms strategy switch, boxes.py:86, looks at it)
+  std::vector<int> n_img((size_t)N);
+  VB200_CUDA_TRY(cudaMemcpyAsync(n_img.data(), w.n_img, (size_t)N * sizeof(int), cudaMemcpyDeviceToHost, st));
+  VB200_CUDA_TRY(cudaStreamSynchronize(st));
+  const bool wide_keys = C > 65536;     // labels < C fit the 16-bit class keys otherwise
+  const int blk = 256;
+  for (int img = 0; img < N; ++img) {
+    const int64_t n = n_img[img];
+    if (n == 0) continue;
+    const size_t o = (size_t)img * sh.nmax;
+    rc = bnms_core<float>(w.cb + o, w.cs + o, w.cl + o, n, nms_thresh, semantics, VB200_BNMS_AUTO, wide_keys,
+                          (char*)workspace + w.bnms_off, workspace_bytes - w.bnms_off, w.keep, w.num_keep, st);
+    if (rc) return rc;
+    const int64_t cap = detections_per_img < n ? detections_per_img : n;
+    det_gather_topk_kernel<<<ceil_div((int)cap, blk), blk, 0, st>>>(w.cb + o, w.cs + o, w.cl + o, w.keep, w.num_keep, detections_per_img,
+                                                                   w.pb + (size_t)img * detections_per_img, w.ps + (size_t)img * detections_per_img,
+                                                                   w.pl + (size_t)img * detections_per_img, w.counts + img);
+    if ((rc = check_launch("det_gather_topk_kernel"))) return rc;
+  }
+  // host read 2: every image's kept count
+  VB200_CUDA_TRY(cudaMemcpyAsync(counts_host, w.counts, (size_t)N * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  VB200_CUDA_TRY(cudaStreamSynchronize(st));
+  int64_t widest = 0;
+  for (int img = 0; img < N; ++img) {
+    VB200_REQUIRE(counts_host[img] >= 0, "single_stage_postprocess: internal error (negative kept count)");
+    widest = counts_host[img] > widest ? counts_host[img] : widest;
+  }
+  if (widest == 0) return 0;
+  const int per = ceil_div((int)widest, blk);
+  ss_concat_kernel<<<(unsigned)((int64_t)N * per), blk, 0, st>>>(w.pb, w.ps, w.pl, w.counts, detections_per_img, (float4*)boxes_out,
+                                                                 (float*)scores_out, labels_out, per);
+  return check_launch("ss_concat_kernel");
 }

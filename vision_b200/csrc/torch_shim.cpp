@@ -410,6 +410,70 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> detection_postprocess(const at::T
   return std::make_tuple(ob.narrow(0, 0, count), os.narrow(0, 0, count), ol.narrow(0, 0, count));
 }
 
+// ---- single-stage detector post-processing (retinanet.py:509-571, fcos.py:489-556, ssd.py:414-463) -----------------
+// logits / ctrness / regression: one [N, A_l, *] tensor per level (views split from [N, sum A, *] are taken as they are: any
+// image and row stride, dense last dimension); anchors: N * L tensors [A_l, 4], image-major; image_sizes: N (h, w) pairs.
+// Returns the detections of all images concatenated plus a host int64 tensor of per-image counts.
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> single_stage_postprocess(
+    int64_t kind, at::TensorList logits, at::TensorList ctrness, at::TensorList regression, at::TensorList anchors,
+    at::IntArrayRef image_sizes, double score_thresh, int64_t topk_candidates, double nms_thresh, int64_t detections_per_img,
+    at::ArrayRef<double> weights, double bbox_xform_clip) {
+  const int64_t L = (int64_t)logits.size();
+  TORCH_CHECK(L >= 1 && L <= 64 && (int64_t)regression.size() == L, "single_stage_postprocess: 1..64 levels, one regression tensor each");
+  TORCH_CHECK(kind != VB200_SS_FCOS || (int64_t)ctrness.size() == L, "single_stage_postprocess: FCOS needs one ctrness tensor per level");
+  TORCH_CHECK(kind != VB200_SS_SSD || L == 1, "single_stage_postprocess: SSD takes one [N, A, C] probability tensor");
+  TORCH_CHECK(weights.size() == 4, "single_stage_postprocess: 4 box coder weights");
+  const at::Tensor& l0 = logits[0];
+  TORCH_CHECK(l0.dim() == 3, "single_stage_postprocess: logits must be [N, A, C]");
+  const int64_t N = l0.size(0), C = l0.size(2);
+  TORCH_CHECK((int64_t)image_sizes.size() == 2 * N && (int64_t)anchors.size() == N * L,
+              "single_stage_postprocess: one image size per image and one anchor tensor per image and level");
+  auto dense_f32 = [&](const at::Tensor& t, int64_t d0, int64_t d1, int64_t d2, const char* what) {
+    TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.get_device() == l0.get_device(), "single_stage_postprocess: ", what,
+                " must be float32 tensors on the logits' GPU");
+    TORCH_CHECK(t.dim() == 3 && t.size(0) == d0 && t.size(1) == d1 && t.size(2) == d2 && (d2 == 1 || t.stride(2) == 1),
+                "single_stage_postprocess: unexpected ", what, " shape or strides");
+  };
+  at::cuda::CUDAGuard guard(l0.device());
+  std::vector<int64_t> A(L), ls(2 * L), cs(2 * L, 0), rs(2 * L), as(N * L);
+  std::vector<const void*> lp(L), cp(L, nullptr), rp(L), ap(N * L);
+  for (int64_t l = 0; l < L; ++l) {
+    A[l] = logits[l].size(1);
+    dense_f32(logits[l], N, A[l], C, "logits");
+    dense_f32(regression[l], N, A[l], 4, "regression");
+    lp[l] = logits[l].data_ptr(); ls[2 * l] = logits[l].stride(0); ls[2 * l + 1] = logits[l].stride(1);
+    rp[l] = regression[l].data_ptr(); rs[2 * l] = regression[l].stride(0); rs[2 * l + 1] = regression[l].stride(1);
+    if (kind == VB200_SS_FCOS) {
+      dense_f32(ctrness[l], N, A[l], 1, "ctrness");
+      cp[l] = ctrness[l].data_ptr(); cs[2 * l] = ctrness[l].stride(0); cs[2 * l + 1] = ctrness[l].stride(1);
+    }
+    for (int64_t n = 0; n < N; ++n) {
+      const at::Tensor& a = anchors[n * L + l];
+      TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kFloat && a.get_device() == l0.get_device() && a.dim() == 2 && a.size(0) == A[l] &&
+                      a.size(1) == 4 && a.stride(1) == 1,
+                  "single_stage_postprocess: anchors must be float32 [A_l, 4] tensors with a dense last dimension");
+      ap[n * L + l] = a.data_ptr();
+      as[n * L + l] = a.stride(0);
+    }
+  }
+  std::vector<double> hw(image_sizes.begin(), image_sizes.end());
+  std::vector<double> wt(weights.begin(), weights.end());
+  const int64_t cap = N * std::max<int64_t>(detections_per_img, 0);
+  at::Tensor ob = at::empty({cap, 4}, l0.options()), os = at::empty({cap}, l0.options());
+  at::Tensor ol = at::empty({cap}, l0.options().dtype(at::kLong));
+  at::Tensor counts = at::zeros({N}, at::TensorOptions().dtype(at::kLong));
+  const size_t wsb = vb200_single_stage_postprocess_workspace_bytes((int)kind, (int)N, (int)L, A.data(), (int)C, topk_candidates,
+                                                                    detections_per_img);
+  at::Tensor ws = workspace(wsb, l0);
+  check_rc(vb200_single_stage_postprocess((int)kind, (int)N, (int)L, A.data(), (int)C, lp.data(), ls.data(), cp.data(), cs.data(), rp.data(),
+                                          rs.data(), ap.data(), as.data(), hw.data(), score_thresh, topk_candidates, nms_thresh,
+                                          detections_per_img, wt.data(), bbox_xform_clip, g_nms_semantics.load(), ws.data_ptr(), wsb,
+                                          ob.data_ptr(), os.data_ptr(), ol.data_ptr<int64_t>(), counts.data_ptr<int64_t>(), cur_stream()),
+           "single_stage_postprocess");
+  const int64_t total = counts.sum().item<int64_t>();
+  return std::make_tuple(ob.narrow(0, 0, total), os.narrow(0, 0, total), ol.narrow(0, 0, total), counts);
+}
+
 // ---- deform_conv2d ---------------------------------------------------------
 // Packed weights are cached per weight tensor: the key is the TensorImpl (held weakly, so a recycled address cannot
 // alias) plus its version counter (an in-place update of the parameter invalidates the entry).  The packed layout follows
@@ -736,6 +800,7 @@ TORCH_LIBRARY(vision_b200, m) {
   m.def("resize_crop_normalize(Tensor input, int resize_h, int resize_w, int crop_top, int crop_left, int crop_h, int crop_w, int mode, bool antialias, float[] mean, float[] std) -> Tensor");
   m.def("box_iou_rotated(Tensor boxes1, Tensor boxes2) -> Tensor");
   m.def("detection_postprocess(Tensor boxes, Tensor scores, Tensor labels, float img_h, float img_w, float score_thresh, bool score_inclusive, float min_size, float nms_thresh, int topk) -> (Tensor, Tensor, Tensor)");
+  m.def("single_stage_postprocess(int kind, Tensor[] logits, Tensor[] ctrness, Tensor[] regression, Tensor[] anchors, int[] image_sizes, float score_thresh, int topk_candidates, float nms_thresh, int detections_per_img, float[] weights, float bbox_xform_clip) -> (Tensor, Tensor, Tensor, Tensor)");
   m.def("multiscale_roi_align(Tensor[] features, Tensor rois, float[] scales, int pooled_height, int pooled_width, int sampling_ratio, int k_min, int k_max, float canonical_scale, float canonical_level, float eps) -> (Tensor, Tensor)");
   m.def("_roi_align_backward(Tensor grad, Tensor rois, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width, int sampling_ratio, bool aligned) -> Tensor");
   m.def("_roi_pool_backward(Tensor grad, Tensor rois, Tensor argmax, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width) -> Tensor");
@@ -767,6 +832,7 @@ TORCH_LIBRARY_IMPL(vision_b200, CUDA, m) {
   m.impl("ps_roi_pool", TORCH_FN(ps_roi_pool));
   m.impl("_ps_roi_pool_backward", TORCH_FN(ps_roi_pool_backward));
   m.impl("detection_postprocess", TORCH_FN(detection_postprocess));
+  m.impl("single_stage_postprocess", TORCH_FN(single_stage_postprocess));
   m.impl("resize_crop_normalize", TORCH_FN(resize_crop_normalize));
   m.impl("box_iou_rotated", TORCH_FN(box_iou_rotated));
   m.impl("_deform_conv2d_backward", TORCH_FN(deform_conv2d_backward));

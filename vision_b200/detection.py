@@ -2,7 +2,11 @@
 ``RoIHeads.postprocess_detections`` (torchvision/models/detection/roi_heads.py:680-737) and
 ``RegionProposalNetwork.filter_proposals`` (rpn.py:242-298).  Everything up to the per-image loop (box decoding, softmax,
 per-level top-k, sigmoid) is the reference's own tensor code; the per-image tail - clip, score filter, remove_small_boxes,
-batched_nms, top-k, gathers - is ONE call of ``vision_b200::detection_postprocess`` per image."""
+batched_nms, top-k, gathers - is ONE call of ``vision_b200::detection_postprocess`` per image.
+
+The single-stage detectors' ``postprocess_detections`` (RetinaNet retinanet.py:509-571, FCOS fcos.py:489-556, SSD / SSDLite
+ssd.py:414-463) are ONE call of ``vision_b200::single_stage_postprocess`` for all images: score, threshold, per-level (or
+per-class) top-k, decode, clip, batched_nms and the top detections.  SSD keeps its softmax prologue as torch code."""
 from __future__ import annotations
 
 import torch
@@ -10,6 +14,11 @@ import torch.nn.functional as F
 from torch import Tensor
 
 from . import _lib
+
+
+# per-segment top-k capacity of the select kernel (VB200_SS_MAX_TOPK in include/vision_b200.h)
+SINGLE_STAGE_MAX_TOPK = 2048
+_SS_RETINANET, _SS_FCOS, _SS_SSD = 0, 1, 2
 
 
 def _fusable(t: Tensor) -> bool:
@@ -71,3 +80,89 @@ def rpn_filter_proposals(self, proposals, objectness, image_shapes, num_anchors_
         final_boxes.append(b)
         final_scores.append(s)
     return final_boxes, final_scores
+
+
+def _traced() -> bool:
+    import torchvision
+
+    return torch.jit.is_scripting() or torch.jit.is_tracing() or torchvision._is_tracing()
+
+
+def _dense_f32(t) -> bool:
+    return isinstance(t, Tensor) and t.is_cuda and t.dtype == torch.float32 and t.dim() >= 2 and t.stride(-1) == 1
+
+
+def _levels_ok(logits, extra, anchors, num_images: int, extra_width: int) -> bool:
+    """Per-level [N, A_l, C] logits, [N, A_l, extra_width] companions and N * L [A_l, 4] anchors, as the kernel takes them;
+    a level of 2^31 or more logits is left to the reference (the kernel indexes a segment with 32 bits)."""
+    if not isinstance(logits, (list, tuple)) or not logits or len(anchors) != num_images * len(logits):
+        return False
+    C = logits[0].shape[-1] if isinstance(logits[0], Tensor) else -1
+    for l, lg in enumerate(logits):
+        if not (_dense_f32(lg) and lg.dim() == 3 and lg.shape[0] == num_images and lg.shape[2] == C and lg.shape[1] * C < 2**31):
+            return False
+        for t, width in zip(extra[l], extra_width):
+            if not (_dense_f32(t) and t.dim() == 3 and tuple(t.shape) == (num_images, lg.shape[1], width)):
+                return False
+    for i, a in enumerate(anchors):
+        if not (_dense_f32(a) and a.dim() == 2 and tuple(a.shape) == (logits[i % len(logits)].shape[1], 4)):
+            return False
+    return True
+
+
+def single_stage_postprocess(kind: int, logits, ctrness, regression, anchors, image_shapes, score_thresh: float, topk_candidates: int,
+                             nms_thresh: float, detections_per_img: int, weights=(1.0, 1.0, 1.0, 1.0), bbox_xform_clip: float = 0.0):
+    """All images of a single-stage detector's postprocess_detections in one call; returns the reference's list of dicts."""
+    _lib.load_ops()
+    sizes = [int(v) for hw in image_shapes for v in hw]
+    boxes, scores, labels, counts = torch.ops.vision_b200.single_stage_postprocess(
+        kind, list(logits), list(ctrness), list(regression), list(anchors), sizes, float(score_thresh), int(topk_candidates),
+        float(nms_thresh), int(detections_per_img), [float(w) for w in weights], float(bbox_xform_clip))
+    counts = counts.tolist()
+    return [{"boxes": b, "scores": s, "labels": l}
+            for b, s, l in zip(boxes.split(counts), scores.split(counts), labels.split(counts))]
+
+
+def retinanet_postprocess_detections(self, head_outputs, anchors, image_shapes, _orig=None):
+    """RetinaNet.postprocess_detections as one fused call (same outputs, same order)."""
+    from torchvision.models.detection import _utils as det_utils
+
+    logits, regression = head_outputs["cls_logits"], head_outputs["bbox_regression"]
+    flat_anchors = [a for per_image in anchors for a in per_image]
+    if (_traced() or type(self.box_coder) is not det_utils.BoxCoder or not 0 <= self.topk_candidates <= SINGLE_STAGE_MAX_TOPK
+            or len(regression) != len(logits) or len(anchors) != len(image_shapes)
+            or not _levels_ok(logits, [(r,) for r in regression], flat_anchors, len(image_shapes), (4,))):
+        return _orig(self, head_outputs, anchors, image_shapes)
+    coder = self.box_coder
+    return single_stage_postprocess(_SS_RETINANET, logits, [], regression, flat_anchors, image_shapes, self.score_thresh,
+                                    self.topk_candidates, self.nms_thresh, self.detections_per_img, coder.weights, coder.bbox_xform_clip)
+
+
+def fcos_postprocess_detections(self, head_outputs, anchors, image_shapes, _orig=None):
+    """FCOS.postprocess_detections as one fused call (same outputs, same order)."""
+    from torchvision.models.detection import _utils as det_utils
+
+    logits, regression, ctrness = head_outputs["cls_logits"], head_outputs["bbox_regression"], head_outputs["bbox_ctrness"]
+    flat_anchors = [a for per_image in anchors for a in per_image]
+    if (_traced() or type(self.box_coder) is not det_utils.BoxLinearCoder or self.box_coder.normalize_by_size is not True
+            or not 0 <= self.topk_candidates <= SINGLE_STAGE_MAX_TOPK or len(regression) != len(logits) or len(ctrness) != len(logits)
+            or len(anchors) != len(image_shapes)
+            or not _levels_ok(logits, list(zip(regression, ctrness)), flat_anchors, len(image_shapes), (4, 1))):
+        return _orig(self, head_outputs, anchors, image_shapes)
+    return single_stage_postprocess(_SS_FCOS, logits, ctrness, regression, flat_anchors, image_shapes, self.score_thresh,
+                                    self.topk_candidates, self.nms_thresh, self.detections_per_img)
+
+
+def ssd_postprocess_detections(self, head_outputs, image_anchors, image_shapes, _orig=None):
+    """SSD.postprocess_detections (also SSDLite) as softmax + one fused call (same outputs, same order)."""
+    from torchvision.models.detection import _utils as det_utils
+
+    logits, regression = head_outputs["cls_logits"], head_outputs["bbox_regression"]
+    if (_traced() or type(self.box_coder) is not det_utils.BoxCoder or not 0 <= self.topk_candidates <= SINGLE_STAGE_MAX_TOPK
+            or not isinstance(image_anchors, (list, tuple)) or len(image_anchors) != len(image_shapes)
+            or not _levels_ok([logits], [(regression,)], list(image_anchors), len(image_shapes), (4,))):
+        return _orig(self, head_outputs, image_anchors, image_shapes)
+    pred_scores = F.softmax(logits, dim=-1)          # ssd.py:418
+    coder = self.box_coder
+    return single_stage_postprocess(_SS_SSD, [pred_scores], [], [regression], image_anchors, image_shapes, self.score_thresh,
+                                    self.topk_candidates, self.nms_thresh, self.detections_per_img, coder.weights, coder.bbox_xform_clip)
