@@ -8,7 +8,8 @@
 // implicit GEMM  out[oc, pix] = sum_k W[oc, k] * col[k, pix],  k = (ci, tap):
 //   * SIMT kernel (this file; fp32 / fp16 / bf16 storage, fp32 accumulate): a CTA owns
 //     a 128(oc) x 64(pix) output tile of one image.  Per offset group it builds a
-//     sampling table in shared memory ONCE — for each (tap, pixel): 4 clamped corner
+//     sampling table in shared memory ONCE (per chunk of taps for kernels whose table
+//     exceeds shared memory, KK > 106) — for each (tap, pixel): 4 clamped corner
 //     offsets + 4 bilinear weights (zeroed out of bounds, pre-multiplied by the
 //     modulation mask) — and reuses it for every input channel of that group, so a
 //     col element costs 4 loads + 4 FMAs.  K is walked in slabs of 16; A (weights) and
@@ -32,11 +33,11 @@ struct SampleEnt { int o[4]; float w[4]; };   // 32 B
 template <typename T>
 __global__ void __launch_bounds__(DCN_THREADS)
 deform_conv2d_simt_kernel(const T* __restrict__ input, const T* __restrict__ weight, const T* __restrict__ offset,
-                          const T* __restrict__ mask, const T* __restrict__ bias, T* __restrict__ out, DcnParams p) {
+                          const T* __restrict__ mask, const T* __restrict__ bias, T* __restrict__ out, DcnParams p, int tab_taps) {
   extern __shared__ __align__(16) unsigned char dsm[];
   const int KK = p.kh * p.kw;
-  SampleEnt* tab = reinterpret_cast<SampleEnt*>(dsm);                 // [KK][BN]
-  float* As = reinterpret_cast<float*>(tab + (size_t)KK * BN);        // [BK][BM]
+  SampleEnt* tab = reinterpret_cast<SampleEnt*>(dsm);                 // [tab_taps][BN]
+  float* As = reinterpret_cast<float*>(tab + (size_t)tab_taps * BN);  // [BK][BM]
   float* Bs = As + BK * BMP;                                          // [BK][BN]
 
   const int tid = threadIdx.x;
@@ -62,83 +63,92 @@ deform_conv2d_simt_kernel(const T* __restrict__ input, const T* __restrict__ wei
   const int og_lo = ci_lo / c_per_off, og_hi = (ci_hi - 1) / c_per_off;
 
   for (int og = og_lo; og <= og_hi; ++og) {
-    // ---- sampling table for (offset group og, this pixel tile) ----
-    __syncthreads();
     const T* __restrict__ off_b = offset + ((int64_t)b * p.offset_groups + og) * 2 * KK * HWo;
     const T* __restrict__ msk_b = p.use_mask ? mask + ((int64_t)b * p.offset_groups + og) * KK * HWo : nullptr;
-    for (int e = tid; e < KK * BN; e += DCN_THREADS) {
-      const int tap = e / BN, px = e - tap * BN;
-      const int pix = pix0 + px;
-      SampleEnt se;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) { se.o[q] = 0; se.w[q] = 0.f; }
-      if (pix < HWo) {
-        const int oy = pix / p.out_w, ox = pix - oy * p.out_w;
-        const int i = tap / p.kw, j = tap - i * p.kw;
-        const float oh = to_acc(off_b[(int64_t)(2 * tap) * HWo + pix]);
-        const float ow = to_acc(off_b[(int64_t)(2 * tap + 1) * HWo + pix]);
-        const float mv = p.use_mask ? to_acc(msk_b[(int64_t)tap * HWo + pix]) : 1.f;
-        const float y = add_rn((float)(oy * p.stride_h - p.pad_h + i * p.dil_h), oh);
-        const float x = add_rn((float)(ox * p.stride_w - p.pad_w + j * p.dil_w), ow);
-        if (!(y <= -1.f || (float)p.in_h <= y || x <= -1.f || (float)p.in_w <= x)) {
-          const int hl = (int)floorf(y), wl = (int)floorf(x);
-          const int hh_i = hl + 1, wh_i = wl + 1;
-          const float lh = sub_rn(y, (float)hl), lw = sub_rn(x, (float)wl);
-          const float hh = sub_rn(1.f, lh), hw = sub_rn(1.f, lw);
-          const bool t0 = hl >= 0, t1 = hh_i <= p.in_h - 1, l0 = wl >= 0, l1 = wh_i <= p.in_w - 1;
-          const int hlc = max(hl, 0), hhc = min(hh_i, p.in_h - 1), wlc = max(wl, 0), whc = min(wh_i, p.in_w - 1);
-          se.o[0] = hlc * p.in_w + wlc; se.w[0] = (t0 && l0) ? mv * (hh * hw) : 0.f;
-          se.o[1] = hlc * p.in_w + whc; se.w[1] = (t0 && l1) ? mv * (hh * lw) : 0.f;
-          se.o[2] = hhc * p.in_w + wlc; se.w[2] = (t1 && l0) ? mv * (lh * hw) : 0.f;
-          se.o[3] = hhc * p.in_w + whc; se.w[3] = (t1 && l1) ? mv * (lh * lw) : 0.f;
-        }
-      }
-      tab[e] = se;
-    }
-    __syncthreads();
-
     const int c_start = max(ci_lo, og * c_per_off), c_end = min(ci_hi, (og + 1) * c_per_off);
-    const int k_start = (c_start - ci_lo) * KK, k_end = (c_end - ci_lo) * KK;   // within-group k range
-    for (int k0 = k_start; k0 < k_end; k0 += BK) {
-      // A slab: As[kk][m] = W[g*cout_g + oc0 + m][k0 + kk]
-      for (int e = tid; e < BK * BM; e += DCN_THREADS) {
-        const int m = e / BK, kk = e - m * BK;
-        const int k = k0 + kk, oc = oc0 + m;
-        float v = 0.f;
-        if (k < k_end && oc < cout_g) v = to_acc(weight[((int64_t)(g * cout_g + oc)) * Kg + k]);
-        As[kk * BMP + m] = v;
-      }
-      // B slab: Bs[kk][px] = sum_q w_q * in[ci][o_q]
-      for (int e = tid; e < BK * BN; e += DCN_THREADS) {
-        const int kk = e / BN, px = e - kk * BN;
-        const int k = k0 + kk;
-        float v = 0.f;
-        if (k < k_end) {
-          const int cil = k / KK, tap = k - cil * KK;
-          const T* __restrict__ pl = in_b + (int64_t)(ci_lo + cil) * p.in_h * p.in_w;
-          const SampleEnt se = tab[tap * BN + px];
-          v = se.w[0] * to_acc(pl[se.o[0]]);
-          v = fmaf(se.w[1], to_acc(pl[se.o[1]]), v);
-          v = fmaf(se.w[2], to_acc(pl[se.o[2]]), v);
-          v = fmaf(se.w[3], to_acc(pl[se.o[3]]), v);
+    // taps [t0, t0 + nt) per table; one chunk (t0 = 0, nt = KK) unless the whole table exceeds shared memory.  Within a chunk
+    // the contraction index kl = (channel - c_start) * nt + (tap - t0), so with one chunk k = k_start + kl, the weight row order.
+    for (int t0 = 0; t0 < KK; t0 += tab_taps) {
+      const int nt = min(tab_taps, KK - t0);
+      // ---- sampling table for (offset group og, taps [t0, t0 + nt), this pixel tile) ----
+      __syncthreads();
+      for (int e = tid; e < nt * BN; e += DCN_THREADS) {
+        const int tl = e / BN, px = e - tl * BN;
+        const int tap = t0 + tl;
+        const int pix = pix0 + px;
+        SampleEnt se;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) { se.o[q] = 0; se.w[q] = 0.f; }
+        if (pix < HWo) {
+          const int oy = pix / p.out_w, ox = pix - oy * p.out_w;
+          const int i = tap / p.kw, j = tap - i * p.kw;
+          const float oh = to_acc(off_b[(int64_t)(2 * tap) * HWo + pix]);
+          const float ow = to_acc(off_b[(int64_t)(2 * tap + 1) * HWo + pix]);
+          const float mv = p.use_mask ? to_acc(msk_b[(int64_t)tap * HWo + pix]) : 1.f;
+          const float y = add_rn((float)(oy * p.stride_h - p.pad_h + i * p.dil_h), oh);
+          const float x = add_rn((float)(ox * p.stride_w - p.pad_w + j * p.dil_w), ow);
+          if (!(y <= -1.f || (float)p.in_h <= y || x <= -1.f || (float)p.in_w <= x)) {
+            const int hl = (int)floorf(y), wl = (int)floorf(x);
+            const int hh_i = hl + 1, wh_i = wl + 1;
+            const float lh = sub_rn(y, (float)hl), lw = sub_rn(x, (float)wl);
+            const float hh = sub_rn(1.f, lh), hw = sub_rn(1.f, lw);
+            const bool t0_ = hl >= 0, t1 = hh_i <= p.in_h - 1, l0 = wl >= 0, l1 = wh_i <= p.in_w - 1;
+            const int hlc = max(hl, 0), hhc = min(hh_i, p.in_h - 1), wlc = max(wl, 0), whc = min(wh_i, p.in_w - 1);
+            se.o[0] = hlc * p.in_w + wlc; se.w[0] = (t0_ && l0) ? mv * (hh * hw) : 0.f;
+            se.o[1] = hlc * p.in_w + whc; se.w[1] = (t0_ && l1) ? mv * (hh * lw) : 0.f;
+            se.o[2] = hhc * p.in_w + wlc; se.w[2] = (t1 && l0) ? mv * (lh * hw) : 0.f;
+            se.o[3] = hhc * p.in_w + whc; se.w[3] = (t1 && l1) ? mv * (lh * lw) : 0.f;
+          }
         }
-        Bs[kk * BN + px] = v;
+        tab[e] = se;
       }
       __syncthreads();
+
+      const int cil0 = c_start - ci_lo, nk = (c_end - c_start) * nt;
+      for (int k0 = 0; k0 < nk; k0 += BK) {
+        // A slab: As[kk][m] = W[g*cout_g + oc0 + m][cil * KK + tap]
+        for (int e = tid; e < BK * BM; e += DCN_THREADS) {
+          const int m = e / BK, kk = e - m * BK;
+          const int kl = k0 + kk, oc = oc0 + m;
+          float v = 0.f;
+          if (kl < nk && oc < cout_g) {
+            const int cl = kl / nt, tap = t0 + (kl - cl * nt);
+            v = to_acc(weight[((int64_t)(g * cout_g + oc)) * Kg + (cil0 + cl) * KK + tap]);
+          }
+          As[kk * BMP + m] = v;
+        }
+        // B slab: Bs[kk][px] = sum_q w_q * in[ci][o_q]
+        for (int e = tid; e < BK * BN; e += DCN_THREADS) {
+          const int kk = e / BN, px = e - kk * BN;
+          const int kl = k0 + kk;
+          float v = 0.f;
+          if (kl < nk) {
+            const int cl = kl / nt, tl = kl - cl * nt;
+            const T* __restrict__ pl = in_b + (int64_t)(c_start + cl) * p.in_h * p.in_w;
+            const SampleEnt se = tab[tl * BN + px];
+            v = se.w[0] * to_acc(pl[se.o[0]]);
+            v = fmaf(se.w[1], to_acc(pl[se.o[1]]), v);
+            v = fmaf(se.w[2], to_acc(pl[se.o[2]]), v);
+            v = fmaf(se.w[3], to_acc(pl[se.o[3]]), v);
+          }
+          Bs[kk * BN + px] = v;
+        }
+        __syncthreads();
 #pragma unroll
-      for (int kk = 0; kk < BK; ++kk) {
-        float a[8], bb[4];
-        const float4 a0 = *reinterpret_cast<const float4*>(As + kk * BMP + tm * 8);
-        const float4 a1 = *reinterpret_cast<const float4*>(As + kk * BMP + tm * 8 + 4);
-        const float4 b0 = *reinterpret_cast<const float4*>(Bs + kk * BN + tn * 4);
-        a[0] = a0.x; a[1] = a0.y; a[2] = a0.z; a[3] = a0.w; a[4] = a1.x; a[5] = a1.y; a[6] = a1.z; a[7] = a1.w;
-        bb[0] = b0.x; bb[1] = b0.y; bb[2] = b0.z; bb[3] = b0.w;
+        for (int kk = 0; kk < BK; ++kk) {
+          float a[8], bb[4];
+          const float4 a0 = *reinterpret_cast<const float4*>(As + kk * BMP + tm * 8);
+          const float4 a1 = *reinterpret_cast<const float4*>(As + kk * BMP + tm * 8 + 4);
+          const float4 b0 = *reinterpret_cast<const float4*>(Bs + kk * BN + tn * 4);
+          a[0] = a0.x; a[1] = a0.y; a[2] = a0.z; a[3] = a0.w; a[4] = a1.x; a[5] = a1.y; a[6] = a1.z; a[7] = a1.w;
+          bb[0] = b0.x; bb[1] = b0.y; bb[2] = b0.z; bb[3] = b0.w;
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
+          for (int i = 0; i < 8; ++i)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], bb[j], acc[i][j]);
+            for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], bb[j], acc[i][j]);
+        }
+        __syncthreads();
       }
-      __syncthreads();
     }
   }
   // ---- epilogue: + bias, NCHW store ----
@@ -161,17 +171,22 @@ template <typename T>
 int launch_simt(const void* input, const void* weight, const void* offset, const void* mask, const void* bias, void* out,
                 const DcnParams& p, cudaStream_t st) {
   const int KK = p.kh * p.kw;
-  const size_t smem = (size_t)KK * BN * sizeof(SampleEnt) + (size_t)(BK * BMP + BK * BN) * 4;
-  if (smem > (size_t)max_smem_optin() - 1024) {
-    set_error("deform_conv2d: kernel %dx%d too large for the shared-memory sampling table", p.kh, p.kw);
+  // the sampling table holds every tap when it fits (up to 106 taps with H100's 227 KB opt-in), else as many taps as fit
+  const size_t slabs = (size_t)(BK * BMP + BK * BN) * 4;
+  const size_t optin = (size_t)max_smem_optin();
+  const size_t fit = optin > 1024 + slabs ? (optin - 1024 - slabs) / (BN * sizeof(SampleEnt)) : 0;
+  if (fit == 0) {       // not even one tap of the table fits (the chunk loop would not advance)
+    set_error("deform_conv2d: %zu bytes of opt-in shared memory hold no tap of the sampling table", optin);
     return VB200_EUNSUPPORTED;
   }
+  const int tab_taps = (size_t)KK < fit ? KK : (int)fit;
+  const size_t smem = (size_t)tab_taps * BN * sizeof(SampleEnt) + slabs;
   if (smem > 48 * 1024)
     VB200_CUDA_TRY(ensure_dyn_smem<deform_conv2d_simt_kernel<T>>(smem));
   const int cout_g = p.c_out / p.groups;
   dim3 grid((unsigned)ceil_div(p.out_h * p.out_w, BN), (unsigned)(p.groups * ceil_div(cout_g, BM)), (unsigned)p.batch);
   deform_conv2d_simt_kernel<T><<<grid, DCN_THREADS, smem, st>>>((const T*)input, (const T*)weight, (const T*)offset,
-                                                               (const T*)mask, (const T*)bias, (T*)out, p);
+                                                               (const T*)mask, (const T*)bias, (T*)out, p, tab_taps);
   return check_launch("deform_conv2d_simt_kernel");
 }
 

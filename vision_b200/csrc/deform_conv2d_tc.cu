@@ -149,6 +149,12 @@ template <> struct Wgmma<64> {
                    : "l"(da), "l"(db));
   }
 };
+// bf16 m64n64k16 with a run-time scale-d: D = A B^T when scale_d == 0 (the accumulator's old value is ignored), else D += A B^T
+__device__ __forceinline__ void wgmma64_bf16_sd(float (&d)[32], uint64_t da, uint64_t db, int scale_d) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "l"(da), "l"(db), "r"(scale_d));
+}
 template <> struct Wgmma<128> {
   template <int FMT> static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) {
     if constexpr (FMT == 1)
@@ -424,18 +430,24 @@ deform_conv2d_tc_kernel(const T* __restrict__ nhwc, const T* __restrict__ wpacke
 // fp32 inputs on the tensor core: three-way bf16 split (bf16x3).
 // A float v is v1 + v2 + v3 with v1 = bf16(v), v2 = bf16(v - v1), v3 = bf16(v - v1 - v2) (8 + 8 + 8 mantissa bits); the
 // product a*b is a1b1 + (a1b2 + a2b1) + (a2b2 + a1b3 + a3b1) + O(2^-24): SIX bf16 MMAs per K step reproduce the fp32
-// result to ~1e-7 relative per product - inside the 1e-5 budget of the fp32 rows, at 6x the bf16 tensor time, still
-// several times faster than a SIMT fp32 implicit GEMM (or the reference's im2col + SGEMM).  Same structure as
+// product to about 2^-24 relative - inside the 1e-5 budget of the fp32 rows with the accumulation below - at 6x the
+// bf16 tensor time, still several times faster than a SIMT fp32 implicit GEMM (or the reference's im2col + SGEMM).  Same structure as
 // deform_conv2d_tc_kernel: M = 128 pixels, N = BN couts, K step 32 channels (SWIZZLE_64B); a stage holds A1 A2 A3
 // (8 KB each) and B1 B2 B3 (BN x 64 B each); the gather reads a channels-last fp32 staging copy (one 128-byte line =
 // 32 channels per pixel corner), blends in fp32 and writes the three splits.
 // ACCUMULATION: the tensor core adds into its fp32 accumulator with truncation (about one ulp of the accumulator per MMA
 // instruction, a bias that grows linearly with the number of MMAs into one accumulator).  So (1) the five correction
-// terms go to their OWN accumulator (its magnitude is 2^-8 of the result, so its truncation is invisible) and (2) the
-// a1 b1 terms rotate over THREE accumulators by K step; the epilogue adds the four with round-to-nearest.
-// BN = 64: 3 + 1 accumulators x 32 registers per thread.
+// terms go to their OWN accumulator (its magnitude is 2^-8 of the result, so its truncation is invisible), (2) the
+// a1 b1 terms alternate over TWO accumulators by K step and (3) after every T3_FOLD of its own K steps an accumulator is
+// added, round-to-nearest, into a register total, so none takes more than 16 truncating MMAs.  The fold reads an
+// accumulator whose MMAs are complete while the MMAs of the next step (into the other one) are in flight, so the
+// pipeline does not drain; the accumulator's next MMA then overwrites it (scale-d 0) - zeroing the registers instead
+// would serialise the wgmma pipeline.  Without (3) (three rotating accumulators) the error grew with depth past the 1e-5
+// bound: 2.2e-5 of 1 + |ref| at K = 10240 on post-ReLU-like activations.  The epilogue adds the total, the two and the
+// corrections with round-to-nearest.
+// BN = 64: 2 + 1 accumulators + the total x 32 registers per thread.
 // =================================================================================================
-constexpr int T3_KB = 32, T3_STAGES = 4, T3_MAIN = 3;
+constexpr int T3_KB = 32, T3_STAGES = 4, T3_MAIN = 2, T3_FOLD = 8;
 constexpr int T3_ROW = 2 * T3_KB;                 // 64-byte tile rows
 constexpr int T3_A = TC_BM * T3_ROW;              // 8 KB per A split
 
@@ -444,6 +456,12 @@ __device__ __forceinline__ void split3(float v, __nv_bfloat16& a, __nv_bfloat16&
   const float r1 = v - __bfloat162float(a);      // exact: the residual has at most 16 significant bits
   b = __float2bfloat16_rn(r1);
   c = __float2bfloat16_rn(r1 - __bfloat162float(b));
+}
+
+template <int R>
+__device__ __forceinline__ void fold_acc(float (&total)[R], const float (&a)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) total[i] = __fadd_rn(total[i], a[i]);
 }
 
 // weights [Cout][Cin][KK] fp32 -> per (n tile, stage q = cslab32 * KK + tap): B1 | B2 | B3 swizzled tiles of BN x 32
@@ -517,9 +535,10 @@ deform_conv2d_tc3_kernel(const float* __restrict__ nhwc, const __nv_bfloat16* __
   const int cchunk = lane & 7, pq = lane >> 3;             // lane -> (pixel sub-index, 4-channel chunk of the 32-channel line)
   const int prow0 = warp * 16 + pq;
   const float* __restrict__ in_b = nhwc + (int64_t)b * HWi * p.c_in;
-  float acc0[BN / 2], acc1[BN / 2], acc2[BN / 2], accs[BN / 2];      // main accumulators (q mod 3) + corrections
+  float acc0[BN / 2], acc1[BN / 2], accs[BN / 2];      // main accumulators (q mod 2) + corrections
+  float total[BN / 2];                                                // folded main accumulators (round-to-nearest)
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; acc2[i] = 0.f; accs[i] = 0.f; }
+  for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; accs[i] = 0.f; total[i] = 0.f; }
   int q = 0;
   for (int og = 0; og < p.offset_groups; ++og) {
     asm volatile("bar.sync 1, %0;" ::"n"(WG_CONSUMERS));
@@ -568,7 +587,7 @@ deform_conv2d_tc3_kernel(const float* __restrict__ nhwc, const __nv_bfloat16* __
       mbar_wait(&fullB[st], (uint32_t)(q / T3_STAGES) & 1u);
       const uint32_t a_addr = smem_u32(a_tile) + (uint32_t)(wg * 64 * T3_ROW);
       const uint32_t b_addr = smem_u32(a_tile) + 3 * T3_A;
-      wg_fence_acc(acc0); wg_fence_acc(acc1); wg_fence_acc(acc2); wg_fence_acc(accs);
+      wg_fence_acc(acc0); wg_fence_acc(acc1); wg_fence_acc(accs); wg_fence_acc(total);
       wg_fence();
       // correction terms (a3b1, a1b3, a2b2, a2b1, a1b2) -> their own accumulator
       constexpr int ia[5] = {2, 0, 1, 1, 0}, ib[5] = {0, 2, 1, 0, 1};
@@ -578,23 +597,31 @@ deform_conv2d_tc3_kernel(const float* __restrict__ nhwc, const __nv_bfloat16* __
         for (int k = 0; k < T3_KB / 16; ++k)
           Wgmma<BN>::template mma<1>(accs, wg_desc<T3_ROW>(a_addr + ia[t] * T3_A + k * 32), wg_desc<T3_ROW>(b_addr + ib[t] * B_BYTES + k * 32));
       }
-      // a1 b1 -> main accumulator q mod 3
+      // a1 b1 -> main accumulator q mod 2, restarted (scale-d 0) when it was folded into the total after its last step
       const int m = q % T3_MAIN;
+      const int keep = (q >= T3_MAIN && ((q - T3_MAIN) / T3_MAIN) % T3_FOLD == T3_FOLD - 1) ? 0 : 1;
+      static_assert(BN == 64, "the main-accumulator MMAs are written for m64n64k16");
 #pragma unroll
       for (int k = 0; k < T3_KB / 16; ++k) {
         const uint64_t da = wg_desc<T3_ROW>(a_addr + k * 32), db = wg_desc<T3_ROW>(b_addr + k * 32);
-        if (m == 0) Wgmma<BN>::template mma<1>(acc0, da, db);
-        else if (m == 1) Wgmma<BN>::template mma<1>(acc1, da, db);
-        else Wgmma<BN>::template mma<1>(acc2, da, db);
+        const int sd = k == 0 ? keep : 1;
+        if (m == 0) wgmma64_bf16_sd(acc0, da, db, sd);
+        else wgmma64_bf16_sd(acc1, da, db, sd);
       }
       wg_commit();
       wg_wait<1>();
-      wg_fence_acc(acc0); wg_fence_acc(acc1); wg_fence_acc(acc2); wg_fence_acc(accs);
+      wg_fence_acc(acc0); wg_fence_acc(acc1); wg_fence_acc(accs); wg_fence_acc(total);
       if (lane == 0 && q > 0) mbar_arrive(&empty[(q - 1) % T3_STAGES]);
+      // step q-1 is complete: fold its main accumulator once that accumulator has taken T3_FOLD steps, if a later step
+      // (q+1) restarts it; otherwise the epilogue adds it
+      if (q > 0 && q + 1 < n_q && ((q - 1) / T3_MAIN) % T3_FOLD == T3_FOLD - 1) {
+        if ((q - 1) % T3_MAIN == 0) fold_acc(total, acc0);
+        else fold_acc(total, acc1);
+      }
     }
   }
   wg_wait<0>();
-  wg_fence_acc(acc0); wg_fence_acc(acc1); wg_fence_acc(acc2); wg_fence_acc(accs);
+  wg_fence_acc(acc0); wg_fence_acc(acc1); wg_fence_acc(accs); wg_fence_acc(total);
 
   // ================= epilogue: registers -> transposed tile in shared memory -> NCHW fp32 =================
   asm volatile("bar.sync 1, %0;" ::"n"(WG_CONSUMERS) : "memory");
@@ -609,7 +636,7 @@ deform_conv2d_tc3_kernel(const float* __restrict__ nhwc, const __nv_bfloat16* __
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int i = 4 * j + 2 * h + e, col = 8 * j + 2 * (lane & 3) + e;
-        const float main = acc2[i] + (acc1[i] + acc0[i]);
+        const float main = total[i] + (acc1[i] + acc0[i]);
         tile[col * LD + row_base + 8 * h] = (main + accs[i]) + (bias ? bias[nt * BN + col] : 0.f);
       }
     }
