@@ -161,7 +161,8 @@ VB200_API int vb200_ps_roi_pool_backward(const void* grad, const void* rois, voi
  * grad_input [batch, channels, height, width] - written IN FULL (no pre-zeroing).  Unlike the reference (atomics,
  * alertNotDeterministic) the fp32 / fixed-sampling-grid path is bit-reproducible: every grad_input plane is
  * accumulated in shared memory by row-owning warps in a fixed order.  That path runs when `deterministic` != 0 (the shim
- * passes torch.are_deterministic_algorithms_enabled(); the reference raises in that mode).  With `deterministic` == 0
+ * passes torch.are_deterministic_algorithms_enabled(); the reference raises in that mode), and for roi_align also when its
+ * tables exceed 32 y samples, 32 x taps or 64 bins.  Otherwise, with `deterministic` == 0,
  * roi_align still accumulates plane by plane in shared memory, but with shared-memory atomics and the RoIs dealt
  * round-robin to the warps (no repeated work; summation order varies like the reference's), and roi_pool /
  * ps_roi_align - one bin per (RoI, plane) - scatter with global atomics.  Other dtypes (F16, F64),

@@ -232,7 +232,7 @@ def test_roi_align_backward_plane_path_vs_reference_and_deterministic(vb, aligne
     assert not vb.installed()
     from test_gpu_parity import force_env
     for (b, c, h, w, k, ph, pw, small) in [(2, 6, 50, 68, 700, 7, 7, False), (1, 3, 24, 30, 400, 7, 7, True), (1, 2, 40, 40, 300, 3, 20, False),
-                                           (3, 2, 9, 11, 100, 2, 2, False)]:
+                                           (3, 2, 9, 11, 100, 2, 2, False), (1, 2, 40, 40, 200, 14, 14, False)]:
         g, rois = _bwd_case(b * 100 + k + sr, b, c, h, w, k, small=small)
         grad = torch.randn(k, c, ph, pw, generator=g) * 0.25
         gd, rd = grad.to(DEV), rois.to(DEV)

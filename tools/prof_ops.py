@@ -1,6 +1,6 @@
 """Small driver for ncu captures: runs one op of the hot path a few times at its BASELINE shape.
     python tools/prof_ops.py roi_align|roi_pool|ps_roi_align|ps_roi_pool|batched_nms|nms|resize|resize128|resize_noaa|deform|deform_f32|
-                             roi_align_bwd|roi_align_bwd_det|multiscale|postprocess|preprocess [iters]
+                             roi_align_bwd|roi_align_bwd_det|roi_align_bwd14|roi_align_bwd14_det|multiscale|postprocess|preprocess [iters]
     python tools/prof_ops.py retinanet_post|fcos_post|ssd_post [iters]     fused vs. reference postprocess_detections,
                              batch 1 and 8, logits N(-4.595, 1) and N(-4.595, 0.5); select-kernel time from torch.profiler"""
 import os
@@ -127,12 +127,13 @@ elif op in ("ps_roi_align", "ps_roi_pool"):
     x, r, kw = workloads.cfg2_roi_align()
     x, r = x[:, :245].contiguous().to(dev), r.to(dev)
     fn = (lambda: vb.ops.ps_roi_align(x, r, 7, 0.25, 2)) if op == "ps_roi_align" else (lambda: vb.ops.ps_roi_pool(x, r, 7, 0.25))
-elif op in ("roi_align_bwd", "roi_align_bwd_det"):
+elif op in ("roi_align_bwd", "roi_align_bwd_det", "roi_align_bwd14", "roi_align_bwd14_det"):
     _, r, kw = workloads.cfg2_roi_align()
     r = r.to(dev)
-    g = torch.randn(1000, 256, 7, 7, device=dev)
+    p = 14 if "bwd14" in op else 7          # 14x14: the Mask R-CNN mask head's pooled size
+    g = torch.randn(1000, 256, p, p, device=dev)
     torch.use_deterministic_algorithms(op.endswith("det"))
-    fn = lambda: torch.ops.vision_b200._roi_align_backward(g, r, 0.25, 7, 7, 1, 256, 200, 272, 2, False)
+    fn = lambda: torch.ops.vision_b200._roi_align_backward(g, r, 0.25, p, p, 1, 256, 200, 272, 2, False)
 elif op == "multiscale":
     from collections import OrderedDict
     gen = torch.Generator().manual_seed(0)

@@ -39,6 +39,32 @@ def roi():
     vb.ops.ps_roi_align(xp, r[:50], 3, 0.25, 2)
 
 
+def bwd():
+    """roi_align / roi_pool / ps_roi_align backward, default and deterministic: atomic plane, row-owning plane (one and several
+    table chunks) and generic atomic kernels; tiny RoIs (duplicate columns) and boxes outside the image"""
+    vb._lib.load_ops()
+    x, r, kw = workloads.cfg2_roi_align(seed=2, k=120, batch=2, channels=4, height=30, width=36)
+    r = r.clone()
+    r[::7, 1:3] -= 90.0
+    r[1::11, 3:] += 400.0
+    r[2::9, 3:] = r[2::9, 1:3] + 0.5
+    x, r = x.to(dev), r.to(dev)
+    xp = torch.randn(2, 2 * 9, 30, 36, device=dev)
+    for det in (False, True):
+        torch.use_deterministic_algorithms(det)
+        for ph, pw, sr in ((7, 7, 2), (14, 14, 3), (3, 20, 2)):
+            g = torch.randn(120, 4, ph, pw, device=dev)
+            for aligned in (False, True):
+                torch.ops.vision_b200._roi_align_backward(g, r, 0.25, ph, pw, 2, 4, 30, 36, sr, aligned)
+        out, am = torch.ops.vision_b200.roi_pool(x, r, 0.25, 7, 7)
+        torch.ops.vision_b200._roi_pool_backward(torch.randn_like(out), r, am, 0.25, 7, 7, 2, 4, 30, 36)
+        out, cm = torch.ops.vision_b200.ps_roi_align(xp, r, 0.25, 3, 3, 2)
+        torch.ops.vision_b200._ps_roi_align_backward(torch.randn_like(out), r, cm, 0.25, 3, 3, 2, 2, 18, 30, 36)
+    torch.use_deterministic_algorithms(False)
+    torch.ops.vision_b200._roi_align_backward(torch.randn(120, 4, 7, 7, device=dev).double(), r.double(), 0.25, 7, 7, 2, 4, 30, 36,
+                                              2, False)
+
+
 def nms():
     for n in (1, 300, 5000):
         b, s, i = [t.to(dev) for t in workloads.cfg3_batched_nms(n=n)]
@@ -104,7 +130,7 @@ def gather():
     torch.ops.vision_b200.deform_conv2d_gather(xi, w, off, m, bias, [t.data_ptr() for t in d], 1, 1, 1, 1, 1, 1, 1, 1, True)
 
 
-for name, fn in (("roi", roi), ("nms", nms), ("resize", resize), ("dcn", dcn), ("gather", gather)):
+for name, fn in (("roi", roi), ("bwd", bwd), ("nms", nms), ("resize", resize), ("dcn", dcn), ("gather", gather)):
     if only in ("all", name):
         fn()
         torch.cuda.synchronize()

@@ -108,87 +108,31 @@ __device__ __forceinline__ void store_plane(float* __restrict__ dst, const float
   }
 }
 
-// ---- roi_align backward, plane-resident ----------------------------------------------------------------------
-// grad [K, C, PH, PW] contiguous fp32; grad_input [B, C, H, W] written in full.
-__global__ void __launch_bounds__(kBwdThreads, 1)
-roi_align_bwd_plane_kernel(const float* __restrict__ grad, const BwdHdr* __restrict__ hdr, const uint2* __restrict__ ys,
-                           const uint2* __restrict__ xe, float* __restrict__ grad_input, int B, int C, int H, int W, int K,
-                           int PH, int PW, int sr, int band) {
+// ---- the row-owning frame of the bit-reproducible plane kernels ------------------------------------------------
+// Warp w owns the rows [w * band, w * band + band) of every plane its CTA accumulates and walks all K RoIs in index order,
+// 32 at a time: lane i tests RoI n0 + i's header against the band (the next 32 headers load under the current chunk), and
+// chunk(plane, c, n0, hits, flags, r0, r1) receives the ballot of the RoIs that touch rows [r0, r1) and the lane's header
+// flags.  hdr_of(c), called once per plane before its chunks, gives channel c's header array (RoI n's header at
+// [n * hdr_stride]), or nullptr when the plane receives nothing.
+template <typename HdrOf, typename Chunk>
+__device__ __forceinline__ void row_owning_planes(float* __restrict__ grad_input, int B, int C, int H, int W, int K, int band,
+                                                  int hdr_stride, HdrOf hdr_of, Chunk chunk) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* plane = reinterpret_cast<float*>(smem_raw);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int NYS = PH * sr, NXE = 2 * PW * sr, NB = PH * PW;
-  const float inv_count = 1.0f / (float)(sr * sr);         // exact for sr = 1, 2, 4; sr = 3 differs from /9 by one rounding
-  const bool pow2 = (sr & (sr - 1)) == 0;
-  const float count = (float)(sr * sr);
-  const int r0 = warp * band, r1 = min(H, r0 + band);
+  const int lane = threadIdx.x & 31, r0 = (threadIdx.x >> 5) * band, r1 = min(H, r0 + band);
   for (int pl = blockIdx.x; pl < B * C; pl += gridDim.x) {
     const int b = pl / C, c = pl - b * C;
+    const int4* __restrict__ hdr = hdr_of(c);
     zero_plane(plane, H * W);
     __syncthreads();
-    if (r0 < H) {
+    if (r0 < H && hdr) {
+      auto header = [&](int n) { return n < K ? __ldg(hdr + (int64_t)n * hdr_stride) : make_int4(-1, 0, -1, 0); };
+      int4 hnext = header(lane);
       for (int n0 = 0; n0 < K; n0 += 32) {
-        const int nl = n0 + lane;
-        bool hit = false;
-        int flags_l = 0;
-        if (nl < K) {
-          const int4 h = __ldg(reinterpret_cast<const int4*>(hdr) + nl);
-          hit = h.x == b && h.y < r1 && h.z >= r0;
-          flags_l = h.w;
-        }
-        unsigned m = __ballot_sync(0xffffffffu, hit);
-        while (m) {
-          const int i = __ffs(m) - 1;
-          m &= m - 1;
-          const int n = n0 + i;
-          const int flags = __shfl_sync(0xffffffffu, flags_l, i);
-          const float* __restrict__ g = grad + ((int64_t)n * C + c) * NB;
-          for (int yc = 0; yc < NYS; yc += 32) {
-            uint2 yy = make_uint2(0xffffffffu, 0u);
-            if (yc + lane < NYS) yy = __ldg(ys + (int64_t)n * NYS + yc + lane);
-            const int lo = (int)yy.x;
-            const float l = __uint_as_float(yy.y);
-            const bool inb = lo >= 0 && lo < r1 && (lo + (l > 0.f ? 1 : 0)) >= r0;
-            const unsigned ymask = __ballot_sync(0xffffffffu, inb);
-            if (!ymask) continue;
-            for (int xc = 0; xc < NXE; xc += 32) {
-              uint2 e = make_uint2(0xffffffffu, 0u);
-              if (xc + lane < NXE) e = __ldg(xe + (int64_t)n * NXE + xc + lane);
-              const bool valid = e.x != 0xffffffffu;
-              const int col = (int)(e.x & 0xffffu), pw = (int)(e.x >> 16);
-              const float wx = __uint_as_float(e.y);
-              bool leader = valid;
-              unsigned group = 0u;
-              if (flags & 1) {
-                const unsigned same = __match_any_sync(0xffffffffu, valid ? col : 0x10000 + lane);
-                group = valid ? same : 0u;
-                leader = valid && (__ffs(same) - 1 == lane);
-              }
-              unsigned mm = ymask;
-              int cur_ph = -1;
-              float gv = 0.f;
-              while (mm) {
-                const int j = __ffs(mm) - 1;
-                mm &= mm - 1;
-                const int lo_j = __shfl_sync(0xffffffffu, lo, j);
-                const float l_j = __shfl_sync(0xffffffffu, l, j);
-                const int ph = (yc + j) / sr;
-                if (ph != cur_ph) {
-                  cur_ph = ph;
-                  gv = valid ? __ldg(g + ph * PW + pw) : 0.f;
-                  gv = pow2 ? gv * inv_count : __fdiv_rn(gv, count);
-                }
-                float a = wx * gv;
-                if (flags & 1) a = ordered_group_sum(a, group);
-                if (leader) {
-                  if (lo_j >= r0) plane[lo_j * W + col] += (1.f - l_j) * a;               // lo_j < r1 holds for in-band samples
-                  if (l_j > 0.f && lo_j + 1 >= r0 && lo_j + 1 < r1) plane[(lo_j + 1) * W + col] += l_j * a;
-                }
-              }
-              __syncwarp();      // the next chunk's lanes may own the same words
-            }
-          }
-        }
+        const int4 h = hnext;
+        hnext = header(n0 + 32 + lane);
+        const bool hit = n0 + lane < K && h.x == b && h.y < r1 && h.z >= r0;
+        chunk(plane, c, n0, __ballot_sync(0xffffffffu, hit), h.w, r0, r1);
       }
     }
     __syncthreads();
@@ -197,106 +141,129 @@ roi_align_bwd_plane_kernel(const float* __restrict__ grad, const BwdHdr* __restr
   }
 }
 
-// Same algorithm for the common shapes (PH*sr <= 32 y samples, 2*PW*sr <= 32 x taps, PH*PW <= 64 bins - e.g. 7x7 bins with
-// sampling_ratio 2): a hit needs one table load per lane and two coalesced loads of the RoI's bin gradients, all
-// independent of each other, so they are issued for hit i+1 BEFORE hit i is processed (the general kernel above chains
-// three L2 round trips per hit and is latency-bound); the bin gradient of a (sample, tap) pair is then a shuffle.
+// Entry k of an axis table of n entries; past the end: no sample (lo = -1) / no tap (~0), weight 0.
+__device__ __forceinline__ uint2 table_entry(const uint2* __restrict__ table, int k, int n) {
+  return k < n ? __ldg(table + k) : make_uint2(0xffffffffu, 0u);
+}
+
+// What a roi_align plane kernel needs of RoI n before it walks the RoI: the first 32 entries of its y and x tables and the
+// first nb_regs (PH * PW when at most 64, else 0) bin gradients of channel c, two registers per lane.  The loads are
+// independent of each other, so the kernels issue them for the next RoI before processing the current one.
 struct HitLoads { uint2 yy, e; float gA, gB; };
 
+__device__ __forceinline__ HitLoads load_hit(const float* __restrict__ grad, const uint2* __restrict__ ys, const uint2* __restrict__ xe,
+                                             int n, int c, int C, int NYS, int NXE, int NB, int nb_regs) {
+  const int lane = threadIdx.x & 31;
+  const float* __restrict__ g = grad + ((int64_t)n * C + c) * NB;
+  HitLoads L;
+  L.yy = table_entry(ys + (int64_t)n * NYS, lane, NYS);
+  L.e = table_entry(xe + (int64_t)n * NXE, lane, NXE);
+  L.gA = lane < nb_regs ? __ldg(g + lane) : 0.f;
+  L.gB = lane + 32 < nb_regs ? __ldg(g + 32 + lane) : 0.f;
+  return L;
+}
+
+// Bin gradient t < 64 out of the registers load_hit filled; every lane must call it.
+__device__ __forceinline__ float bin_grad(const HitLoads& L, int t) {
+  const float ga = __shfl_sync(0xffffffffu, L.gA, t & 31), gb = __shfl_sync(0xffffffffu, L.gB, t & 31);
+  return t < 32 ? ga : gb;
+}
+
+// ---- roi_align backward, plane-resident ----------------------------------------------------------------------
+// grad [K, C, PH, PW] contiguous fp32; grad_input [B, C, H, W] written in full.
+// Row-owning: a hit walks the RoI's y samples and x taps in 32-entry chunks, the next hit's first chunks and bin gradients
+// loading meanwhile.  Lanes are x taps; for each y sample of the chunk that lands in the band, the leader of every group of
+// taps on the same column adds the group's sum, in lane order, into the sample's two rows.  Per word the order is RoI, y
+// chunk, x chunk, sample.  kOneChunk: at most 32 y samples, 32 x taps and 64 bins (7x7 bins with sampling_ratio 2), where
+// the chunk loops and bin-row bookkeeping compiled out keep the per-sample path short.
+template <bool kOneChunk>
 __global__ void __launch_bounds__(kBwdThreads, 1)
-roi_align_bwd_plane_fast_kernel(const float* __restrict__ grad, const BwdHdr* __restrict__ hdr, const uint2* __restrict__ ys,
-                                const uint2* __restrict__ xe, float* __restrict__ grad_input, int B, int C, int H, int W, int K,
-                                int PH, int PW, int sr, int band) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  float* plane = reinterpret_cast<float*>(smem_raw);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+roi_align_bwd_plane_kernel(const float* __restrict__ grad, const BwdHdr* __restrict__ hdr, const uint2* __restrict__ ys,
+                           const uint2* __restrict__ xe, float* __restrict__ grad_input, int B, int C, int H, int W, int K,
+                           int PH, int PW, int sr, int band) {
+  const int lane = threadIdx.x & 31;
   const int NYS = PH * sr, NXE = 2 * PW * sr, NB = PH * PW;
-  const float inv_count = 1.0f / (float)(sr * sr);
+  const bool bins_in_regs = kOneChunk || NB <= 64;            // bin gradients from load_hit's registers
+  const float inv_count = 1.0f / (float)(sr * sr);         // exact for sr = 1, 2, 4; sr = 3 differs from /9 by one rounding
   const bool pow2 = (sr & (sr - 1)) == 0;
   const float count = (float)(sr * sr);
-  const unsigned sr_recip = (65536u + (unsigned)sr - 1u) / (unsigned)sr;      // j / sr == (j * sr_recip) >> 16 for j < 32, sr <= 32
-  const int r0 = warp * band, r1 = min(H, r0 + band);
-  const int4* __restrict__ hdr4 = reinterpret_cast<const int4*>(hdr);
-  for (int pl = blockIdx.x; pl < B * C; pl += gridDim.x) {
-    const int b = pl / C, c = pl - b * C;
-    zero_plane(plane, H * W);
-    __syncthreads();
-    if (r0 < H) {
-      auto issue = [&](HitLoads& L, int n) {
-        const float* __restrict__ g = grad + ((int64_t)n * C + c) * NB;
-        L.yy = lane < NYS ? __ldg(ys + (int64_t)n * NYS + lane) : make_uint2(0xffffffffu, 0u);
-        L.e = lane < NXE ? __ldg(xe + (int64_t)n * NXE + lane) : make_uint2(0xffffffffu, 0u);
-        L.gA = lane < NB ? __ldg(g + lane) : 0.f;
-        L.gB = lane + 32 < NB ? __ldg(g + 32 + lane) : 0.f;
-      };
-      int4 hnext = make_int4(-1, 0, -1, 0);
-      if (lane < K) hnext = __ldg(hdr4 + lane);
-      for (int n0 = 0; n0 < K; n0 += 32) {
-        const int4 h = hnext;
-        hnext = make_int4(-1, 0, -1, 0);
-        if (n0 + 32 + lane < K) hnext = __ldg(hdr4 + n0 + 32 + lane);           // next chunk's headers travel under this chunk's hits
-        const bool hit = (n0 + lane < K) && h.x == b && h.y < r1 && h.z >= r0;
-        unsigned m = __ballot_sync(0xffffffffu, hit);
-        HitLoads cur, nxt;
-        if (m) issue(cur, n0 + __ffs(m) - 1);
-        while (m) {
-          const int i = __ffs(m) - 1;
-          m &= m - 1;
-          if (m) issue(nxt, n0 + __ffs(m) - 1);
-          const int flags = __shfl_sync(0xffffffffu, h.w, i);
-          const int lo = (int)cur.yy.x;
-          const float l = __uint_as_float(cur.yy.y);
-          const bool inb = lo >= 0 && lo < r1 && (lo + (l > 0.f ? 1 : 0)) >= r0;
-          unsigned mm = __ballot_sync(0xffffffffu, inb);
-          const bool valid = cur.e.x != 0xffffffffu;
-          const int col = (int)(cur.e.x & 0xffffu), pw = (int)(cur.e.x >> 16);
-          const float wx = __uint_as_float(cur.e.y);
+  const unsigned sr_recip = (65536u + (unsigned)sr - 1u) / (unsigned)sr;      // j / sr == (j * sr_recip) >> 16 for j < 64, sr <= 8
+  row_owning_planes(grad_input, B, C, H, W, K, band, 1, [&](int) { return reinterpret_cast<const int4*>(hdr); },
+                    [&](float* plane, int c, int n0, unsigned m, int flags_l, int r0, int r1) {
+    HitLoads cur, nxt;
+    if (m) cur = load_hit(grad, ys, xe, n0 + __ffs(m) - 1, c, C, NYS, NXE, NB, bins_in_regs ? NB : 0);
+    while (m) {
+      const int i = __ffs(m) - 1;
+      m &= m - 1;
+      if (m) nxt = load_hit(grad, ys, xe, n0 + __ffs(m) - 1, c, C, NYS, NXE, NB, bins_in_regs ? NB : 0);
+      const int n = n0 + i;
+      const bool dup = __shfl_sync(0xffffffffu, flags_l, i) & 1;
+      const float* __restrict__ g = grad + ((int64_t)n * C + c) * NB;
+      int q0 = 0, s0 = 0;                                  // yc / sr, yc % sr: sample yc + j is in bin row q0 + (s0 + j) / sr
+      for (int yc = 0; kOneChunk ? yc == 0 : yc < NYS; yc += 32) {
+        const uint2 yy = yc ? table_entry(ys + (int64_t)n * NYS, yc + lane, NYS) : cur.yy;
+        const int lo = (int)yy.x;
+        const float l = __uint_as_float(yy.y);
+        const bool inb = lo >= 0 && lo < r1 && (lo + (l > 0.f ? 1 : 0)) >= r0;
+        const unsigned ymask = __ballot_sync(0xffffffffu, inb);
+        for (int xc = 0; ymask && (kOneChunk ? xc == 0 : xc < NXE); xc += 32) {
+          const uint2 e = xc ? table_entry(xe + (int64_t)n * NXE, xc + lane, NXE) : cur.e;
+          const bool valid = e.x != 0xffffffffu;
+          const int col = (int)(e.x & 0xffffu), pw = (int)(e.x >> 16);
+          const float wx = __uint_as_float(e.y);
           bool leader = valid;
           unsigned group = 0u;
-          if (flags & 1) {
+          if (dup) {
             const unsigned same = __match_any_sync(0xffffffffu, valid ? col : 0x10000 + lane);
             group = valid ? same : 0u;
             leader = valid && (__ffs(same) - 1 == lane);
           }
+          unsigned mm = ymask;
+          int cur_ph = -1;
+          float gv = 0.f;
           while (mm) {
             const int j = __ffs(mm) - 1;
             mm &= mm - 1;
             const int lo_j = __shfl_sync(0xffffffffu, lo, j);
             const float l_j = __shfl_sync(0xffffffffu, l, j);
-            const int ph = (int)(((unsigned)j * sr_recip) >> 16);
-            const int t = valid ? ph * PW + pw : 0;
-            const float ga = __shfl_sync(0xffffffffu, cur.gA, t & 31), gb = __shfl_sync(0xffffffffu, cur.gB, t & 31);
-            float gv = t < 32 ? ga : gb;
-            gv = pow2 ? gv * inv_count : __fdiv_rn(gv, count);
+            const int ph = q0 + (int)(((unsigned)(s0 + j) * sr_recip) >> 16);
+            if (bins_in_regs || ph != cur_ph) {            // warp-uniform: from registers, or a new bin row from memory
+              cur_ph = ph;
+              gv = bins_in_regs ? bin_grad(cur, valid ? ph * PW + pw : 0) : valid ? __ldg(g + ph * PW + pw) : 0.f;
+              gv = pow2 ? gv * inv_count : __fdiv_rn(gv, count);
+            }
             float a = wx * gv;
-            if (flags & 1) a = ordered_group_sum(a, group);
+            if (dup) a = ordered_group_sum(a, group);
             if (leader) {
-              if (lo_j >= r0) plane[lo_j * W + col] += (1.f - l_j) * a;
+              if (lo_j >= r0) plane[lo_j * W + col] += (1.f - l_j) * a;               // lo_j < r1 holds for in-band samples
               if (l_j > 0.f && lo_j + 1 >= r0 && lo_j + 1 < r1) plane[(lo_j + 1) * W + col] += l_j * a;
             }
           }
-          cur = nxt;
+          // The next chunk's lanes may own the same words.  A one-chunk hit goes without: the next hit's full-warp shuffles
+          // converge the warp before its adds, and the barrier costs 8% at 7x7 (H100 80GB HBM3, 400 W power limit).
+          if (!kOneChunk) __syncwarp();
         }
+        const int d = (int)(((unsigned)(s0 + 32) * sr_recip) >> 16);
+        q0 += d;
+        s0 += 32 - d * sr;
       }
+      cur = nxt;
     }
-    __syncthreads();
-    store_plane(grad_input + (int64_t)pl * H * W, plane, H * W);
-    __syncthreads();
-  }
+  });
 }
 
-// Non-deterministic sibling of the two kernels above (the default unless the caller asks for determinism): the plane is
-// still resident, but RoIs are dealt to the warps round-robin and every tap is a shared-memory atomic add, so no work is
-// repeated per band (the ownership scheme pays ~10 band hits per RoI).  The shared-memory atomics are cheap while contention
-// is low - a warp's 28 taps of one line hit distinct columns.  The result differs
-// from run to run only in the summation order, as the reference's own atomic kernel does.
+// Non-deterministic sibling of the kernel above (the default for PH * sr <= 32 y samples, 2 * PW * sr <= 32 x taps and
+// PH * PW <= 64 bins unless the caller asks for determinism): the plane is still resident, but RoIs are dealt to the warps
+// round-robin and every tap is a shared-memory atomic add, so no work is repeated per band (the ownership scheme pays ~10
+// band hits per RoI).  The shared-memory atomics are cheap while contention is low - a warp's 28 taps of one line hit
+// distinct columns.  The result differs from run to run only in the summation order, as the reference's own atomic kernel does.
 __global__ void __launch_bounds__(kBwdThreads, 1)
 roi_align_bwd_plane_atomic_kernel(const float* __restrict__ grad, const BwdHdr* __restrict__ hdr, const uint2* __restrict__ ys,
                                   const uint2* __restrict__ xe, float* __restrict__ grad_input, int B, int C, int H, int W, int K,
                                   int PH, int PW, int sr) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* plane = reinterpret_cast<float*>(smem_raw);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, NW = blockDim.x >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, NW = blockDim.x >> 5;
   const int NYS = PH * sr, NXE = 2 * PW * sr, NB = PH * PW;
   const float inv_count = 1.0f / (float)(sr * sr);
   const bool pow2 = (sr & (sr - 1)) == 0;
@@ -307,12 +274,8 @@ roi_align_bwd_plane_atomic_kernel(const float* __restrict__ grad, const BwdHdr* 
     zero_plane(plane, H * W);
     __syncthreads();
     auto issue = [&](HitLoads& L, int& batch, int n) {
-      const float* __restrict__ g = grad + ((int64_t)n * C + c) * NB;
       batch = __ldg(&hdr[n].batch);
-      L.yy = lane < NYS ? __ldg(ys + (int64_t)n * NYS + lane) : make_uint2(0xffffffffu, 0u);
-      L.e = lane < NXE ? __ldg(xe + (int64_t)n * NXE + lane) : make_uint2(0xffffffffu, 0u);
-      L.gA = lane < NB ? __ldg(g + lane) : 0.f;
-      L.gB = lane + 32 < NB ? __ldg(g + 32 + lane) : 0.f;
+      L = load_hit(grad, ys, xe, n, c, C, NYS, NXE, NB, NB);
     };
     HitLoads cur, nxt;
     int cur_b = -1, nxt_b = -1;
@@ -336,9 +299,7 @@ roi_align_bwd_plane_atomic_kernel(const float* __restrict__ grad, const BwdHdr* 
           const int ph = (int)(((unsigned)j * sr_recip) >> 16);
           if (ph != cur_ph) {                       // warp-uniform: a new bin row
             cur_ph = ph;
-            const int t = valid ? ph * PW + pw : 0;
-            const float ga = __shfl_sync(0xffffffffu, cur.gA, t & 31), gb = __shfl_sync(0xffffffffu, cur.gB, t & 31);
-            const float gv = t < 32 ? ga : gb;
+            const float gv = bin_grad(cur, valid ? ph * PW + pw : 0);
             a = wx * (pow2 ? gv * inv_count : __fdiv_rn(gv, count));
           }
           if (valid) {
@@ -374,46 +335,27 @@ __global__ void roi_pool_bwd_hdr_kernel(const float* __restrict__ rois, BwdHdr* 
 __global__ void __launch_bounds__(kBwdThreads, 1)
 roi_pool_bwd_plane_kernel(const float* __restrict__ grad, const int32_t* __restrict__ argmax, const BwdHdr* __restrict__ hdr,
                           float* __restrict__ grad_input, int B, int C, int H, int W, int K, int NB, int band) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  float* plane = reinterpret_cast<float*>(smem_raw);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int r0 = warp * band, r1 = min(H, r0 + band);
-  for (int pl = blockIdx.x; pl < B * C; pl += gridDim.x) {
-    const int b = pl / C, c = pl - b * C;
-    zero_plane(plane, H * W);
-    __syncthreads();
-    if (r0 < H) {
-      const int lo_idx = r0 * W, hi_idx = r1 * W;          // flat argmax range of this band
-      for (int n0 = 0; n0 < K; n0 += 32) {
-        const int nl = n0 + lane;
-        bool hit = false;
-        if (nl < K) {
-          const int4 h = __ldg(reinterpret_cast<const int4*>(hdr) + nl);
-          hit = h.x == b && h.y < r1 && h.z >= r0;
-        }
-        unsigned m = __ballot_sync(0xffffffffu, hit);
-        while (m) {
-          const int i = __ffs(m) - 1;
-          m &= m - 1;
-          const int64_t base = ((int64_t)(n0 + i) * C + c) * NB;
-          for (int k0 = 0; k0 < NB; k0 += 32) {
-            int am = -1;
-            float gv = 0.f;
-            if (k0 + lane < NB) { am = __ldg(argmax + base + k0 + lane); gv = __ldg(grad + base + k0 + lane); }
-            const bool mine = am >= lo_idx && am < hi_idx;
-            // overlapping bin windows may share their maximum: merge equal targets in lane (= bin) order
-            const unsigned same = __match_any_sync(0xffffffffu, mine ? am : -2 - lane);
-            const float sum = ordered_group_sum(gv, mine ? same : 0u);
-            if (mine && (__ffs(same) - 1 == lane)) plane[am] += sum;
-            __syncwarp();
-          }
-        }
+  const int lane = threadIdx.x & 31;
+  row_owning_planes(grad_input, B, C, H, W, K, band, 1, [&](int) { return reinterpret_cast<const int4*>(hdr); },
+                    [&](float* plane, int c, int n0, unsigned m, int, int r0, int r1) {
+    const int lo_idx = r0 * W, hi_idx = r1 * W;          // flat argmax range of this band
+    while (m) {
+      const int i = __ffs(m) - 1;
+      m &= m - 1;
+      const int64_t base = ((int64_t)(n0 + i) * C + c) * NB;
+      for (int k0 = 0; k0 < NB; k0 += 32) {
+        int am = -1;
+        float gv = 0.f;
+        if (k0 + lane < NB) { am = __ldg(argmax + base + k0 + lane); gv = __ldg(grad + base + k0 + lane); }
+        const bool mine = am >= lo_idx && am < hi_idx;
+        // overlapping bin windows may share their maximum: merge equal targets in lane (= bin) order
+        const unsigned same = __match_any_sync(0xffffffffu, mine ? am : -2 - lane);
+        const float sum = ordered_group_sum(gv, mine ? same : 0u);
+        if (mine && (__ffs(same) - 1 == lane)) plane[am] += sum;
+        __syncwarp();
       }
     }
-    __syncthreads();
-    store_plane(grad_input + (int64_t)pl * H * W, plane, H * W);
-    __syncthreads();
-  }
+  });
 }
 
 // ---- ps_roi_align backward, plane-resident -------------------------------------------------------------------
@@ -440,67 +382,51 @@ __global__ void __launch_bounds__(kBwdThreads, 1)
 ps_roi_align_bwd_plane_kernel(const float* __restrict__ grad, const BwdHdr* __restrict__ hdr_ph, const uint2* __restrict__ ys,
                               const uint2* __restrict__ xe, float* __restrict__ grad_input, int B, int C, int H, int W, int K,
                               int PH, int PW, int Cout, int sr, int band) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  float* plane = reinterpret_cast<float*>(smem_raw);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int lane = threadIdx.x & 31;
   const int NYS = PH * sr, NXE = 2 * PW * sr;
-  const int r0 = warp * band, r1 = min(H, r0 + band);
   const bool pow2 = (sr & (sr - 1)) == 0;
   const float inv_count = 1.0f / (float)(sr * sr), count = (float)(sr * sr);
   const int ntap = sr * 2 * sr;                 // lanes of one bin: (iy, k)
-  for (int pl = blockIdx.x; pl < B * C; pl += gridDim.x) {
-    const int b = pl / C, c_in = pl - b * C;
-    const int pw = c_in % PW, ph = (c_in / PW) % PH, co = c_in / (PW * PH);
-    zero_plane(plane, H * W);
-    __syncthreads();
-    if (r0 < H && co < Cout) {
-      for (int n0 = 0; n0 < K; n0 += 32) {
-        const int nl = n0 + lane;
-        bool hit = false;
-        if (nl < K) {
-          const int4 h = __ldg(reinterpret_cast<const int4*>(hdr_ph) + (int64_t)nl * PH + ph);
-          hit = h.x == b && h.y < r1 && h.z >= r0;
+  int pw, ph, co;                               // of the current plane; channels past Cout * PH * PW receive nothing
+  auto hdr_of = [&](int c_in) {
+    pw = c_in % PW; ph = (c_in / PW) % PH; co = c_in / (PW * PH);
+    return co < Cout ? reinterpret_cast<const int4*>(hdr_ph) + ph : nullptr;
+  };
+  row_owning_planes(grad_input, B, C, H, W, K, band, PH, hdr_of, [&](float* plane, int, int n0, unsigned m, int, int r0, int r1) {
+    while (m) {
+      const int i = __ffs(m) - 1;
+      m &= m - 1;
+      const int n = n0 + i;
+      float gv = __ldg(grad + (((int64_t)n * Cout + co) * PH + ph) * PW + pw);
+      gv = pow2 ? gv * inv_count : __fdiv_rn(gv, count);
+      for (int t0 = 0; t0 < ntap; t0 += 32) {
+        const int t = t0 + lane;
+        int lo = -1, col = 0;
+        float l = 0.f, wx = 0.f;
+        bool valid = false;
+        if (t < ntap) {
+          const int iy = t / (2 * sr), k = t - iy * 2 * sr;
+          const uint2 yy = __ldg(ys + (int64_t)n * NYS + ph * sr + iy);
+          const uint2 e = __ldg(xe + (int64_t)n * NXE + pw * 2 * sr + k);
+          lo = (int)yy.x; l = __uint_as_float(yy.y);
+          valid = lo >= 0 && e.x != 0xffffffffu;
+          col = (int)(e.x & 0xffffu); wx = __uint_as_float(e.y);
         }
-        unsigned m = __ballot_sync(0xffffffffu, hit);
-        while (m) {
-          const int i = __ffs(m) - 1;
-          m &= m - 1;
-          const int n = n0 + i;
-          float gv = __ldg(grad + (((int64_t)n * Cout + co) * PH + ph) * PW + pw);
-          gv = pow2 ? gv * inv_count : __fdiv_rn(gv, count);
-          for (int t0 = 0; t0 < ntap; t0 += 32) {
-            const int t = t0 + lane;
-            int lo = -1, col = 0;
-            float l = 0.f, wx = 0.f;
-            bool valid = false;
-            if (t < ntap) {
-              const int iy = t / (2 * sr), k = t - iy * 2 * sr;
-              const uint2 yy = __ldg(ys + (int64_t)n * NYS + ph * sr + iy);
-              const uint2 e = __ldg(xe + (int64_t)n * NXE + pw * 2 * sr + k);
-              lo = (int)yy.x; l = __uint_as_float(yy.y);
-              valid = lo >= 0 && e.x != 0xffffffffu;
-              col = (int)(e.x & 0xffffu); wx = __uint_as_float(e.y);
-            }
-            const float a = wx * gv;
+        const float a = wx * gv;
 #pragma unroll
-            for (int cy = 0; cy < 2; ++cy) {
-              const int row = lo + cy;
-              const float wy = cy ? l : 1.f - l;
-              const bool mine = valid && wy != 0.f && row >= r0 && row < r1;
-              const int addr = row * W + col;
-              const unsigned same = __match_any_sync(0xffffffffu, mine ? addr : -2 - lane);
-              const float sum = ordered_group_sum(wy * a, mine ? same : 0u);
-              if (mine && (__ffs(same) - 1 == lane)) plane[addr] += sum;
-              __syncwarp();
-            }
-          }
+        for (int cy = 0; cy < 2; ++cy) {
+          const int row = lo + cy;
+          const float wy = cy ? l : 1.f - l;
+          const bool mine = valid && wy != 0.f && row >= r0 && row < r1;
+          const int addr = row * W + col;
+          const unsigned same = __match_any_sync(0xffffffffu, mine ? addr : -2 - lane);
+          const float sum = ordered_group_sum(wy * a, mine ? same : 0u);
+          if (mine && (__ffs(same) - 1 == lane)) plane[addr] += sum;
+          __syncwarp();
         }
       }
     }
-    __syncthreads();
-    store_plane(grad_input + (int64_t)pl * H * W, plane, H * W);
-    __syncthreads();
-  }
+  });
 }
 
 // ---- generic atomic scatter (any dtype / adaptive sampling / plane too large) ---------------------------------
@@ -610,10 +536,12 @@ BwdWs carve_bwd(void* base, int K, int PH, int PW, int sr) {
   return w;
 }
 
+size_t plane_smem_bytes(int H, int W) { return (((size_t)H * W + 3) & ~(size_t)3) * 4; }
+
 // plane path: fp32, fixed sampling grid, plane fits shared memory, 16-bit column / bin fields
 bool bwd_plane_ok(int dtype, int H, int W, int PH, int PW, int sr, bool need_sr) {
   if (dtype != VB200_F32) return false;
-  if ((size_t)(((size_t)H * W + 3) & ~(size_t)3) * 4 + 1024 > (size_t)max_smem_optin()) return false;
+  if (plane_smem_bytes(H, W) + 1024 > (size_t)max_smem_optin()) return false;
   if (W >= 65536 || PW >= 65536 || H < 1 || W < 1) return false;
   if (need_sr && (sr < 1 || sr > 8)) return false;
   const char* force = env_override(ENV_ROI_BWD_PATH);      // "atomic" pins the generic kernel (testing)
@@ -622,6 +550,38 @@ bool bwd_plane_ok(int dtype, int H, int W, int PH, int PW, int sr, bool need_sr)
 }
 
 int bwd_band(int H) { return ceil_div(H, kBwdThreads / 32); }
+
+// A plane kernel on `planes` (image, channel) planes of H x W: persistent CTAs, at most one per SM, the plane in dynamic
+// shared memory.
+template <auto kernel, typename... Args>
+int launch_plane(const char* name, int planes, int H, int W, cudaStream_t st, Args... args) {
+  const size_t smem = plane_smem_bytes(H, W);
+  VB200_CUDA_TRY(ensure_dyn_smem<kernel>(smem));
+  kernel<<<planes < sm_count() ? planes : sm_count(), kBwdThreads, smem, st>>>(args...);
+  return check_launch(name);
+}
+
+// Checks shared by the backward entry points; `bytes` is set to the size of grad_input [batch, channels, height, width],
+// 0 when it is empty and there is nothing to do.
+int bwd_prologue(const char* op, const void* grad_input, int dtype, int batch, int channels, int height, int width, int num_rois,
+                 int pooled_h, int pooled_w, size_t& bytes) {
+  bytes = 0;
+  VB200_REQUIRE(pooled_h > 0 && pooled_w > 0, "%s: pooled size must be positive", op);
+  VB200_REQUIRE(batch >= 0 && channels >= 0 && height >= 0 && width >= 0 && num_rois >= 0, "%s: negative size", op);
+  const int64_t in_elems = (int64_t)batch * channels * height * width;
+  if (in_elems == 0) return 0;
+  VB200_REQUIRE(grad_input, "%s: null grad_input", op);
+  VB200_REQUIRE(in_elems < (1ll << 31), "%s: tensor too large for 32-bit indexing", op);
+  VB200_REQUIRE(dtype == VB200_F32 || dtype == VB200_F64 || dtype == VB200_F16, "%s: unsupported dtype %d", op, dtype);
+  bytes = (size_t)in_elems * (dtype == VB200_F64 ? 8 : dtype == VB200_F16 ? 2 : 4);
+  return 0;
+}
+
+// grad_input zeroed for the atomic scatter kernels, or as the whole result when no RoI contributes
+int zero_fill(void* grad_input, size_t bytes, cudaStream_t st) {
+  VB200_CUDA_TRY(cudaMemsetAsync(grad_input, 0, bytes, st));
+  return 0;
+}
 
 }  // namespace
 }  // namespace vb200
@@ -637,17 +597,15 @@ extern "C" int vb200_roi_align_backward(const void* grad, const void* rois, void
                                         int channels, int height, int width, int num_rois, int pooled_h, int pooled_w,
                                         double spatial_scale, int sampling_ratio, int aligned, int deterministic,
                                         void* workspace, size_t workspace_bytes, vb200_stream stream) {
-  VB200_REQUIRE(batch >= 0 && channels >= 0 && height >= 0 && width >= 0 && num_rois >= 0, "roi_align_backward: negative size");
-  VB200_REQUIRE(pooled_h > 0 && pooled_w > 0, "roi_align_backward: pooled size must be positive");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t in_elems = (int64_t)batch * channels * height * width;
-  if (in_elems == 0) return 0;
-  VB200_REQUIRE(grad_input, "roi_align_backward: null grad_input");
-  VB200_REQUIRE(in_elems < (1ll << 31) && (int64_t)num_rois * channels * pooled_h * pooled_w < (1ll << 31),
+  size_t bytes;
+  if (int rc = bwd_prologue("roi_align_backward", grad_input, dtype, batch, channels, height, width, num_rois, pooled_h, pooled_w,
+                            bytes))
+    return rc;
+  if (bytes == 0) return 0;
+  VB200_REQUIRE((int64_t)num_rois * channels * pooled_h * pooled_w < (1ll << 31),
                 "roi_align_backward: tensor too large for 32-bit indexing");
-  const size_t esize = dtype == VB200_F64 ? 8 : dtype == VB200_F16 ? 2 : 4;
-  VB200_REQUIRE(dtype == VB200_F32 || dtype == VB200_F64 || dtype == VB200_F16, "roi_align_backward: unsupported dtype %d", dtype);
-  if (num_rois == 0) { VB200_CUDA_TRY(cudaMemsetAsync(grad_input, 0, (size_t)in_elems * esize, st)); return 0; }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (num_rois == 0) return zero_fill(grad_input, bytes, st);
   VB200_REQUIRE(grad && rois, "roi_align_backward: null pointer");
   const BwdWs ws = carve_bwd(workspace, num_rois, pooled_h, pooled_w, sampling_ratio);
   if (bwd_plane_ok(dtype, height, width, pooled_h, pooled_w, sampling_ratio, true) && workspace && workspace_bytes >= ws.total) {
@@ -656,31 +614,21 @@ extern "C" int vb200_roi_align_backward(const void* grad, const void* rois, void
                                                                            (float)spatial_scale, aligned, 0);
     int rc = check_launch("roi_bwd_geometry_kernel");
     if (rc) return rc;
-    const size_t smem = (((size_t)height * width + 3) & ~(size_t)3) * 4;
     const int planes = batch * channels;
-    const int grid = planes < sm_count() ? planes : sm_count();
     const bool small_tables = pooled_h * sampling_ratio <= 32 && 2 * pooled_w * sampling_ratio <= 32 && pooled_h * pooled_w <= 64;
-    if (small_tables && !deterministic) {
-      VB200_CUDA_TRY(ensure_dyn_smem<roi_align_bwd_plane_atomic_kernel>(smem));
-      roi_align_bwd_plane_atomic_kernel<<<grid, kBwdThreads, smem, st>>>((const float*)grad, ws.hdr, ws.ys, ws.xe,
-                                                                        (float*)grad_input, batch, channels, height, width, num_rois,
-                                                                        pooled_h, pooled_w, sampling_ratio);
-      return check_launch("roi_align_bwd_plane_atomic_kernel");
-    }
-    if (small_tables) {
-      VB200_CUDA_TRY(ensure_dyn_smem<roi_align_bwd_plane_fast_kernel>(smem));
-      roi_align_bwd_plane_fast_kernel<<<grid, kBwdThreads, smem, st>>>((const float*)grad, ws.hdr, ws.ys, ws.xe, (float*)grad_input,
-                                                                      batch, channels, height, width, num_rois, pooled_h, pooled_w,
-                                                                      sampling_ratio, bwd_band(height));
-      return check_launch("roi_align_bwd_plane_fast_kernel");
-    }
-    VB200_CUDA_TRY(ensure_dyn_smem<roi_align_bwd_plane_kernel>(smem));
-    roi_align_bwd_plane_kernel<<<grid, kBwdThreads, smem, st>>>((const float*)grad, ws.hdr, ws.ys, ws.xe, (float*)grad_input, batch,
-                                                               channels, height, width, num_rois, pooled_h, pooled_w, sampling_ratio,
-                                                               bwd_band(height));
-    return check_launch("roi_align_bwd_plane_kernel");
+    if (small_tables && !deterministic)
+      return launch_plane<roi_align_bwd_plane_atomic_kernel>("roi_align_bwd_plane_atomic_kernel", planes, height, width, st,
+                                                             (const float*)grad, ws.hdr, ws.ys, ws.xe, (float*)grad_input, batch,
+                                                             channels, height, width, num_rois, pooled_h, pooled_w, sampling_ratio);
+    if (small_tables)
+      return launch_plane<roi_align_bwd_plane_kernel<true>>("roi_align_bwd_plane_kernel", planes, height, width, st, (const float*)grad,
+                                                    ws.hdr, ws.ys, ws.xe, (float*)grad_input, batch, channels, height, width,
+                                                    num_rois, pooled_h, pooled_w, sampling_ratio, bwd_band(height));
+    return launch_plane<roi_align_bwd_plane_kernel<false>>("roi_align_bwd_plane_kernel", planes, height, width, st, (const float*)grad,
+                                                    ws.hdr, ws.ys, ws.xe, (float*)grad_input, batch, channels, height, width,
+                                                    num_rois, pooled_h, pooled_w, sampling_ratio, bwd_band(height));
   }
-  VB200_CUDA_TRY(cudaMemsetAsync(grad_input, 0, (size_t)in_elems * esize, st));
+  if (int rc = zero_fill(grad_input, bytes, st)) return rc;
   const int ch_per_cta = channels >= 64 ? 32 : (channels >= 16 ? 16 : channels);
   dim3 grid((unsigned)num_rois, (unsigned)ceil_div(channels, ch_per_cta));
   return dispatch_roi_dtype(dtype, "roi_align_backward: unsupported dtype %d", [&](auto t) {
@@ -697,17 +645,14 @@ extern "C" int vb200_ps_roi_align_backward(const void* grad, const void* rois, c
                                            int pooled_w, double spatial_scale, int sampling_ratio, int deterministic,
                                            void* workspace, size_t workspace_bytes, vb200_stream stream) {
   (void)channel_mapping;   // c_in = (c_out * PH + ph) * PW + pw by construction (ps_roi_align_kernel.cu:95); not re-read
-  VB200_REQUIRE(pooled_h > 0 && pooled_w > 0, "ps_roi_align_backward: pooled size must be positive");
-  VB200_REQUIRE(batch >= 0 && channels >= 0 && height >= 0 && width >= 0 && num_rois >= 0, "ps_roi_align_backward: negative size");
+  size_t bytes;
+  if (int rc = bwd_prologue("ps_roi_align_backward", grad_input, dtype, batch, channels, height, width, num_rois, pooled_h,
+                            pooled_w, bytes))
+    return rc;
+  if (bytes == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  const int64_t in_elems = (int64_t)batch * channels * height * width;
-  if (in_elems == 0) return 0;
-  VB200_REQUIRE(grad_input, "ps_roi_align_backward: null grad_input");
-  VB200_REQUIRE(in_elems < (1ll << 31), "ps_roi_align_backward: tensor too large for 32-bit indexing");
-  VB200_REQUIRE(dtype == VB200_F32 || dtype == VB200_F64 || dtype == VB200_F16, "ps_roi_align_backward: unsupported dtype %d", dtype);
-  const size_t esize = dtype == VB200_F64 ? 8 : dtype == VB200_F16 ? 2 : 4;
   const int Cout = channels / (pooled_h * pooled_w);
-  if (num_rois == 0 || Cout == 0) { VB200_CUDA_TRY(cudaMemsetAsync(grad_input, 0, (size_t)in_elems * esize, st)); return 0; }
+  if (num_rois == 0 || Cout == 0) return zero_fill(grad_input, bytes, st);
   VB200_REQUIRE(grad && rois, "ps_roi_align_backward: null pointer");
   const BwdWs ws = carve_bwd(workspace, num_rois, pooled_h, pooled_w, sampling_ratio);
   // One bin per (RoI, plane): the atomic scatter is the faster kernel here (sr*sr*4 atomics per output); the plane kernel is
@@ -723,15 +668,12 @@ extern "C" int vb200_ps_roi_align_backward(const void* grad, const void* rois, c
                                                                                     sampling_ratio);
     rc = check_launch("ps_roi_align_bwd_hdr_kernel");
     if (rc) return rc;
-    const size_t smem = (((size_t)height * width + 3) & ~(size_t)3) * 4;
-    VB200_CUDA_TRY(ensure_dyn_smem<ps_roi_align_bwd_plane_kernel>(smem));
-    const int planes = batch * channels;
-    ps_roi_align_bwd_plane_kernel<<<planes < sm_count() ? planes : sm_count(), kBwdThreads, smem, st>>>(
-        (const float*)grad, ws.hdr_ph, ws.ys, ws.xe, (float*)grad_input, batch, channels, height, width, num_rois, pooled_h,
-        pooled_w, Cout, sampling_ratio, bwd_band(height));
-    return check_launch("ps_roi_align_bwd_plane_kernel");
+    return launch_plane<ps_roi_align_bwd_plane_kernel>("ps_roi_align_bwd_plane_kernel", batch * channels, height, width, st,
+                                                       (const float*)grad, ws.hdr_ph, ws.ys, ws.xe, (float*)grad_input, batch,
+                                                       channels, height, width, num_rois, pooled_h, pooled_w, Cout, sampling_ratio,
+                                                       bwd_band(height));
   }
-  VB200_CUDA_TRY(cudaMemsetAsync(grad_input, 0, (size_t)in_elems * esize, st));
+  if (int rc = zero_fill(grad_input, bytes, st)) return rc;
   const int ch_per_cta = Cout >= 64 ? 32 : (Cout >= 16 ? 16 : Cout);
   dim3 grid((unsigned)num_rois, (unsigned)ceil_div(Cout, ch_per_cta));
   return dispatch_roi_dtype(dtype, "ps_roi_align_backward: unsupported dtype %d", [&](auto t) {
@@ -747,16 +689,13 @@ extern "C" int vb200_roi_pool_backward(const void* grad, const void* rois, const
                                        int batch, int channels, int height, int width, int num_rois, int pooled_h, int pooled_w,
                                        double spatial_scale, int deterministic, void* workspace, size_t workspace_bytes,
                                        vb200_stream stream) {
-  VB200_REQUIRE(pooled_h > 0 && pooled_w > 0, "roi_pool_backward: pooled size must be positive");
-  VB200_REQUIRE(batch >= 0 && channels >= 0 && height >= 0 && width >= 0 && num_rois >= 0, "roi_pool_backward: negative size");
+  size_t bytes;
+  if (int rc = bwd_prologue("roi_pool_backward", grad_input, dtype, batch, channels, height, width, num_rois, pooled_h, pooled_w,
+                            bytes))
+    return rc;
+  if (bytes == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  const int64_t in_elems = (int64_t)batch * channels * height * width;
-  if (in_elems == 0) return 0;
-  VB200_REQUIRE(grad_input, "roi_pool_backward: null grad_input");
-  VB200_REQUIRE(in_elems < (1ll << 31), "roi_pool_backward: tensor too large for 32-bit indexing");
-  VB200_REQUIRE(dtype == VB200_F32 || dtype == VB200_F64 || dtype == VB200_F16, "roi_pool_backward: unsupported dtype %d", dtype);
-  const size_t esize = dtype == VB200_F64 ? 8 : dtype == VB200_F16 ? 2 : 4;
-  if (num_rois == 0) { VB200_CUDA_TRY(cudaMemsetAsync(grad_input, 0, (size_t)in_elems * esize, st)); return 0; }
+  if (num_rois == 0) return zero_fill(grad_input, bytes, st);
   VB200_REQUIRE(grad && rois && argmax, "roi_pool_backward: null pointer");
   const BwdWs ws = carve_bwd(workspace, num_rois, pooled_h, pooled_w, 1);
   // one atomic per output element is hard to beat; the plane kernel is the bit-reproducible alternative
@@ -765,15 +704,11 @@ extern "C" int vb200_roi_pool_backward(const void* grad, const void* rois, const
                                                                      (float)spatial_scale);
     int rc = check_launch("roi_pool_bwd_hdr_kernel");
     if (rc) return rc;
-    const size_t smem = (((size_t)height * width + 3) & ~(size_t)3) * 4;
-    VB200_CUDA_TRY(ensure_dyn_smem<roi_pool_bwd_plane_kernel>(smem));
-    const int planes = batch * channels;
-    roi_pool_bwd_plane_kernel<<<planes < sm_count() ? planes : sm_count(), kBwdThreads, smem, st>>>(
-        (const float*)grad, argmax, ws.hdr, (float*)grad_input, batch, channels, height, width, num_rois, pooled_h * pooled_w,
-        bwd_band(height));
-    return check_launch("roi_pool_bwd_plane_kernel");
+    return launch_plane<roi_pool_bwd_plane_kernel>("roi_pool_bwd_plane_kernel", batch * channels, height, width, st, (const float*)grad,
+                                                   argmax, ws.hdr, (float*)grad_input, batch, channels, height, width, num_rois,
+                                                   pooled_h * pooled_w, bwd_band(height));
   }
-  VB200_CUDA_TRY(cudaMemsetAsync(grad_input, 0, (size_t)in_elems * esize, st));
+  if (int rc = zero_fill(grad_input, bytes, st)) return rc;
   const int64_t total = (int64_t)num_rois * channels * pooled_h * pooled_w;
   const int grid = (int)(ceil_div64(total, 256) < (int64_t)sm_count() * 16 ? ceil_div64(total, 256) : (int64_t)sm_count() * 16);
   return dispatch_roi_dtype(dtype, "roi_pool_backward: unsupported dtype %d", [&](auto t) {
@@ -787,15 +722,13 @@ extern "C" int vb200_roi_pool_backward(const void* grad, const void* rois, const
 extern "C" int vb200_ps_roi_pool_backward(const void* grad, const void* rois, void* grad_input, int dtype, int batch, int channels,
                                           int height, int width, int num_rois, int pooled_h, int pooled_w, double spatial_scale,
                                           vb200_stream stream) {
-  VB200_REQUIRE(pooled_h > 0 && pooled_w > 0, "ps_roi_pool_backward: pooled size must be positive");
-  const int64_t in_elems = (int64_t)batch * channels * height * width;
-  if (in_elems == 0) return 0;
-  VB200_REQUIRE(grad_input, "ps_roi_pool_backward: null grad_input");
-  VB200_REQUIRE(in_elems < (1ll << 31), "ps_roi_pool_backward: tensor too large for 32-bit indexing");
-  VB200_REQUIRE(dtype == VB200_F32 || dtype == VB200_F64 || dtype == VB200_F16, "ps_roi_pool_backward: unsupported dtype %d", dtype);
+  size_t bytes;
+  if (int rc = bwd_prologue("ps_roi_pool_backward", grad_input, dtype, batch, channels, height, width, num_rois, pooled_h, pooled_w,
+                            bytes))
+    return rc;
+  if (bytes == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t esize = dtype == VB200_F64 ? 8 : dtype == VB200_F16 ? 2 : 4;
-  VB200_CUDA_TRY(cudaMemsetAsync(grad_input, 0, (size_t)in_elems * esize, st));
+  if (int rc = zero_fill(grad_input, bytes, st)) return rc;
   const int Cout = channels / (pooled_h * pooled_w);
   const int64_t total = (int64_t)num_rois * Cout * pooled_h * pooled_w;
   if (total == 0) return 0;
