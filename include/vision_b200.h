@@ -322,6 +322,25 @@ VB200_API int vb200_deform_conv2d_backward_inputs(const void* dcol, const void* 
                                         void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs, int c_in,
                                         int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w,
                                         int dil_h, int dil_w, int offset_groups, int use_mask, vb200_stream stream);
+/* Bit-reproducible grad_input (the reference instead raises under torch.use_deterministic_algorithms,
+ * alertNotDeterministic("compute_grad_input"), deformable_col2im's caller :441).  With `deterministic` set,
+ * vb200_deform_conv2d_backward_inputs_ex writes grad_input IN FULL (no pre-zeroing) by a gather instead of the scatter: the
+ * samples are binned by the cell (floor y, floor x) they fall in and sorted stably, and each grad_input[b, c, y, x] is summed
+ * over the cells (y, x), (y, x-1), (y-1, x), (y-1, x-1) in that order, inside a cell in ascending (offset group, tap, output
+ * pixel) order, in fp32 (double for F64) and rounded once.  The value depends on image b's data alone.  grad_offset /
+ * grad_mask are the same as without the flag.  The workspace (vb200_deform_conv2d_backward_inputs_workspace_bytes, host
+ * arithmetic only, 0 for an empty shape) holds the sort keys, the cell table and one record per sample; images are processed
+ * in passes whose sample count fits int32 and key range fits 32 bits, and a shape whose single image exceeds that returns
+ * VB200_EUNSUPPORTED before anything is launched.  With deterministic == 0 the call is vb200_deform_conv2d_backward_inputs
+ * (workspace unused, grad_input pre-zeroed and scattered with atomics). */
+VB200_API size_t vb200_deform_conv2d_backward_inputs_workspace_bytes(int dtype, int n_imgs, int c_in, int in_h, int in_w, int kh, int kw,
+                                                           int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w,
+                                                           int offset_groups);
+VB200_API int vb200_deform_conv2d_backward_inputs_ex(const void* dcol, const void* input, const void* offset, const void* mask,
+                                           void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs, int c_in,
+                                           int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w,
+                                           int dil_h, int dil_w, int offset_groups, int use_mask, int deterministic,
+                                           void* workspace, size_t workspace_bytes, vb200_stream stream);
 
 /* ---- resize ------------------------------------------------------------
  * Replaces the interpolate path of resize_image,

@@ -1,6 +1,6 @@
 """Small driver for ncu captures: runs one op of the hot path a few times at its BASELINE shape.
     python tools/prof_ops.py roi_align|roi_pool|ps_roi_align|ps_roi_pool|batched_nms|nms|resize|resize128|resize_noaa|deform|deform_f32|
-                             roi_align_bwd|roi_align_bwd_det|roi_align_bwd14|roi_align_bwd14_det|multiscale|postprocess|preprocess [iters]
+                             deform_bwd|deform_bwd_det|deform_bwd_f32|deform_bwd_det_f32|roi_align_bwd|roi_align_bwd_det|roi_align_bwd14|roi_align_bwd14_det|multiscale|postprocess|preprocess [iters]
     python tools/prof_ops.py retinanet_post|fcos_post|ssd_post [iters]     fused vs. reference postprocess_detections,
                              batch 1 and 8, logits N(-4.595, 1) and N(-4.595, 0.5); select-kernel time from torch.profiler"""
 import os
@@ -170,6 +170,15 @@ elif op in ("deform", "deform_f32"):
     dt = torch.bfloat16 if op == "deform" else torch.float32
     xi, off, w, bi, m = [t.to(dev) for t in workloads.cfg4_deform_conv2d(batch=int(os.environ.get('DCN_BATCH', '32')), dtype=dt)]
     fn = lambda: vb.ops.deform_conv2d(xi, off, w, bi, 1, 1, 1, m)
+elif op in ("deform_bwd", "deform_bwd_det", "deform_bwd_f32", "deform_bwd_det_f32"):
+    # the whole deform_conv2d backward (two GEMMs + our kernels) at cfg4; _det: grad_input by the deterministic gather
+    import warnings
+    dt = torch.float32 if op.endswith("_f32") else torch.bfloat16
+    xi, off, w, bi, m = [t.to(dev) for t in workloads.cfg4_deform_conv2d(batch=int(os.environ.get('DCN_BATCH', '32')), dtype=dt)]
+    g = torch.randn(xi.shape[0], w.shape[0], xi.shape[2], xi.shape[3], device=dev).to(dt)
+    torch.use_deterministic_algorithms("_det" in op, warn_only=True)        # warn_only: the shim's GEMMs are cuBLAS
+    warnings.simplefilter("ignore", UserWarning)
+    fn = lambda: torch.ops.vision_b200._deform_conv2d_backward(g, xi, w, off, m, bi, 1, 1, 1, 1, 1, 1, 1, 1, True)
 else:
     raise SystemExit(f"unknown op {op}")
 for _ in range(2):

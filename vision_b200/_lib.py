@@ -43,7 +43,8 @@ def core() -> ctypes.CDLL:
                          "vb200_roi_align_workspace_bytes", "vb200_deform_conv2d_workspace_bytes",
                          "vb200_roi_backward_workspace_bytes", "vb200_multiscale_roi_align_workspace_bytes",
                          "vb200_detection_postprocess_workspace_bytes", "vb200_deform_conv2d_packed_weight_bytes",
-                         "vb200_single_stage_postprocess_workspace_bytes"):
+                         "vb200_single_stage_postprocess_workspace_bytes",
+                         "vb200_deform_conv2d_backward_inputs_workspace_bytes"):
                 getattr(lib, name).restype = ctypes.c_size_t
             _core = lib
         return _core
@@ -79,4 +80,5 @@ ABI_SYMBOLS = (
     "vb200_multiscale_roi_align_workspace_bytes", "vb200_multiscale_roi_align_supported", "vb200_multiscale_roi_align_forward",
     "vb200_roi_backward_workspace_bytes", "vb200_roi_align_backward", "vb200_roi_pool_backward", "vb200_ps_roi_align_backward",
     "vb200_single_stage_postprocess_workspace_bytes", "vb200_single_stage_postprocess",
+    "vb200_deform_conv2d_backward_inputs_workspace_bytes", "vb200_deform_conv2d_backward_inputs_ex",
 )

@@ -15,6 +15,24 @@
 //     grad_mask (sum dcol * bilinear), grad_offset (sum dcol * mask * d bilinear / d{y, x}) - written once, no atomics,
 //     deterministic - and scatters grad_input with atomics (as the reference does).
 // Arithmetic follows bilinear_interpolate (:97-134) and get_coordinate_weight (:503-536).
+//
+// Deterministic grad_input (torch.use_deterministic_algorithms): the scatter is turned into a gather.  A sample whose
+// cell (hl, wl) = (floor y, floor x) is known writes exactly the four pixels (hl, wl), (hl, wl+1), (hl+1, wl), (hl+1, wl+1),
+// so pixel (y, x) receives from the samples of the cells (y, x), (y, x-1), (y-1, x), (y-1, x-1) - as their corner 0, 1,
+// 2, 3.  Per pass of images:
+//   1. dcn_bin_samples_kernel: key = (image x offset group, cell) per sample; samples outside the image or with no
+//      contributing corner get a sentinel key that sorts last;
+//   2. cub::DeviceRadixSort::SortPairs(key, sample index): stable, so within a cell the samples keep ascending index;
+//   3. dcn_cell_start_kernel (first sorted position of every key, by binary search) and dcn_cell_records_kernel (per
+//      sorted sample: its dcol column tap*HWo + pix, the mask of contributing corners and mask * corner weight);
+//   4. dcn_grad_input_gather_kernel: every grad_input element written once, no atomics.
+// Summation order of grad_input[b, c, y, x]: cells (y, x), (y, x-1), (y-1, x), (y-1, x-1) in that order; inside a cell the
+// samples in ascending ((offset group, tap), output pixel) index; one accumulator of Acc<T> (fp32, double for F64), rounded
+// once to T.  It depends on image b's data alone, never on the other images of the call or on how they are split into passes.
+#include <cub/cub.cuh>
+
+#include <algorithm>
+
 #include "common.cuh"
 #include "dcn_params.h"
 
@@ -27,6 +45,7 @@ struct Sample {
   bool ok[4];        // corner inside the image
   A lh, lw;          // fractional parts
   bool inside;       // bilinear_interpolate's outer test: -1 < y < H and -1 < x < W
+  int hl, wl;        // the sample's cell: floor(y), floor(x)
 };
 
 template <typename A>
@@ -34,6 +53,7 @@ __device__ __forceinline__ Sample<A> make_sample(A y, A x, int H, int W) {
   Sample<A> s;
   const int hl = (int)floor(y), wl = (int)floor(x);
   const int hh = hl + 1, wh = wl + 1;
+  s.hl = hl; s.wl = wl;
   s.lh = y - (A)hl; s.lw = x - (A)wl;
   s.inside = !(y <= (A)-1 || (A)H <= y || x <= (A)-1 || (A)W <= x);
   const bool t0 = hl >= 0 && hl < H, t1 = hh >= 0 && hh < H, l0 = wl >= 0 && wl < W, l1 = wh >= 0 && wh < W;
@@ -43,6 +63,35 @@ __device__ __forceinline__ Sample<A> make_sample(A y, A x, int H, int W) {
   s.o[2] = hhc * W + wlc; s.ok[2] = t1 && l0;
   s.o[3] = hhc * W + whc; s.ok[3] = t1 && l1;
   return s;
+}
+
+// One sample = (image b, offset group og, tap, output pixel pix), enumerated as idx = ((b * offset_groups + og) * KK + tap)
+// * HWo + pix by every kernel of this file; this is its position, mask value and bilinear geometry.
+template <typename A>
+struct SamplePoint {
+  int b, og, tap, pix;
+  int64_t ob;        // (b * offset_groups + og) * 2 * KK: the (image, group)'s first offset channel
+  A m;               // mask value (1 without a mask)
+  Sample<A> s;
+};
+
+template <typename T>
+__device__ __forceinline__ SamplePoint<typename Acc<T>::type> sample_point(int64_t idx, int HWo, int KK, const T* __restrict__ offset,
+                                                                          const T* __restrict__ mask, const DcnParams& p) {
+  using A = typename Acc<T>::type;
+  SamplePoint<A> q;
+  q.pix = (int)(idx % HWo);
+  q.tap = (int)((idx / HWo) % KK);
+  q.og = (int)((idx / HWo / KK) % p.offset_groups);
+  q.b = (int)(idx / HWo / KK / p.offset_groups);
+  const int oy = q.pix / p.out_w, ox = q.pix - oy * p.out_w;
+  const int i = q.tap / p.kw, j = q.tap - i * p.kw;
+  q.ob = ((int64_t)q.b * p.offset_groups + q.og) * 2 * KK;
+  const A y = (A)(oy * p.stride_h - p.pad_h + i * p.dil_h) + (A)to_acc(offset[(q.ob + 2 * q.tap) * HWo + q.pix]);
+  const A x = (A)(ox * p.stride_w - p.pad_w + j * p.dil_w) + (A)to_acc(offset[(q.ob + 2 * q.tap + 1) * HWo + q.pix]);
+  q.m = p.use_mask ? (A)to_acc(mask[(((int64_t)q.b * p.offset_groups + q.og) * KK + q.tap) * HWo + q.pix]) : (A)1;
+  q.s = make_sample<A>(y, x, p.in_h, p.in_w);
+  return q;
 }
 
 // columns[n][(c * KK + tap)][pix] = mask * bilinear(input[n][c], y, x)
@@ -55,17 +104,10 @@ dcn_sample_columns_kernel(const T* __restrict__ input, const T* __restrict__ off
   const int c_per_off = p.c_in / p.offset_groups;
   const int64_t total = (int64_t)n_imgs * p.offset_groups * KK * HWo;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-    const int pix = (int)(idx % HWo);
-    const int tap = (int)((idx / HWo) % KK);
-    const int og = (int)((idx / HWo / KK) % p.offset_groups);
-    const int b = (int)(idx / HWo / KK / p.offset_groups);
-    const int oy = pix / p.out_w, ox = pix - oy * p.out_w;
-    const int i = tap / p.kw, j = tap - i * p.kw;
-    const int64_t ob = ((int64_t)b * p.offset_groups + og) * 2 * KK;
-    const A y = (A)(oy * p.stride_h - p.pad_h + i * p.dil_h) + (A)to_acc(offset[(ob + 2 * tap) * HWo + pix]);
-    const A x = (A)(ox * p.stride_w - p.pad_w + j * p.dil_w) + (A)to_acc(offset[(ob + 2 * tap + 1) * HWo + pix]);
-    const A m = p.use_mask ? (A)to_acc(mask[(((int64_t)b * p.offset_groups + og) * KK + tap) * HWo + pix]) : (A)1;
-    const Sample<A> s = make_sample<A>(y, x, p.in_h, p.in_w);
+    const SamplePoint<A> q = sample_point<T>(idx, HWo, KK, offset, mask, p);
+    const Sample<A>& s = q.s;
+    const int b = q.b, og = q.og, tap = q.tap, pix = q.pix;
+    const A m = q.m;
     const A hh = (A)1 - s.lh, hw = (A)1 - s.lw;
     const A w1 = hh * hw, w2 = hh * s.lw, w3 = s.lh * hw, w4 = s.lh * s.lw;
     for (int cl = 0; cl < c_per_off; ++cl) {
@@ -82,8 +124,9 @@ dcn_sample_columns_kernel(const T* __restrict__ input, const T* __restrict__ off
   }
 }
 
-// dcol [n][(c * KK + tap)][pix] = (weight^T x grad_out); writes grad_offset / grad_mask, scatters grad_input (pre-zeroed).
-template <typename T>
+// dcol [n][(c * KK + tap)][pix] = (weight^T x grad_out); writes grad_offset / grad_mask and, with SCATTER, scatters
+// grad_input (pre-zeroed).  The deterministic path instantiates it without the scatter and gathers grad_input instead.
+template <typename T, bool SCATTER>
 __global__ void __launch_bounds__(256)
 dcn_backward_inputs_kernel(const T* __restrict__ dcol, const T* __restrict__ input, const T* __restrict__ offset, const T* __restrict__ mask,
                            T* __restrict__ grad_input, T* __restrict__ grad_offset, T* __restrict__ grad_mask, DcnParams p, int n_imgs) {
@@ -92,17 +135,11 @@ dcn_backward_inputs_kernel(const T* __restrict__ dcol, const T* __restrict__ inp
   const int c_per_off = p.c_in / p.offset_groups;
   const int64_t total = (int64_t)n_imgs * p.offset_groups * KK * HWo;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-    const int pix = (int)(idx % HWo);
-    const int tap = (int)((idx / HWo) % KK);
-    const int og = (int)((idx / HWo / KK) % p.offset_groups);
-    const int b = (int)(idx / HWo / KK / p.offset_groups);
-    const int oy = pix / p.out_w, ox = pix - oy * p.out_w;
-    const int i = tap / p.kw, j = tap - i * p.kw;
-    const int64_t ob = ((int64_t)b * p.offset_groups + og) * 2 * KK;
-    const A y = (A)(oy * p.stride_h - p.pad_h + i * p.dil_h) + (A)to_acc(offset[(ob + 2 * tap) * HWo + pix]);
-    const A x = (A)(ox * p.stride_w - p.pad_w + j * p.dil_w) + (A)to_acc(offset[(ob + 2 * tap + 1) * HWo + pix]);
-    const A m = p.use_mask ? (A)to_acc(mask[(((int64_t)b * p.offset_groups + og) * KK + tap) * HWo + pix]) : (A)1;
-    const Sample<A> s = make_sample<A>(y, x, p.in_h, p.in_w);
+    const SamplePoint<A> q = sample_point<T>(idx, HWo, KK, offset, mask, p);
+    const Sample<A>& s = q.s;
+    const int b = q.b, og = q.og, tap = q.tap, pix = q.pix;
+    const int64_t ob = q.ob;
+    const A m = q.m;
     const A hh = (A)1 - s.lh, hw = (A)1 - s.lw;
     const A w1 = hh * hw, w2 = hh * s.lw, w3 = s.lh * hw, w4 = s.lh * s.lw;
     A gy = 0, gx = 0, gm = 0;
@@ -118,12 +155,14 @@ dcn_backward_inputs_kernel(const T* __restrict__ dcol, const T* __restrict__ inp
       gx += m * (s.lh * (v4 - v3) + hh * (v2 - v1)) * d;
       if (s.inside) {
         gm += d * (w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4);
-        const A md = m * d;
-        T* __restrict__ gi = grad_input + plane_off;
-        if (s.ok[0] && w1 != (A)0) atomic_add<T>(gi + s.o[0], md * w1);
-        if (s.ok[1] && w2 != (A)0) atomic_add<T>(gi + s.o[1], md * w2);
-        if (s.ok[2] && w3 != (A)0) atomic_add<T>(gi + s.o[2], md * w3);
-        if (s.ok[3] && w4 != (A)0) atomic_add<T>(gi + s.o[3], md * w4);
+        if constexpr (SCATTER) {
+          const A md = m * d;
+          T* __restrict__ gi = grad_input + plane_off;
+          if (s.ok[0] && w1 != (A)0) atomic_add<T>(gi + s.o[0], md * w1);
+          if (s.ok[1] && w2 != (A)0) atomic_add<T>(gi + s.o[1], md * w2);
+          if (s.ok[2] && w3 != (A)0) atomic_add<T>(gi + s.o[2], md * w3);
+          if (s.ok[3] && w4 != (A)0) atomic_add<T>(gi + s.o[3], md * w4);
+        }
       }
     }
     grad_offset[(ob + 2 * tap) * HWo + pix] = from_acc<T, A>(gy);
@@ -132,23 +171,224 @@ dcn_backward_inputs_kernel(const T* __restrict__ dcol, const T* __restrict__ inp
   }
 }
 
+// ---- deterministic grad_input: bin, sort, cell table, gather -------------------------------------------------------------
+// Corner k of a sample contributes to grad_input when it lies in the image and its bilinear weight is not exactly 0 (the
+// scatter's test).  Bit k of the result; w[k] = that weight.
+template <typename A>
+__device__ __forceinline__ int live_corners(const Sample<A>& s, A w[4]) {
+  const A hh = (A)1 - s.lh, hw = (A)1 - s.lw;
+  w[0] = hh * hw; w[1] = hh * s.lw; w[2] = s.lh * hw; w[3] = s.lh * s.lw;
+  int bits = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) bits |= (s.ok[k] && w[k] != (A)0) ? (1 << k) : 0;
+  return s.inside ? bits : 0;
+}
+
+// key = (b * offset_groups + og) * (H+1)(W+1) + (hl+1) * (W+1) + (wl+1); `sentinel` (= segments x cells) for a sample that
+// contributes nothing.  vals = the sample index (the sort's payload).
+template <typename T>
+__global__ void __launch_bounds__(256)
+dcn_bin_samples_kernel(const T* __restrict__ offset, const T* __restrict__ mask, uint32_t* __restrict__ keys, int* __restrict__ vals,
+                       DcnParams p, int n_samples, uint32_t sentinel) {
+  using A = typename Acc<T>::type;
+  const int cw = p.in_w + 1, cells = (p.in_h + 1) * cw, HWo = p.out_h * p.out_w, KK = p.kh * p.kw;
+  for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < n_samples; idx += gridDim.x * blockDim.x) {
+    const SamplePoint<A> q = sample_point<T>(idx, HWo, KK, offset, mask, p);
+    A w[4];
+    const int bits = live_corners(q.s, w);
+    keys[idx] = bits ? (uint32_t)(((int64_t)q.b * p.offset_groups + q.og) * cells + (q.s.hl + 1) * cw + (q.s.wl + 1)) : sentinel;
+    vals[idx] = idx;
+  }
+}
+
+// start[v] = first sorted position whose key is >= v, for v in [0, sentinel]: the samples of cell v are [start[v], start[v+1]).
+__global__ void __launch_bounds__(256)
+dcn_cell_start_kernel(const uint32_t* __restrict__ keys_sorted, int n_samples, int* __restrict__ start, uint32_t sentinel) {
+  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v <= (int64_t)sentinel; v += (int64_t)gridDim.x * blockDim.x) {
+    int lo = 0, hi = n_samples;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (keys_sorted[mid] < (uint32_t)v) lo = mid + 1; else hi = mid;
+    }
+    start[v] = lo;
+  }
+}
+
+// One record per sorted sample: col = tap * HWo + pix (its dcol column inside the channel's KK x HWo block), the live-corner
+// bits, and mw[k] = mask * corner weight k (0 for a dead corner; the bits, not the zero, decide whether it is added).
+template <typename A>
+struct alignas(4 * sizeof(A)) CornerW { A v[4]; };
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+dcn_cell_records_kernel(const uint32_t* __restrict__ keys_sorted, const int* __restrict__ vals_sorted, const T* __restrict__ offset,
+                        const T* __restrict__ mask, int2* __restrict__ rec_col, CornerW<typename Acc<T>::type>* __restrict__ rec_w,
+                        DcnParams p, int n_samples, uint32_t sentinel) {
+  using A = typename Acc<T>::type;
+  const int HWo = p.out_h * p.out_w;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_samples; i += gridDim.x * blockDim.x) {
+    if (keys_sorted[i] == sentinel) continue;        // never read: the cell table ends before the first sentinel
+    const SamplePoint<A> q = sample_point<T>(vals_sorted[i], HWo, p.kh * p.kw, offset, mask, p);
+    A w[4];
+    const int bits = live_corners(q.s, w);
+    CornerW<A> r;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) r.v[k] = (bits >> k & 1) ? q.m * w[k] : (A)0;
+    rec_col[i] = make_int2(q.tap * HWo + q.pix, bits);
+    rec_w[i] = r;
+  }
+}
+
+// grad_input[b, c, y, x] = sum over the cells (y, x), (y, x-1), (y-1, x), (y-1, x-1) - the pixel is their corner 0, 1, 2, 3 -
+// and over each cell's records in sorted order, of mw[k] * dcol[b, c * KK + tap, pix].  A CTA owns (image, offset group,
+// CPB channels of the group, 256 pixels); a thread owns one pixel (lanes along x) and the CPB channels in registers, so
+// each record is read once for CPB channels.  Every pixel is written, with 0 where nothing lands.
+template <typename T, int CPB>
+__global__ void __launch_bounds__(256)
+dcn_grad_input_gather_kernel(const T* __restrict__ dcol, const int* __restrict__ cell_start, const int2* __restrict__ rec_col,
+                             const CornerW<typename Acc<T>::type>* __restrict__ rec_w, T* __restrict__ grad_input, DcnParams p,
+                             int n_tiles, int n_cchunks) {
+  using A = typename Acc<T>::type;
+  const int HWo = p.out_h * p.out_w, HWi = p.in_h * p.in_w, KK = p.kh * p.kw;
+  const int c_per_off = p.c_in / p.offset_groups;
+  const int cw = p.in_w + 1, cells = (p.in_h + 1) * cw;
+  const int tile = (int)(blockIdx.x % n_tiles);
+  const int cc = (int)((blockIdx.x / n_tiles) % n_cchunks);
+  const int seg = (int)(blockIdx.x / n_tiles / n_cchunks);           // b * offset_groups + og
+  const int b = seg / p.offset_groups, og = seg - b * p.offset_groups;
+  const int pix = tile * 256 + threadIdx.x;
+  if (pix >= HWi) return;
+  const int y = pix / p.in_w, x = pix - y * p.in_w;
+  const int c0 = og * c_per_off + cc * CPB, nc = min(CPB, c_per_off - cc * CPB);
+  const T* __restrict__ dc = dcol + ((int64_t)b * p.c_in + c0) * KK * HWo;
+  const int64_t cstride = (int64_t)KK * HWo;
+  const int* __restrict__ cs = cell_start + (int64_t)seg * cells;
+  const int cell0 = (y + 1) * cw + (x + 1);
+  A acc[CPB];
+#pragma unroll
+  for (int j = 0; j < CPB; ++j) acc[j] = (A)0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int cell = cell0 - (k >> 1) * cw - (k & 1);
+    const int beg = cs[cell], end = cs[cell + 1];
+    for (int r = beg; r < end; ++r) {
+      const int2 hdr = rec_col[r];
+      if (!(hdr.y >> k & 1)) continue;
+      const A mw = rec_w[r].v[k];
+#pragma unroll
+      for (int j = 0; j < CPB; ++j)
+        if (j < nc) acc[j] += mw * (A)to_acc(dc[j * cstride + hdr.x]);
+    }
+  }
+  T* __restrict__ gi = grad_input + ((int64_t)b * p.c_in + c0) * HWi + pix;
+#pragma unroll
+  for (int j = 0; j < CPB; ++j)
+    if (j < nc) gi[(int64_t)j * HWi] = from_acc<T, A>(acc[j]);
+}
+
+// channels per gather thread: the accumulators stay in registers
+template <typename T> struct GatherCpb { static constexpr int value = 16; };
+template <> struct GatherCpb<double> { static constexpr int value = 8; };
+
+// Images per pass of the deterministic path: sample indices and sorted positions are int, keys are 32-bit.  0 when one image
+// alone exceeds that (the caller then reports the shape as unsupported).
+int det_pass_imgs(const DcnParams& p, int n_imgs) {
+  const int64_t spi = (int64_t)p.offset_groups * p.kh * p.kw * p.out_h * p.out_w;
+  const int64_t kpi = (int64_t)p.offset_groups * (p.in_h + 1) * (p.in_w + 1);
+  const int64_t by_samples = ((int64_t)INT32_MAX - 1) / spi, by_keys = ((int64_t)UINT32_MAX - 1) / kpi;
+  return (int)std::min<int64_t>({(int64_t)n_imgs, by_samples, by_keys});
+}
+
+struct DetWs {
+  uint32_t *keys_in, *keys_out; int *vals_in, *vals_out, *cell_start; int2* rec_col; void* rec_w;
+  void* cub_temp; size_t cub_bytes; size_t total;
+};
+
+DetWs carve_det(void* base, const DcnParams& p, int pass_imgs, size_t acc_bytes) {
+  const int n = (int)((int64_t)pass_imgs * p.offset_groups * p.kh * p.kw * p.out_h * p.out_w);
+  const size_t nk = (size_t)pass_imgs * p.offset_groups * (p.in_h + 1) * (p.in_w + 1) + 1;
+  Carver c(base);
+  DetWs w;
+  w.keys_in = c.take<uint32_t>(n);
+  w.keys_out = c.take<uint32_t>(n);
+  w.vals_in = c.take<int>(n);
+  w.vals_out = c.take<int>(n);
+  w.cell_start = c.take<int>(nk);
+  w.rec_col = c.take<int2>(n);
+  w.rec_w = c.take<char>((size_t)n * 4 * acc_bytes);
+  w.cub_bytes = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, w.cub_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int*)nullptr, (int*)nullptr,
+                                  n, 0, 32);
+  w.cub_temp = c.take<char>(w.cub_bytes);
+  w.total = c.off;
+  return w;
+}
+
+int grid_for(int64_t total) {
+  return (int)(ceil_div64(total, 256) < (int64_t)sm_count() * 32 ? ceil_div64(total, 256) : (int64_t)sm_count() * 32);
+}
+
 template <typename T>
 int launch_columns(const void* input, const void* offset, const void* mask, void* columns, const DcnParams& p, int n_imgs, cudaStream_t st) {
   const int64_t total = (int64_t)n_imgs * p.offset_groups * p.kh * p.kw * p.out_h * p.out_w;
   if (total == 0) return 0;
-  const int grid = (int)(ceil_div64(total, 256) < (int64_t)sm_count() * 32 ? ceil_div64(total, 256) : (int64_t)sm_count() * 32);
+  const int grid = grid_for(total);
   dcn_sample_columns_kernel<T><<<grid, 256, 0, st>>>((const T*)input, (const T*)offset, (const T*)mask, (T*)columns, p, n_imgs);
   return check_launch("dcn_sample_columns_kernel");
 }
-template <typename T>
+template <typename T, bool SCATTER = true>
 int launch_bwd_inputs(const void* dcol, const void* input, const void* offset, const void* mask, void* gi, void* go, void* gm,
                       const DcnParams& p, int n_imgs, cudaStream_t st) {
   const int64_t total = (int64_t)n_imgs * p.offset_groups * p.kh * p.kw * p.out_h * p.out_w;
   if (total == 0) return 0;
-  const int grid = (int)(ceil_div64(total, 256) < (int64_t)sm_count() * 32 ? ceil_div64(total, 256) : (int64_t)sm_count() * 32);
-  dcn_backward_inputs_kernel<T><<<grid, 256, 0, st>>>((const T*)dcol, (const T*)input, (const T*)offset, (const T*)mask, (T*)gi, (T*)go,
-                                                     (T*)gm, p, n_imgs);
+  const int grid = grid_for(total);
+  dcn_backward_inputs_kernel<T, SCATTER><<<grid, 256, 0, st>>>((const T*)dcol, (const T*)input, (const T*)offset, (const T*)mask, (T*)gi,
+                                                              (T*)go, (T*)gm, p, n_imgs);
   return check_launch("dcn_backward_inputs_kernel");
+}
+
+// grad_offset / grad_mask by the scatter-free instantiation, then grad_input pass by pass (bin, sort, cell table, gather).
+template <typename T>
+int launch_bwd_inputs_det(const void* dcol, const void* input, const void* offset, const void* mask, void* gi, void* go, void* gm,
+                          const DcnParams& p, int n_imgs, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  using A = typename Acc<T>::type;
+  constexpr int CPB = GatherCpb<T>::value;
+  const int pass = det_pass_imgs(p, n_imgs);
+  const DetWs w = carve_det(workspace, p, pass, sizeof(A));
+  if (workspace_bytes < w.total) {
+    set_error("deform_conv2d_backward_inputs: workspace too small (%zu < %zu)", workspace_bytes, w.total);
+    return VB200_EWORKSPACE;
+  }
+  int rc = launch_bwd_inputs<T, false>(dcol, input, offset, mask, nullptr, go, gm, p, n_imgs, st);
+  if (rc) return rc;
+  const int KK = p.kh * p.kw, HWo = p.out_h * p.out_w, HWi = p.in_h * p.in_w;
+  const int64_t cells = (int64_t)(p.in_h + 1) * (p.in_w + 1);
+  const int n_tiles = ceil_div(HWi, 256), n_cchunks = ceil_div(p.c_in / p.offset_groups, CPB);
+  for (int b0 = 0; b0 < n_imgs; b0 += pass) {
+    const int nb = std::min(pass, n_imgs - b0);
+    const int n = (int)((int64_t)nb * p.offset_groups * KK * HWo);
+    const uint32_t sentinel = (uint32_t)((int64_t)nb * p.offset_groups * cells);
+    const T* off_b = (const T*)offset + (int64_t)b0 * p.offset_groups * 2 * KK * HWo;
+    const T* mask_b = p.use_mask ? (const T*)mask + (int64_t)b0 * p.offset_groups * KK * HWo : nullptr;
+    const T* dcol_b = (const T*)dcol + (int64_t)b0 * p.c_in * KK * HWo;
+    T* gi_b = (T*)gi + (int64_t)b0 * p.c_in * HWi;
+    dcn_bin_samples_kernel<T><<<grid_for(n), 256, 0, st>>>(off_b, mask_b, w.keys_in, w.vals_in, p, n, sentinel);
+    if ((rc = check_launch("dcn_bin_samples_kernel"))) return rc;
+    const int end_bit = 32 - __builtin_clz(sentinel | 1u);          // only the bits the key range needs
+    size_t tb = w.cub_bytes;
+    VB200_CUDA_TRY(cub::DeviceRadixSort::SortPairs(w.cub_temp, tb, w.keys_in, w.keys_out, w.vals_in, w.vals_out, n, 0, end_bit, st));
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
+    dcn_cell_start_kernel<<<grid_for((int64_t)sentinel + 1), 256, 0, st>>>(w.keys_out, n, w.cell_start, sentinel);
+    if ((rc = check_launch("dcn_cell_start_kernel"))) return rc;
+    dcn_cell_records_kernel<T><<<grid_for(n), 256, 0, st>>>(w.keys_out, w.vals_out, off_b, mask_b, w.rec_col, (CornerW<A>*)w.rec_w, p, n,
+                                                           sentinel);
+    if ((rc = check_launch("dcn_cell_records_kernel"))) return rc;
+    const int64_t blocks = (int64_t)nb * p.offset_groups * n_cchunks * n_tiles;
+    dcn_grad_input_gather_kernel<T, CPB><<<(unsigned)blocks, 256, 0, st>>>(dcol_b, w.cell_start, w.rec_col, (const CornerW<A>*)w.rec_w, gi_b,
+                                                                          p, n_tiles, n_cchunks);
+    if ((rc = check_launch("dcn_grad_input_gather_kernel"))) return rc;
+  }
+  return 0;
 }
 
 int fill_params(DcnParams& p, int c_in, int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w, int dil_h,
@@ -187,10 +427,24 @@ extern "C" int vb200_deform_conv2d_sample_columns(const void* input, const void*
   return VB200_EUNSUPPORTED;
 }
 
-extern "C" int vb200_deform_conv2d_backward_inputs(const void* dcol, const void* input, const void* offset, const void* mask,
-                                                   void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs, int c_in,
-                                                   int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w,
-                                                   int dil_h, int dil_w, int offset_groups, int use_mask, vb200_stream stream) {
+extern "C" size_t vb200_deform_conv2d_backward_inputs_workspace_bytes(int dtype, int n_imgs, int c_in, int in_h, int in_w, int kh, int kw,
+                                                                     int stride_h, int stride_w, int pad_h, int pad_w, int dil_h,
+                                                                     int dil_w, int offset_groups) {
+  DcnParams p;
+  if (n_imgs <= 0 || c_in <= 0 || in_h <= 0 || in_w <= 0 || kh <= 0 || kw <= 0 || stride_h <= 0 || stride_w <= 0 || dil_h <= 0 ||
+      dil_w <= 0 || pad_h < 0 || pad_w < 0)
+    return 0;
+  if (fill_params(p, c_in, in_h, in_w, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, offset_groups, 0) != 0) return 0;
+  const int pass = det_pass_imgs(p, n_imgs);
+  if (pass == 0) return 0;
+  return carve_det(nullptr, p, pass, dtype == VB200_F64 ? sizeof(double) : sizeof(float)).total;
+}
+
+extern "C" int vb200_deform_conv2d_backward_inputs_ex(const void* dcol, const void* input, const void* offset, const void* mask,
+                                                      void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs,
+                                                      int c_in, int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h,
+                                                      int pad_w, int dil_h, int dil_w, int offset_groups, int use_mask, int deterministic,
+                                                      void* workspace, size_t workspace_bytes, vb200_stream stream) {
   DcnParams p;
   VB200_REQUIRE(kh > 0 && kw > 0 && stride_h > 0 && stride_w > 0 && dil_h > 0 && dil_w > 0 && pad_h >= 0 && pad_w >= 0,
                 "deform_conv2d_backward_inputs: bad geometry");
@@ -200,12 +454,35 @@ extern "C" int vb200_deform_conv2d_backward_inputs(const void* dcol, const void*
   VB200_REQUIRE(dcol && input && offset && grad_input && grad_offset && (!use_mask || (mask && grad_mask)), "deform_conv2d_backward_inputs: null pointer");
   VB200_REQUIRE((int64_t)in_h * in_w < (1ll << 31), "deform_conv2d_backward_inputs: image too large");
   cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case VB200_F32: return launch_bwd_inputs<float>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
-    case VB200_F64: return launch_bwd_inputs<double>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
-    case VB200_F16: return launch_bwd_inputs<__half>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
-    case VB200_BF16: return launch_bwd_inputs<__nv_bfloat16>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
+  if (deterministic) {
+    if (det_pass_imgs(p, n_imgs) == 0) {
+      set_error("deform_conv2d_backward_inputs: one image has too many samples or cells for the deterministic grad_input");
+      return VB200_EUNSUPPORTED;
+    }
+    VB200_REQUIRE(workspace, "deform_conv2d_backward_inputs: null workspace");
+    switch (dtype) {
+      case VB200_F32: return launch_bwd_inputs_det<float>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, workspace, workspace_bytes, st);
+      case VB200_F64: return launch_bwd_inputs_det<double>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, workspace, workspace_bytes, st);
+      case VB200_F16: return launch_bwd_inputs_det<__half>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, workspace, workspace_bytes, st);
+      case VB200_BF16: return launch_bwd_inputs_det<__nv_bfloat16>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, workspace, workspace_bytes, st);
+    }
+  } else {
+    switch (dtype) {
+      case VB200_F32: return launch_bwd_inputs<float>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
+      case VB200_F64: return launch_bwd_inputs<double>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
+      case VB200_F16: return launch_bwd_inputs<__half>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
+      case VB200_BF16: return launch_bwd_inputs<__nv_bfloat16>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
+    }
   }
   set_error("deform_conv2d_backward_inputs: unsupported dtype %d", dtype);
   return VB200_EUNSUPPORTED;
+}
+
+extern "C" int vb200_deform_conv2d_backward_inputs(const void* dcol, const void* input, const void* offset, const void* mask,
+                                                   void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs, int c_in,
+                                                   int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w,
+                                                   int dil_h, int dil_w, int offset_groups, int use_mask, vb200_stream stream) {
+  return vb200_deform_conv2d_backward_inputs_ex(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, dtype, n_imgs, c_in, in_h,
+                                                in_w, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, offset_groups, use_mask, 0,
+                                                nullptr, 0, stream);
 }

@@ -608,6 +608,8 @@ void deform_conv2d_gather(const at::Tensor& input, const at::Tensor& weight, con
 // ---- deform_conv2d backward (schema csrc/ops/deform_conv2d.cpp:103-104; reference deform_conv2d_kernel.cu:647-1033) -------
 // Two plain GEMMs (cuBLAS through at::matmul: weight^T x grad_out -> dcol; grad_out x columns^T -> grad_weight) around two
 // kernels of ours: the fused grad_input / grad_offset / grad_mask pass and the column sampler (deform_conv2d_bwd.cu).
+// Under torch.use_deterministic_algorithms (warn_only included) grad_input is gathered instead of scattered (bit-reproducible,
+// written in full) and dcol is one GEMM per image, so every gradient of image b depends on image b's data alone.
 std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> deform_conv2d_backward(
     const at::Tensor& grad, const at::Tensor& input, const at::Tensor& weight, const at::Tensor& offset, const at::Tensor& mask,
     const at::Tensor& bias, int64_t stride_h, int64_t stride_w, int64_t pad_h, int64_t pad_w, int64_t dilation_h, int64_t dilation_w,
@@ -625,14 +627,25 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> deform_co
               "deform_conv2d_backward: all tensors must share one dtype");
   const int dt = dtype_code(st, "deform_conv2d_backward");
   TORCH_CHECK(dt == VB200_F32 || dt == VB200_F64 || dt == VB200_F16 || dt == VB200_BF16, "deform_conv2d_backward: unsupported dtype ", st);
-  at::Tensor grad_input = at::zeros_like(input_c), grad_offset = at::empty_like(offset_c), grad_weight = at::zeros_like(weight_c);
+  const bool det = at::globalContext().deterministicAlgorithms();
+  size_t ws_img = 0;                 // deterministic workspace of one image; 0 = the gather does not run
+  if (det && B > 0 && C_in > 0 && grad_c.numel() > 0) {
+    ws_img = vb200_deform_conv2d_backward_inputs_workspace_bytes(dt, 1, (int)C_in, (int)H, (int)W, (int)kh, (int)kw, (int)stride_h,
+                                                                 (int)stride_w, (int)pad_h, (int)pad_w, (int)dilation_h, (int)dilation_w,
+                                                                 (int)n_offset_grps);
+    // only an image whose samples or cells overflow the gather's 32-bit indices: raise (or warn) as the reference does
+    if (ws_img == 0) at::globalContext().alertNotDeterministic("deform_conv2d_backward: grad_input of an image this large");
+  }
+  const bool gather = ws_img > 0;
+  at::Tensor grad_input = gather ? at::empty_like(input_c) : at::zeros_like(input_c);
+  at::Tensor grad_offset = at::empty_like(offset_c), grad_weight = at::zeros_like(weight_c);
   at::Tensor grad_mask = use_mask ? at::empty_like(mask_c) : at::zeros_like(mask_c);
   at::Tensor grad_bias = at::ones_like(bias) * (grad_c.numel() ? grad_c.sum({0, 2, 3}) : at::zeros_like(bias));   // deform_conv2d_kernel.cu:1231
   if (B == 0 || grad_c.numel() == 0) return std::make_tuple(grad_input, grad_weight, grad_offset, grad_mask, grad_bias);
   const int64_t out_h = grad_c.size(2), out_w = grad_c.size(3), HWo = out_h * out_w, cout_g = C_out / n_weight_grps;
   TORCH_CHECK(grad_c.size(0) == B && grad_c.size(1) == C_out && offset_c.size(2) == out_h && offset_c.size(3) == out_w,
               "deform_conv2d_backward: grad / offset shapes do not match the forward geometry");
-  const int64_t per_img = C_in * KK * HWo * (int64_t)input_c.element_size();
+  const int64_t per_img = C_in * KK * HWo * (int64_t)input_c.element_size() + (int64_t)ws_img;
   const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(B, (int64_t)(1ll << 30) / std::max<int64_t>(per_img, 1)));
   const bool low = st == at::kHalf || st == at::kBFloat16;
   at::Tensor gw_acc = low ? at::zeros({C_out, cin_g * KK}, input_c.options().dtype(at::kFloat)) : grad_weight.view({C_out, cin_g * KK});
@@ -644,6 +657,17 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> deform_co
     // dcol = weight^T x grad_out, per weight group
     for (int64_t grp = 0; grp < n_weight_grps; ++grp) {
       at::Tensor wt = w2.narrow(0, grp * cout_g, cout_g).t();                                  // [cin_g*KK, cout_g]
+      if (gather) {
+        // one GEMM per image: a batched GEMM may choose its kernel by the batch size, and so could change image b's bits
+        // with the images around it.  Operands off a 16-byte boundary are staged, so the same kernel runs wherever the image sits.
+        for (int64_t i = 0; i < nb; ++i) {
+          at::Tensor g_img = g[i].narrow(0, grp * cout_g, cout_g);
+          if ((uintptr_t)g_img.data_ptr() % 16) g_img = g_img.clone();
+          at::Tensor dst = buf[i].narrow(0, grp * cin_g * KK, cin_g * KK);
+          if ((uintptr_t)dst.data_ptr() % 16) dst.copy_(at::mm(wt, g_img)); else at::mm_out(dst, wt, g_img);
+        }
+        continue;
+      }
       at::Tensor d = at::matmul(wt, g.narrow(1, grp * cout_g, cout_g));                        // [nb, cin_g*KK, HWo]
       if (n_weight_grps == 1) buf = d; else buf.narrow(1, grp * cin_g * KK, cin_g * KK).copy_(d);
     }
@@ -651,10 +675,15 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> deform_co
     at::Tensor gi_b = grad_input.narrow(0, b0, nb), go_b = grad_offset.narrow(0, b0, nb);
     const void* mk = use_mask ? mask_c.narrow(0, b0, nb).data_ptr() : nullptr;
     void* gm = use_mask ? grad_mask.narrow(0, b0, nb).data_ptr() : nullptr;
-    check_rc(vb200_deform_conv2d_backward_inputs(buf.data_ptr(), in_b.data_ptr(), off_b.data_ptr(), mk, gi_b.data_ptr(), go_b.data_ptr(), gm,
-                                                 dt, (int)nb, (int)C_in, (int)H, (int)W, (int)kh, (int)kw, (int)stride_h, (int)stride_w,
-                                                 (int)pad_h, (int)pad_w, (int)dilation_h, (int)dilation_w, (int)n_offset_grps,
-                                                 use_mask ? 1 : 0, cur_stream()),
+    const size_t wsb = gather ? vb200_deform_conv2d_backward_inputs_workspace_bytes(dt, (int)nb, (int)C_in, (int)H, (int)W, (int)kh, (int)kw,
+                                                                                    (int)stride_h, (int)stride_w, (int)pad_h, (int)pad_w,
+                                                                                    (int)dilation_h, (int)dilation_w, (int)n_offset_grps)
+                              : 0;
+    at::Tensor ws = gather ? workspace(wsb, input_c) : at::Tensor();
+    check_rc(vb200_deform_conv2d_backward_inputs_ex(buf.data_ptr(), in_b.data_ptr(), off_b.data_ptr(), mk, gi_b.data_ptr(), go_b.data_ptr(), gm,
+                                                    dt, (int)nb, (int)C_in, (int)H, (int)W, (int)kh, (int)kw, (int)stride_h, (int)stride_w,
+                                                    (int)pad_h, (int)pad_w, (int)dilation_h, (int)dilation_w, (int)n_offset_grps,
+                                                    use_mask ? 1 : 0, gather ? 1 : 0, gather ? ws.data_ptr() : nullptr, wsb, cur_stream()),
              "deform_conv2d_backward");
     // columns for grad_weight (the buffer is reused)
     check_rc(vb200_deform_conv2d_sample_columns(in_b.data_ptr(), off_b.data_ptr(), mk, buf.data_ptr(), dt, (int)nb, (int)C_in, (int)H, (int)W,
