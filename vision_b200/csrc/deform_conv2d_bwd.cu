@@ -34,36 +34,10 @@
 #include <algorithm>
 
 #include "common.cuh"
-#include "dcn_params.h"
+#include "dcn_geometry.cuh"
 
 namespace vb200 {
 namespace {
-
-template <typename A>
-struct Sample {
-  int o[4];          // y*W + x of the four corners (clamped into the image)
-  bool ok[4];        // corner inside the image
-  A lh, lw;          // fractional parts
-  bool inside;       // bilinear_interpolate's outer test: -1 < y < H and -1 < x < W
-  int hl, wl;        // the sample's cell: floor(y), floor(x)
-};
-
-template <typename A>
-__device__ __forceinline__ Sample<A> make_sample(A y, A x, int H, int W) {
-  Sample<A> s;
-  const int hl = (int)floor(y), wl = (int)floor(x);
-  const int hh = hl + 1, wh = wl + 1;
-  s.hl = hl; s.wl = wl;
-  s.lh = y - (A)hl; s.lw = x - (A)wl;
-  s.inside = !(y <= (A)-1 || (A)H <= y || x <= (A)-1 || (A)W <= x);
-  const bool t0 = hl >= 0 && hl < H, t1 = hh >= 0 && hh < H, l0 = wl >= 0 && wl < W, l1 = wh >= 0 && wh < W;
-  const int hlc = min(max(hl, 0), H - 1), hhc = min(max(hh, 0), H - 1), wlc = min(max(wl, 0), W - 1), whc = min(max(wh, 0), W - 1);
-  s.o[0] = hlc * W + wlc; s.ok[0] = t0 && l0;
-  s.o[1] = hlc * W + whc; s.ok[1] = t0 && l1;
-  s.o[2] = hhc * W + wlc; s.ok[2] = t1 && l0;
-  s.o[3] = hhc * W + whc; s.ok[3] = t1 && l1;
-  return s;
-}
 
 // One sample = (image b, offset group og, tap, output pixel pix), enumerated as idx = ((b * offset_groups + og) * KK + tap)
 // * HWo + pix by every kernel of this file; this is its position, mask value and bilinear geometry.
@@ -84,12 +58,9 @@ __device__ __forceinline__ SamplePoint<typename Acc<T>::type> sample_point(int64
   q.tap = (int)((idx / HWo) % KK);
   q.og = (int)((idx / HWo / KK) % p.offset_groups);
   q.b = (int)(idx / HWo / KK / p.offset_groups);
-  const int oy = q.pix / p.out_w, ox = q.pix - oy * p.out_w;
-  const int i = q.tap / p.kw, j = q.tap - i * p.kw;
   q.ob = ((int64_t)q.b * p.offset_groups + q.og) * 2 * KK;
-  const A y = (A)(oy * p.stride_h - p.pad_h + i * p.dil_h) + (A)to_acc(offset[(q.ob + 2 * q.tap) * HWo + q.pix]);
-  const A x = (A)(ox * p.stride_w - p.pad_w + j * p.dil_w) + (A)to_acc(offset[(q.ob + 2 * q.tap + 1) * HWo + q.pix]);
-  q.m = p.use_mask ? (A)to_acc(mask[(((int64_t)q.b * p.offset_groups + q.og) * KK + q.tap) * HWo + q.pix]) : (A)1;
+  A y, x;
+  sample_position<A>(offset + q.ob * HWo, mask + q.ob / 2 * HWo, p, q.tap, q.pix, y, x, q.m);
   q.s = make_sample<A>(y, x, p.in_h, p.in_w);
   return q;
 }
@@ -108,16 +79,16 @@ dcn_sample_columns_kernel(const T* __restrict__ input, const T* __restrict__ off
     const Sample<A>& s = q.s;
     const int b = q.b, og = q.og, tap = q.tap, pix = q.pix;
     const A m = q.m;
-    const A hh = (A)1 - s.lh, hw = (A)1 - s.lw;
-    const A w1 = hh * hw, w2 = hh * s.lw, w3 = s.lh * hw, w4 = s.lh * s.lw;
+    A w[4];
+    corner_weights(s, w);
     for (int cl = 0; cl < c_per_off; ++cl) {
       const int c = og * c_per_off + cl;
       const T* __restrict__ plane = input + ((int64_t)b * p.c_in + c) * HWi;
       A val = 0;
       if (s.inside) {
-        const A v1 = s.ok[0] ? (A)to_acc(plane[s.o[0]]) : (A)0, v2 = s.ok[1] ? (A)to_acc(plane[s.o[1]]) : (A)0;
-        const A v3 = s.ok[2] ? (A)to_acc(plane[s.o[2]]) : (A)0, v4 = s.ok[3] ? (A)to_acc(plane[s.o[3]]) : (A)0;
-        val = w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4;
+        A v[4];
+        corner_values(plane, s, v);
+        val = blend(w, v);
       }
       columns[((int64_t)b * p.c_in * KK + (int64_t)c * KK + tap) * HWo + pix] = from_acc<T, A>(m * val);
     }
@@ -141,27 +112,30 @@ dcn_backward_inputs_kernel(const T* __restrict__ dcol, const T* __restrict__ inp
     const int64_t ob = q.ob;
     const A m = q.m;
     const A hh = (A)1 - s.lh, hw = (A)1 - s.lw;
-    const A w1 = hh * hw, w2 = hh * s.lw, w3 = s.lh * hw, w4 = s.lh * s.lw;
+    A w[4];
+    corner_weights(s, w);
     A gy = 0, gx = 0, gm = 0;
     for (int cl = 0; cl < c_per_off; ++cl) {
       const int c = og * c_per_off + cl;
       const int64_t plane_off = ((int64_t)b * p.c_in + c) * HWi;
       const T* __restrict__ plane = input + plane_off;
       const A d = (A)to_acc(dcol[((int64_t)b * p.c_in * KK + (int64_t)c * KK + tap) * HWo + pix]);
-      const A v1 = s.ok[0] ? (A)to_acc(plane[s.o[0]]) : (A)0, v2 = s.ok[1] ? (A)to_acc(plane[s.o[1]]) : (A)0;
-      const A v3 = s.ok[2] ? (A)to_acc(plane[s.o[2]]) : (A)0, v4 = s.ok[3] ? (A)to_acc(plane[s.o[3]]) : (A)0;
-      // get_coordinate_weight (:503-536): d val / dy and d val / dx of the bilinear sample
-      gy += m * (s.lw * (v4 - v2) + hw * (v3 - v1)) * d;
-      gx += m * (s.lh * (v4 - v3) + hh * (v2 - v1)) * d;
+      A v[4];
+      corner_values(plane, s, v);
+      // get_coordinate_weight (:503-536): d val / dy and d val / dx of the bilinear sample.  The fma is spelled out: left
+      // to the compiler, which product it fuses changes with the surrounding code, and with it the last bit.
+      gy += m * fma(hw, v[2] - v[0], s.lw * (v[3] - v[1])) * d;
+      gx += m * fma(hh, v[1] - v[0], s.lh * (v[3] - v[2])) * d;
       if (s.inside) {
-        gm += d * (w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4);
+        gm += d * blend(w, v);
         if constexpr (SCATTER) {
           const A md = m * d;
           T* __restrict__ gi = grad_input + plane_off;
-          if (s.ok[0] && w1 != (A)0) atomic_add<T>(gi + s.o[0], md * w1);
-          if (s.ok[1] && w2 != (A)0) atomic_add<T>(gi + s.o[1], md * w2);
-          if (s.ok[2] && w3 != (A)0) atomic_add<T>(gi + s.o[2], md * w3);
-          if (s.ok[3] && w4 != (A)0) atomic_add<T>(gi + s.o[3], md * w4);
+          // written out: as a loop over k, the channel loop is no longer unrolled (4 atomics in flight instead of 12)
+          if (s.ok[0] && w[0] != (A)0) atomic_add<T>(gi + s.o[0], md * w[0]);
+          if (s.ok[1] && w[1] != (A)0) atomic_add<T>(gi + s.o[1], md * w[1]);
+          if (s.ok[2] && w[2] != (A)0) atomic_add<T>(gi + s.o[2], md * w[2]);
+          if (s.ok[3] && w[3] != (A)0) atomic_add<T>(gi + s.o[3], md * w[3]);
         }
       }
     }
@@ -176,8 +150,7 @@ dcn_backward_inputs_kernel(const T* __restrict__ dcol, const T* __restrict__ inp
 // scatter's test).  Bit k of the result; w[k] = that weight.
 template <typename A>
 __device__ __forceinline__ int live_corners(const Sample<A>& s, A w[4]) {
-  const A hh = (A)1 - s.lh, hw = (A)1 - s.lw;
-  w[0] = hh * hw; w[1] = hh * s.lw; w[2] = s.lh * hw; w[3] = s.lh * s.lw;
+  corner_weights(s, w);
   int bits = 0;
 #pragma unroll
   for (int k = 0; k < 4; ++k) bits |= (s.ok[k] && w[k] != (A)0) ? (1 << k) : 0;
@@ -391,14 +364,6 @@ int launch_bwd_inputs_det(const void* dcol, const void* input, const void* offse
   return 0;
 }
 
-int fill_params(DcnParams& p, int c_in, int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w, int dil_h,
-                int dil_w, int offset_groups, int use_mask) {
-  p = DcnParams{0, c_in, in_h, in_w, 0, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, 1, offset_groups, use_mask, 0, 0};
-  p.out_h = (in_h + 2 * pad_h - (dil_h * (kh - 1) + 1)) / stride_h + 1;
-  p.out_w = (in_w + 2 * pad_w - (dil_w * (kw - 1) + 1)) / stride_w + 1;
-  return (p.out_h > 0 && p.out_w > 0 && offset_groups > 0 && c_in % offset_groups == 0) ? 0 : -1;
-}
-
 }  // namespace
 }  // namespace vb200
 
@@ -409,32 +374,24 @@ extern "C" int vb200_deform_conv2d_sample_columns(const void* input, const void*
                                                   int pad_h, int pad_w, int dil_h, int dil_w, int offset_groups, int use_mask,
                                                   vb200_stream stream) {
   DcnParams p;
-  VB200_REQUIRE(kh > 0 && kw > 0 && stride_h > 0 && stride_w > 0 && dil_h > 0 && dil_w > 0 && pad_h >= 0 && pad_w >= 0,
-                "deform_conv2d_sample_columns: bad geometry");
-  VB200_REQUIRE(fill_params(p, c_in, in_h, in_w, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, offset_groups, use_mask) == 0,
-                "deform_conv2d_sample_columns: bad sizes");
+  if (const int rc = dcn_params(p, n_imgs, c_in, in_h, in_w, 0, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, 1, offset_groups,
+                                use_mask))
+    return rc;
   if (n_imgs == 0 || c_in == 0) return 0;
   VB200_REQUIRE(input && offset && columns && (!use_mask || mask), "deform_conv2d_sample_columns: null pointer");
   VB200_REQUIRE((int64_t)in_h * in_w < (1ll << 31), "deform_conv2d_sample_columns: image too large");
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case VB200_F32: return launch_columns<float>(input, offset, mask, columns, p, n_imgs, st);
-    case VB200_F64: return launch_columns<double>(input, offset, mask, columns, p, n_imgs, st);
-    case VB200_F16: return launch_columns<__half>(input, offset, mask, columns, p, n_imgs, st);
-    case VB200_BF16: return launch_columns<__nv_bfloat16>(input, offset, mask, columns, p, n_imgs, st);
-  }
-  set_error("deform_conv2d_sample_columns: unsupported dtype %d", dtype);
-  return VB200_EUNSUPPORTED;
+  return dispatch_dcn_dtype(dtype, "deform_conv2d_sample_columns: unsupported dtype %d", [&](auto t) {
+    return launch_columns<decltype(t)>(input, offset, mask, columns, p, n_imgs, (cudaStream_t)stream);
+  });
 }
 
 extern "C" size_t vb200_deform_conv2d_backward_inputs_workspace_bytes(int dtype, int n_imgs, int c_in, int in_h, int in_w, int kh, int kw,
                                                                      int stride_h, int stride_w, int pad_h, int pad_w, int dil_h,
                                                                      int dil_w, int offset_groups) {
   DcnParams p;
-  if (n_imgs <= 0 || c_in <= 0 || in_h <= 0 || in_w <= 0 || kh <= 0 || kw <= 0 || stride_h <= 0 || stride_w <= 0 || dil_h <= 0 ||
-      dil_w <= 0 || pad_h < 0 || pad_w < 0)
+  if (n_imgs <= 0 || c_in <= 0 || in_h <= 0 || in_w <= 0 ||
+      dcn_params(p, n_imgs, c_in, in_h, in_w, 0, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, 1, offset_groups, 0) != 0)
     return 0;
-  if (fill_params(p, c_in, in_h, in_w, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, offset_groups, 0) != 0) return 0;
   const int pass = det_pass_imgs(p, n_imgs);
   if (pass == 0) return 0;
   return carve_det(nullptr, p, pass, dtype == VB200_F64 ? sizeof(double) : sizeof(float)).total;
@@ -446,10 +403,9 @@ extern "C" int vb200_deform_conv2d_backward_inputs_ex(const void* dcol, const vo
                                                       int pad_w, int dil_h, int dil_w, int offset_groups, int use_mask, int deterministic,
                                                       void* workspace, size_t workspace_bytes, vb200_stream stream) {
   DcnParams p;
-  VB200_REQUIRE(kh > 0 && kw > 0 && stride_h > 0 && stride_w > 0 && dil_h > 0 && dil_w > 0 && pad_h >= 0 && pad_w >= 0,
-                "deform_conv2d_backward_inputs: bad geometry");
-  VB200_REQUIRE(fill_params(p, c_in, in_h, in_w, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, offset_groups, use_mask) == 0,
-                "deform_conv2d_backward_inputs: bad sizes");
+  if (const int rc = dcn_params(p, n_imgs, c_in, in_h, in_w, 0, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, 1, offset_groups,
+                                use_mask))
+    return rc;
   if (n_imgs == 0 || c_in == 0) return 0;
   VB200_REQUIRE(dcol && input && offset && grad_input && grad_offset && (!use_mask || (mask && grad_mask)), "deform_conv2d_backward_inputs: null pointer");
   VB200_REQUIRE((int64_t)in_h * in_w < (1ll << 31), "deform_conv2d_backward_inputs: image too large");
@@ -460,22 +416,13 @@ extern "C" int vb200_deform_conv2d_backward_inputs_ex(const void* dcol, const vo
       return VB200_EUNSUPPORTED;
     }
     VB200_REQUIRE(workspace, "deform_conv2d_backward_inputs: null workspace");
-    switch (dtype) {
-      case VB200_F32: return launch_bwd_inputs_det<float>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, workspace, workspace_bytes, st);
-      case VB200_F64: return launch_bwd_inputs_det<double>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, workspace, workspace_bytes, st);
-      case VB200_F16: return launch_bwd_inputs_det<__half>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, workspace, workspace_bytes, st);
-      case VB200_BF16: return launch_bwd_inputs_det<__nv_bfloat16>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, workspace, workspace_bytes, st);
-    }
-  } else {
-    switch (dtype) {
-      case VB200_F32: return launch_bwd_inputs<float>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
-      case VB200_F64: return launch_bwd_inputs<double>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
-      case VB200_F16: return launch_bwd_inputs<__half>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
-      case VB200_BF16: return launch_bwd_inputs<__nv_bfloat16>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
-    }
   }
-  set_error("deform_conv2d_backward_inputs: unsupported dtype %d", dtype);
-  return VB200_EUNSUPPORTED;
+  return dispatch_dcn_dtype(dtype, "deform_conv2d_backward_inputs: unsupported dtype %d", [&](auto t) {
+    using T = decltype(t);
+    if (deterministic)
+      return launch_bwd_inputs_det<T>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, workspace, workspace_bytes, st);
+    return launch_bwd_inputs<T>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
+  });
 }
 
 extern "C" int vb200_deform_conv2d_backward_inputs(const void* dcol, const void* input, const void* offset, const void* mask,

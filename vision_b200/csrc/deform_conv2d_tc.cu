@@ -21,7 +21,7 @@
 #include <type_traits>
 
 #include "common.cuh"
-#include "dcn_params.h"
+#include "dcn_geometry.cuh"
 
 namespace vb200 {
 
@@ -198,45 +198,6 @@ template <> struct Elem<__half> {
   static __device__ __forceinline__ uint32_t pk(float a, float b) { __half2 v = __floats2half2_rn(a, b); return *reinterpret_cast<uint32_t*>(&v); }
 };
 
-struct __align__(16) TcEnt { int o[4]; float w[4]; };   // clamped corner pixel indices (y*W+x) + bilinear weights x mask
-
-// [KK][128] sampling table of one offset group: per (tap, pixel of the tile) the clamped corner BYTE offsets into one
-// channels-last image (pixel index x c_in x esize) and the bilinear weights x mask (zero outside the image or the tile).
-template <typename T>
-__device__ __forceinline__ void build_table(TcEnt* tab, const T* __restrict__ off_b, const T* __restrict__ msk_b, const DcnParams& p,
-                                            int pix0, int esize, int tid, int nthreads) {
-  const int KK = p.kh * p.kw, HWo = p.out_h * p.out_w;
-  for (int e = tid; e < KK * TC_BM; e += nthreads) {
-    const int tap = e / TC_BM, px = e - tap * TC_BM;
-    const int pix = pix0 + px;
-    TcEnt se;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) { se.o[q] = 0; se.w[q] = 0.f; }
-    if (pix < HWo) {
-      const int oy = pix / p.out_w, ox = pix - oy * p.out_w;
-      const int i = tap / p.kw, j = tap - i * p.kw;
-      const float oh = to_acc(off_b[(int64_t)(2 * tap) * HWo + pix]);
-      const float ow = to_acc(off_b[(int64_t)(2 * tap + 1) * HWo + pix]);
-      const float mv = p.use_mask ? to_acc(msk_b[(int64_t)tap * HWo + pix]) : 1.f;
-      const float y = add_rn((float)(oy * p.stride_h - p.pad_h + i * p.dil_h), oh);
-      const float x = add_rn((float)(ox * p.stride_w - p.pad_w + j * p.dil_w), ow);
-      if (!(y <= -1.f || (float)p.in_h <= y || x <= -1.f || (float)p.in_w <= x)) {
-        const int hl = (int)floorf(y), wl = (int)floorf(x);
-        const int hh_i = hl + 1, wh_i = wl + 1;
-        const float lh = y - (float)hl, lw = x - (float)wl;
-        const float hh = 1.f - lh, hw = 1.f - lw;
-        const bool t0 = hl >= 0, t1 = hh_i <= p.in_h - 1, l0 = wl >= 0, l1 = wh_i <= p.in_w - 1;
-        const int hlc = max(hl, 0), hhc = min(hh_i, p.in_h - 1), wlc = max(wl, 0), whc = min(wh_i, p.in_w - 1);
-        se.o[0] = (hlc * p.in_w + wlc) * p.c_in * esize; se.w[0] = (t0 && l0) ? mv * (hh * hw) : 0.f;
-        se.o[1] = (hlc * p.in_w + whc) * p.c_in * esize; se.w[1] = (t0 && l1) ? mv * (hh * lw) : 0.f;
-        se.o[2] = (hhc * p.in_w + wlc) * p.c_in * esize; se.w[2] = (t1 && l0) ? mv * (lh * hw) : 0.f;
-        se.o[3] = (hhc * p.in_w + whc) * p.c_in * esize; se.w[3] = (t1 && l1) ? mv * (lh * lw) : 0.f;
-      }
-    }
-    tab[e] = se;
-  }
-}
-
 // Writes the finished [BN channels][128 pixels] tile (shared memory, row pitch LD elements) to NCHW `out` and to the
 // peer slots of the fused all-gather: 16-byte runs along the pixels of each channel where the tile is whole and aligned.
 template <typename T, int BN>
@@ -283,7 +244,7 @@ deform_conv2d_tc_kernel(const T* __restrict__ nhwc, const T* __restrict__ wpacke
   unsigned char* stages = smem;
   uint64_t* fullB = reinterpret_cast<uint64_t*>(stages + STAGES * STAGE_BYTES);
   uint64_t* empty = fullB + STAGES;
-  TcEnt* tab = reinterpret_cast<TcEnt*>(stages + ((STAGES * STAGE_BYTES + 2 * STAGES * 8 + 31) & ~31));
+  DcnTabEnt* tab = reinterpret_cast<DcnTabEnt*>(stages + ((STAGES * STAGE_BYTES + 2 * STAGES * 8 + 31) & ~31));
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int KK = p.kh * p.kw;
@@ -333,7 +294,7 @@ deform_conv2d_tc_kernel(const T* __restrict__ nhwc, const T* __restrict__ wpacke
     asm volatile("bar.sync 1, %0;" ::"n"(WG_CONSUMERS));     // previous table no longer read
     const T* __restrict__ off_b = offset + ((int64_t)b * p.offset_groups + og) * 2 * KK * HWo;
     const T* __restrict__ msk_b = p.use_mask ? mask + ((int64_t)b * p.offset_groups + og) * KK * HWo : nullptr;
-    build_table<T>(tab, off_b, msk_b, p, pix0, 2, tid, WG_CONSUMERS);
+    fill_sample_table<TC_BM>(tab, off_b, msk_b, p, 0, KK, pix0, p.c_in * (int)sizeof(T), tid, WG_CONSUMERS);
     asm volatile("bar.sync 1, %0;" ::"n"(WG_CONSUMERS));
     // channel slab outer, tap inner (L1 reuse across taps)
     for (int sl = 0; sl < slabs_per_og; ++sl, ++q) {
@@ -345,7 +306,7 @@ deform_conv2d_tc_kernel(const T* __restrict__ nhwc, const T* __restrict__ wpacke
       float4 wq[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {                        // all 16 loads in flight before the blend
-        const TcEnt* se = tab + tap * TC_BM + prow0 + 4 * i;
+        const DcnTabEnt* se = tab + tap * TC_BM + prow0 + 4 * i;
         const uint4 o = *reinterpret_cast<const uint4*>(se->o);
         wq[i] = *reinterpret_cast<const float4*>(se->w);
         v[i][0] = __ldg(reinterpret_cast<const uint4*>(in_c + (o.x + lane_off)));
@@ -497,7 +458,7 @@ deform_conv2d_tc3_kernel(const float* __restrict__ nhwc, const __nv_bfloat16* __
   unsigned char* stages = smem;
   uint64_t* fullB = reinterpret_cast<uint64_t*>(stages + T3_STAGES * STAGE_BYTES);
   uint64_t* empty = fullB + T3_STAGES;
-  TcEnt* tab = reinterpret_cast<TcEnt*>(stages + ((T3_STAGES * STAGE_BYTES + 2 * T3_STAGES * 8 + 31) & ~31));
+  DcnTabEnt* tab = reinterpret_cast<DcnTabEnt*>(stages + ((T3_STAGES * STAGE_BYTES + 2 * T3_STAGES * 8 + 31) & ~31));
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int KK = p.kh * p.kw;
@@ -544,7 +505,7 @@ deform_conv2d_tc3_kernel(const float* __restrict__ nhwc, const __nv_bfloat16* __
     asm volatile("bar.sync 1, %0;" ::"n"(WG_CONSUMERS));
     const float* __restrict__ off_b = offset + ((int64_t)b * p.offset_groups + og) * 2 * KK * HWo;
     const float* __restrict__ msk_b = p.use_mask ? mask + ((int64_t)b * p.offset_groups + og) * KK * HWo : nullptr;
-    build_table<float>(tab, off_b, msk_b, p, pix0, 4, tid, WG_CONSUMERS);
+    fill_sample_table<TC_BM>(tab, off_b, msk_b, p, 0, KK, pix0, p.c_in * (int)sizeof(float), tid, WG_CONSUMERS);
     asm volatile("bar.sync 1, %0;" ::"n"(WG_CONSUMERS));
     for (int sl = 0; sl < slabs_per_og; ++sl, ++q) {
       const int cs_local = sl / KK, tap = sl - cs_local * KK;
@@ -554,7 +515,7 @@ deform_conv2d_tc3_kernel(const float* __restrict__ nhwc, const __nv_bfloat16* __
       float4 wq[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        const TcEnt* se = tab + tap * TC_BM + prow0 + 4 * i;
+        const DcnTabEnt* se = tab + tap * TC_BM + prow0 + 4 * i;
         const uint4 o = *reinterpret_cast<const uint4*>(se->o);
         wq[i] = *reinterpret_cast<const float4*>(se->w);
         v[i][0] = __ldg(reinterpret_cast<const float4*>(in_c + (o.x + lane_off)));
@@ -646,7 +607,7 @@ deform_conv2d_tc3_kernel(const float* __restrict__ nhwc, const __nv_bfloat16* __
 }
 
 size_t tc3_smem_bytes(int BN, int KK) {
-  return (size_t)T3_STAGES * (3 * T3_A + 3 * BN * T3_ROW) + 64 + (size_t)KK * TC_BM * sizeof(TcEnt) + 1024;
+  return (size_t)T3_STAGES * (3 * T3_A + 3 * BN * T3_ROW) + 64 + (size_t)KK * TC_BM * sizeof(DcnTabEnt) + 1024;
 }
 constexpr int T3_BN = 64;
 bool tc3_eligible(int dtype, const DcnParams& p) {
@@ -662,7 +623,7 @@ bool tc3_eligible(int dtype, const DcnParams& p) {
 // BN = 256: 3 stages x 48 KB; BN = 128: 4 stages x 32 KB (plus the [KK][128] sampling table).
 constexpr int tc_stages(int BN) { return BN == 256 ? 3 : 4; }
 size_t tc_smem_bytes(int BN, int KK) {
-  return (size_t)tc_stages(BN) * (TC_BM + BN) * 128 + 64 + (size_t)KK * TC_BM * sizeof(TcEnt) + 1024;
+  return (size_t)tc_stages(BN) * (TC_BM + BN) * 128 + 64 + (size_t)KK * TC_BM * sizeof(DcnTabEnt) + 1024;
 }
 int tc_pick_bn(const DcnParams& p) {
   const int KK = p.kh * p.kw;
