@@ -1,6 +1,7 @@
 """Small driver for ncu captures: runs one op of the hot path a few times at its BASELINE shape.
     python tools/prof_ops.py roi_align|roi_pool|ps_roi_align|ps_roi_pool|batched_nms|nms|resize|resize128|resize_noaa|deform|deform_f32|
-                             deform_bwd|deform_bwd_det|deform_bwd_f32|deform_bwd_det_f32|roi_align_bwd|roi_align_bwd_det|roi_align_bwd14|roi_align_bwd14_det|multiscale|postprocess|preprocess [iters]
+                             deform_bwd|deform_bwd_det|deform_bwd_f32|deform_bwd_det_f32|roi_align_bwd|roi_align_bwd_det|roi_align_bwd14|roi_align_bwd14_det|
+                             roi_align_bwd_p2[14][_f16][_det]|multiscale|postprocess|preprocess [iters]
     python tools/prof_ops.py retinanet_post|fcos_post|ssd_post [iters]     fused vs. reference postprocess_detections,
                              batch 1 and 8, logits N(-4.595, 1) and N(-4.595, 0.5); select-kernel time from torch.profiler"""
 import os
@@ -134,6 +135,26 @@ elif op in ("roi_align_bwd", "roi_align_bwd_det", "roi_align_bwd14", "roi_align_
     g = torch.randn(1000, 256, p, p, device=dev)
     torch.use_deterministic_algorithms(op.endswith("det"))
     fn = lambda: torch.ops.vision_b200._roi_align_backward(g, r, 0.25, p, p, 1, 256, 200, 272, 2, False)
+elif op.startswith("roi_align_bwd_p2"):
+    # FPN P2 of a padded 800 x 1344 batch of 2 (2 x 256 x 192 x 336; an fp32 plane does not fit in shared memory), 1000 RoIs,
+    # sr 2: roi_align_bwd_p2[14][_f16][_det] - 14x14 bins (mask head) instead of 7x7, fp16 instead of fp32, deterministic mode
+    gen = torch.Generator().manual_seed(0)
+    p = 14 if "p214" in op else 7
+    dt = torch.float16 if "_f16" in op else torch.float32
+    wh = torch.exp(torch.rand(1000, 2, generator=gen) * 3.0 + 2.5)
+    xy = torch.rand(1000, 2, generator=gen) * torch.tensor([1344.0, 768.0]) * 0.9
+    r = torch.cat([torch.randint(0, 2, (1000, 1), generator=gen).float(), xy, xy + wh], 1).to(dt).to(dev)
+    g = torch.randn(1000, 256, p, p, device=dev).to(dt)
+    torch.use_deterministic_algorithms(op.endswith("_det"))
+    fn = lambda: torch.ops.vision_b200._roi_align_backward(g, r, 0.25, p, p, 2, 256, 192, 336, 2, False)
+    gpu = torch.cuda.get_device_name()
+    try:
+        import subprocess
+        gpu += ", power limit " + subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
+                                                 text=True).stdout.strip().splitlines()[0]
+    except Exception:
+        pass
+    print(f"{op}: {gpu}")
 elif op == "multiscale":
     from collections import OrderedDict
     gen = torch.Generator().manual_seed(0)

@@ -8,6 +8,8 @@
    attribute is rebound (detection models call ``box_ops.batched_nms`` at call time).
 3. ``MultiScaleRoIAlign`` (torchvision/ops/poolers.py:147-228): the module-level ``_multiscale_roi_align`` is rebound
    to the fused kernel (device-side LevelMapper + one gather launch over all FPN levels) when the shape is covered.
+   ``torchvision.ops.roi_align``'s deterministic-mode route (a compiled pure-PyTorch roi_align) is rebound to the
+   dispatcher op, whose backward is bit-reproducible in that mode.
 4. detection post-processing: ``RoIHeads.postprocess_detections`` and ``RegionProposalNetwork.filter_proposals`` keep their
    tensor prologue and run the per-image tail (clip, filters, batched_nms, top-k, gathers) as one fused call;
    ``RetinaNet``, ``FCOS`` and ``SSD`` (and so SSDLite) ``postprocess_detections`` run as one fused call for all images.
@@ -70,6 +72,25 @@ def install() -> None:
         return orig_msra(x_filtered, boxes, output_size, sampling_ratio, scales, mapper)
 
     tv_poolers._multiscale_roi_align = _multiscale_roi_align
+
+    # ---- roi_align under torch.use_deterministic_algorithms (roi_align.py:250-256): torchvision sends CUDA inputs to a
+    # torch.compile'd pure-PyTorch roi_align, since its own backward is atomic.  Ours is bit-reproducible in that mode, so
+    # the route is rebound to the dispatcher op.  torchvision's lazy compile rebinds the name on its first call, so the
+    # fall-back puts ours back afterwards.
+    import sys
+
+    tv_roi_align_mod = sys.modules["torchvision.ops.roi_align"]
+    orig_det_roi_align = tv_roi_align_mod._roi_align
+
+    def _roi_align(input, rois, spatial_scale, pooled_height, pooled_width, sampling_ratio, aligned):
+        if input.is_cuda and input.dtype in (torch.float32, torch.float64, torch.float16):
+            return torch.ops.torchvision.roi_align(input, rois, spatial_scale, pooled_height, pooled_width, sampling_ratio, aligned)
+        try:
+            return orig_det_roi_align(input, rois, spatial_scale, pooled_height, pooled_width, sampling_ratio, aligned)
+        finally:
+            tv_roi_align_mod._roi_align = _roi_align
+
+    tv_roi_align_mod._roi_align = _roi_align
 
     # ---- detection post-processing around batched_nms (roi_heads.py:680-737, rpn.py:242-298) ----
     from torchvision.models.detection import roi_heads as tv_roi_heads, rpn as tv_rpn
@@ -138,6 +159,7 @@ def install() -> None:
 
     _state.update(dict(tv_boxes=tv_boxes, torchvision=torchvision, orig_batched_nms=orig_batched_nms,
                        registry=registry, saved_registry=saved, tv_poolers=tv_poolers, orig_msra=orig_msra,
+                       tv_roi_align_mod=tv_roi_align_mod, orig_det_roi_align=orig_det_roi_align,
                        tv_roi_heads=tv_roi_heads, tv_rpn=tv_rpn, orig_pp=orig_pp, orig_fp=orig_fp,
                        tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage))
 
@@ -149,6 +171,7 @@ def uninstall() -> None:
     _state["tv_boxes"].batched_nms = _state["orig_batched_nms"]
     _state["torchvision"].ops.batched_nms = _state["orig_batched_nms"]
     _state["tv_poolers"]._multiscale_roi_align = _state["orig_msra"]
+    _state["tv_roi_align_mod"]._roi_align = _state["orig_det_roi_align"]
     _state["tv_presets"].ImageClassification.forward = _state["orig_preset_forward"]
     _state["tv_roi_heads"].RoIHeads.postprocess_detections = _state["orig_pp"]
     _state["tv_rpn"].RegionProposalNetwork.filter_proposals = _state["orig_fp"]

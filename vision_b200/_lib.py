@@ -81,4 +81,5 @@ ABI_SYMBOLS = (
     "vb200_roi_backward_workspace_bytes", "vb200_roi_align_backward", "vb200_roi_pool_backward", "vb200_ps_roi_align_backward",
     "vb200_single_stage_postprocess_workspace_bytes", "vb200_single_stage_postprocess",
     "vb200_deform_conv2d_backward_inputs_workspace_bytes", "vb200_deform_conv2d_backward_inputs_ex",
+    "vb200_ps_roi_pool_backward_ex", "vb200_roi_backward_deterministic_supported",
 )

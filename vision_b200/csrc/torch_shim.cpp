@@ -52,6 +52,16 @@ at::Tensor workspace(size_t bytes, const at::Tensor& like) {
 }
 
 // ---- roi ops -------------------------------------------------------------
+// The deterministic flag for a RoI backward: torch's, after alerting (an error in strict mode, a warning with warn_only)
+// when the bit-reproducible kernels cannot take this grad_input and the op would scatter with atomics.  A dtype the ops do
+// not take is left to the entry point's own error.
+bool roi_backward_deterministic(int dt, int64_t height, int64_t width, const char* alert) {
+  if (!at::globalContext().deterministicAlgorithms()) return false;
+  const bool known = dt == VB200_F32 || dt == VB200_F64 || dt == VB200_F16;
+  if (known && !vb200_roi_backward_deterministic_supported(dt, (int)height, (int)width)) at::globalContext().alertNotDeterministic(alert);
+  return true;
+}
+
 void check_roi_inputs(const at::Tensor& input, const at::Tensor& rois) {
   TORCH_CHECK(input.is_cuda(), "input must be a CUDA tensor");
   TORCH_CHECK(rois.is_cuda(), "rois must be a CUDA tensor");
@@ -166,10 +176,14 @@ at::Tensor ps_roi_pool_backward(const at::Tensor& grad, const at::Tensor& rois, 
   at::cuda::CUDAGuard guard(grad.device());
   at::Tensor grad_input = at::empty({batch_size, channels, height, width}, grad.options());
   if (grad_input.numel() == 0) return grad_input;
+  const int dt = dtype_code(grad.scalar_type(), "ps_roi_pool_backward");
   at::Tensor g = grad.contiguous(), r = rois.contiguous();
-  check_rc(vb200_ps_roi_pool_backward(g.data_ptr(), r.data_ptr(), grad_input.data_ptr(), dtype_code(grad.scalar_type(), "ps_roi_pool_backward"),
-                                      (int)batch_size, (int)channels, (int)height, (int)width, (int)r.size(0), (int)pooled_height,
-                                      (int)pooled_width, spatial_scale, cur_stream()),
+  const bool det = roi_backward_deterministic(dt, height, width, "ps_roi_pool_backward: a grad_input row too wide for shared memory");
+  const size_t wsb = vb200_roi_backward_workspace_bytes((int)r.size(0), (int)pooled_height, (int)pooled_width, 1);
+  at::Tensor ws = workspace(wsb, grad);
+  check_rc(vb200_ps_roi_pool_backward_ex(g.data_ptr(), r.data_ptr(), grad_input.data_ptr(), dt, (int)batch_size, (int)channels,
+                                         (int)height, (int)width, (int)r.size(0), (int)pooled_height, (int)pooled_width, spatial_scale,
+                                         det ? 1 : 0, wsb ? ws.data_ptr() : nullptr, wsb, cur_stream()),
            "ps_roi_pool_backward");
   return grad_input;
 }
@@ -234,12 +248,13 @@ at::Tensor roi_align_backward(const at::Tensor& grad, const at::Tensor& rois, do
   at::Tensor grad_input = at::empty({batch_size, channels, height, width}, grad.options());
   if (grad_input.numel() == 0) return grad_input;
   const int dt = dtype_code(grad.scalar_type(), "roi_align_backward");
+  const bool det = roi_backward_deterministic(dt, height, width, "roi_align_backward: a grad_input row too wide for shared memory");
   at::Tensor g = grad.contiguous(), r = rois.contiguous();
   const size_t wsb = vb200_roi_backward_workspace_bytes((int)r.size(0), (int)pooled_height, (int)pooled_width, (int)sampling_ratio);
   at::Tensor ws = workspace(wsb, grad);
   check_rc(vb200_roi_align_backward(g.data_ptr(), r.data_ptr(), grad_input.data_ptr(), dt, (int)batch_size, (int)channels,
                                     (int)height, (int)width, (int)r.size(0), (int)pooled_height, (int)pooled_width, spatial_scale,
-                                    (int)sampling_ratio, aligned ? 1 : 0, at::globalContext().deterministicAlgorithms() ? 1 : 0,
+                                    (int)sampling_ratio, aligned ? 1 : 0, det ? 1 : 0,
                                     wsb ? ws.data_ptr() : nullptr, wsb, cur_stream()),
            "roi_align_backward");
   return grad_input;
@@ -254,12 +269,13 @@ at::Tensor roi_pool_backward(const at::Tensor& grad, const at::Tensor& rois, con
   at::Tensor grad_input = at::empty({batch_size, channels, height, width}, grad.options());
   if (grad_input.numel() == 0) return grad_input;
   const int dt = dtype_code(grad.scalar_type(), "roi_pool_backward");
+  const bool det = roi_backward_deterministic(dt, height, width, "roi_pool_backward: a grad_input row too wide for shared memory");
   at::Tensor g = grad.contiguous(), r = rois.contiguous(), am = argmax.contiguous();
   const size_t wsb = vb200_roi_backward_workspace_bytes((int)r.size(0), (int)pooled_height, (int)pooled_width, 1);
   at::Tensor ws = workspace(wsb, grad);
   check_rc(vb200_roi_pool_backward(g.data_ptr(), r.data_ptr(), am.data_ptr<int32_t>(), grad_input.data_ptr(), dt, (int)batch_size,
                                    (int)channels, (int)height, (int)width, (int)r.size(0), (int)pooled_height, (int)pooled_width,
-                                   spatial_scale, at::globalContext().deterministicAlgorithms() ? 1 : 0,
+                                   spatial_scale, det ? 1 : 0,
                                    wsb ? ws.data_ptr() : nullptr, wsb, cur_stream()),
            "roi_pool_backward");
   return grad_input;
@@ -274,13 +290,14 @@ at::Tensor ps_roi_align_backward(const at::Tensor& grad, const at::Tensor& rois,
   at::Tensor grad_input = at::empty({batch_size, channels, height, width}, grad.options());
   if (grad_input.numel() == 0) return grad_input;
   const int dt = dtype_code(grad.scalar_type(), "ps_roi_align_backward");
+  const bool det = roi_backward_deterministic(dt, height, width, "ps_roi_align_backward: a grad_input row too wide for shared memory");
   at::Tensor g = grad.contiguous(), r = rois.contiguous(), cm = channel_mapping.contiguous();
   const size_t wsb = vb200_roi_backward_workspace_bytes((int)r.size(0), (int)pooled_height, (int)pooled_width, (int)sampling_ratio);
   at::Tensor ws = workspace(wsb, grad);
   check_rc(vb200_ps_roi_align_backward(g.data_ptr(), r.data_ptr(), cm.data_ptr<int32_t>(), grad_input.data_ptr(), dt, (int)batch_size,
                                        (int)channels, (int)height, (int)width, (int)r.size(0), (int)pooled_height,
                                        (int)pooled_width, spatial_scale, (int)sampling_ratio,
-                                       at::globalContext().deterministicAlgorithms() ? 1 : 0, wsb ? ws.data_ptr() : nullptr, wsb,
+                                       det ? 1 : 0, wsb ? ws.data_ptr() : nullptr, wsb,
                                        cur_stream()),
            "ps_roi_align_backward");
   return grad_input;
