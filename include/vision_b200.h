@@ -270,6 +270,24 @@ VB200_API int vb200_single_stage_postprocess(int kind, int num_images, int num_l
                                    int semantics, void* workspace, size_t workspace_bytes, void* boxes_out,
                                    void* scores_out, int64_t* labels_out, int64_t* counts_host, vb200_stream stream);
 
+/* ---- Keypoint R-CNN keypoints from heatmaps ------------------------------------------------------------------------
+ * Replaces heatmaps_to_keypoints, torchvision/models/detection/roi_heads.py:237-307 (its per-RoI loop of bicubic
+ * F.interpolate, argmax and coordinate arithmetic), for all RoIs of a call at once.
+ * maps [K, N, H, W] (F32 / F16 / BF16, H and W at most VB200_KP_MAX_SIDE), rois [K, 4] fp32 (x1, y1, x2, y2).
+ * Per RoI the map is resized to ceil(max(y2 - y1, 1)) x ceil(max(x2 - x1, 1)) as ATen's CUDA upsample_bicubic2d does it
+ * (align_corners=False, the result rounded to the map dtype, a same-size map copied unchanged), and each keypoint's argmax
+ * (NaN above everything, ties and NaNs to the lowest index) is mapped back into the image with the reference's fp32
+ * arithmetic.  Output: xy_out [K, 3, N] (x, y, then a row of ones; the reference returns its permute(0, 2, 1)) and
+ * scores_out [K, N], the resized map's value at the argmax.  A box whose resized map has a non-finite size or 2^31 or more
+ * pixels (the reference raises for the first and cannot allocate the second) gets NaN outputs.
+ * workspace: vb200_heatmaps_to_keypoints_workspace_bytes(K, N) bytes, a function of the shapes only.  Three launches
+ * whatever K; asynchronous. */
+#define VB200_KP_MAX_SIDE 128
+VB200_API size_t vb200_heatmaps_to_keypoints_workspace_bytes(int64_t num_rois, int num_keypoints);
+VB200_API int vb200_heatmaps_to_keypoints(const void* maps, int dtype, const float* rois, int64_t num_rois, int num_keypoints,
+                                          int height, int width, float* xy_out, float* scores_out, void* workspace,
+                                          size_t workspace_bytes, vb200_stream stream);
+
 /* ---- deform_conv2d -----------------------------------------------------
  * Replaces deform_conv2d_forward_kernel, csrc/ops/cuda/deform_conv2d_kernel.cu:1035-1255
  * (schema torchvision::deform_conv2d, csrc/ops/deform_conv2d.cpp:101-102).

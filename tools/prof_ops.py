@@ -3,7 +3,8 @@
                              deform_bwd|deform_bwd_det|deform_bwd_f32|deform_bwd_det_f32|roi_align_bwd|roi_align_bwd_det|roi_align_bwd14|roi_align_bwd14_det|
                              roi_align_bwd_p2[14][_f16][_det]|multiscale|postprocess|preprocess [iters]
     python tools/prof_ops.py retinanet_post|fcos_post|ssd_post [iters]     fused vs. reference postprocess_detections,
-                             batch 1 and 8, logits N(-4.595, 1) and N(-4.595, 0.5); select-kernel time from torch.profiler"""
+                             batch 1 and 8, logits N(-4.595, 1) and N(-4.595, 0.5); select-kernel time from torch.profiler
+    python tools/prof_ops.py keypoints_post [iters]     fused vs. reference keypointrcnn_inference, batch 1 and 8"""
 import os
 import sys
 
@@ -113,8 +114,73 @@ def single_stage_post(kind: str, iters: int) -> None:
                   f"({bound_us / passes if passes else 0:.0%}); outputs identical: {same}")
 
 
+def keypoints_post(iters: int) -> None:
+    """Keypoint R-CNN's keypointrcnn_inference at batch 1 and 8, 100 detections per image, 17 x 56 x 56 maps N(0, 1), box
+    sides U(16, 600) on 800 x 1088: the fused call against the uninstalled loop; kernel times from torch.profiler."""
+    import subprocess
+
+    from torch.profiler import ProfilerActivity, profile
+    from torchvision.models.detection import roi_heads
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+    print(f"keypoints_post: {gpu.strip().splitlines()[0] if gpu.strip() else 'unknown GPU'}")
+    for batch in (1, 8):
+        gen = torch.Generator(device=dev).manual_seed(0)
+        x = torch.randn(batch * 100, 17, 56, 56, generator=gen, device=dev)
+        boxes = []
+        for _ in range(batch):
+            wh = torch.rand(100, 2, generator=gen, device=dev) * 584 + 16
+            xy = torch.rand(100, 2, generator=gen, device=dev) * (torch.tensor([1088.0, 800.0], device=dev) - wh)
+            boxes.append(torch.cat([xy, xy + wh], 1))
+        fn = lambda: roi_heads.keypointrcnn_inference(x, boxes)
+
+        def timed(n):
+            for _ in range(2):
+                fn()
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(n):
+                fn()
+            e1.record()
+            torch.cuda.synchronize()
+            return e0.elapsed_time(e1) / n
+
+        vb.uninstall()
+        ref_out = fn()
+        t_ref = timed(max(1, iters // 10))
+        vb.install()
+        try:
+            got = fn()
+            t_ours = timed(iters)
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(iters):
+                    fn()
+                torch.cuda.synchronize()
+        finally:
+            vb.uninstall()
+        kern_us = {}
+        for e in prof.key_averages():
+            for name in ("kp_geometry_kernel", "kp_sweep_kernel", "kp_finalize_kernel"):
+                if name in e.key:
+                    kern_us[name] = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / iters
+        # the bound from shapes: every output pixel of every resized map costs at least the 4-term y combination (4 FMAs)
+        # once the row values are tabled; fp32 FMA peak of the data sheet, 67 TFLOP/s = 33.5 T FMA/s
+        pixels = sum(float(((b[:, 2] - b[:, 0]).clamp(min=1).ceil() * (b[:, 3] - b[:, 1]).clamp(min=1).ceil()).sum()) for b in boxes) * 17
+        bound_us = pixels * 4 / 33.5e12 * 1e6
+        sweep = kern_us.get("kp_sweep_kernel", 0.0)
+        same = all(torch.equal(a.view(torch.int32), b.view(torch.int32)) for ra, rb in zip(ref_out, got) for a, b in zip(ra, rb))
+        kernels = ", ".join(f"{k} {v:.1f} us" for k, v in kern_us.items())
+        print(f"  batch {batch}: {pixels / 1e6:.0f} M output pixels; reference {t_ref:.3f} ms, fused {t_ours:.3f} ms "
+              f"({t_ref / t_ours:.0f}x); {kernels}; 4 FMA/pixel bound {bound_us:.1f} us ({bound_us / sweep if sweep else 0:.0%} of the sweep); "
+              f"outputs identical: {same}")
+
+
 if op in ("retinanet_post", "fcos_post", "ssd_post"):
     single_stage_post(op, iters)
+    raise SystemExit(0)
+if op == "keypoints_post":
+    keypoints_post(iters)
     raise SystemExit(0)
 if op == "roi_align":
     x, r, kw = workloads.cfg2_roi_align()

@@ -12,7 +12,9 @@
    dispatcher op, whose backward is bit-reproducible in that mode.
 4. detection post-processing: ``RoIHeads.postprocess_detections`` and ``RegionProposalNetwork.filter_proposals`` keep their
    tensor prologue and run the per-image tail (clip, filters, batched_nms, top-k, gathers) as one fused call;
-   ``RetinaNet``, ``FCOS`` and ``SSD`` (and so SSDLite) ``postprocess_detections`` run as one fused call for all images.
+   ``RetinaNet``, ``FCOS`` and ``SSD`` (and so SSDLite) ``postprocess_detections`` run as one fused call for all images;
+   the module globals ``roi_heads.keypointrcnn_inference`` and ``roi_heads.heatmaps_to_keypoints`` (Keypoint R-CNN) are
+   rebound to one keypoint-extraction call for all images.
 5. ``resize`` has no torchvision kernel (transforms/v2/functional/_geometry.py:283-362 calls
    F.interpolate): the entries of ``_KERNEL_REGISTRY[resize]`` for Tensor / Image / Video are swapped.
 CPU tensors and unsupported dtypes/modes keep flowing to the reference implementation.
@@ -112,6 +114,21 @@ def install() -> None:
     tv_roi_heads.RoIHeads.postprocess_detections = postprocess_detections
     tv_rpn.RegionProposalNetwork.filter_proposals = filter_proposals
 
+    # ---- Keypoint R-CNN inference (roi_heads.py:237-354): RoIHeads.forward looks up keypointrcnn_inference at call time ----
+    orig_kri = tv_roi_heads.keypointrcnn_inference
+    orig_h2k = tv_roi_heads.heatmaps_to_keypoints
+
+    @functools.wraps(orig_kri)
+    def keypointrcnn_inference(x, boxes):
+        return _det.keypointrcnn_inference(x, boxes, _orig=orig_kri)
+
+    @functools.wraps(orig_h2k)
+    def heatmaps_to_keypoints(maps, rois):
+        return _det.heatmaps_to_keypoints(maps, rois, _orig=orig_h2k)
+
+    tv_roi_heads.keypointrcnn_inference = keypointrcnn_inference
+    tv_roi_heads.heatmaps_to_keypoints = heatmaps_to_keypoints
+
     # ---- single-stage detectors (retinanet.py:509-571, fcos.py:489-556, ssd.py:414-463) ----
     from torchvision.models.detection import fcos as tv_fcos, retinanet as tv_retinanet, ssd as tv_ssd
 
@@ -160,7 +177,7 @@ def install() -> None:
     _state.update(dict(tv_boxes=tv_boxes, torchvision=torchvision, orig_batched_nms=orig_batched_nms,
                        registry=registry, saved_registry=saved, tv_poolers=tv_poolers, orig_msra=orig_msra,
                        tv_roi_align_mod=tv_roi_align_mod, orig_det_roi_align=orig_det_roi_align,
-                       tv_roi_heads=tv_roi_heads, tv_rpn=tv_rpn, orig_pp=orig_pp, orig_fp=orig_fp,
+                       tv_roi_heads=tv_roi_heads, tv_rpn=tv_rpn, orig_pp=orig_pp, orig_fp=orig_fp, orig_kri=orig_kri, orig_h2k=orig_h2k,
                        tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage))
 
 
@@ -175,6 +192,8 @@ def uninstall() -> None:
     _state["tv_presets"].ImageClassification.forward = _state["orig_preset_forward"]
     _state["tv_roi_heads"].RoIHeads.postprocess_detections = _state["orig_pp"]
     _state["tv_rpn"].RegionProposalNetwork.filter_proposals = _state["orig_fp"]
+    _state["tv_roi_heads"].keypointrcnn_inference = _state["orig_kri"]
+    _state["tv_roi_heads"].heatmaps_to_keypoints = _state["orig_h2k"]
     for cls, orig in _state["single_stage"].items():
         cls.postprocess_detections = orig
     reg = _state["registry"]

@@ -14,6 +14,7 @@
 //                              plane, per-tile weight tables in shared memory.
 //   resize_aa_stream_kernel    bilinear-AA downscale fast path (see below).
 //   resize_noaa_kernel         antialias=False bilinear / bicubic gather.
+#include "bicubic.cuh"
 #include "common.cuh"
 
 namespace vb200 {
@@ -189,9 +190,6 @@ resize_crop_norm_kernel(const T* __restrict__ in, float* __restrict__ out, int C
   out[plane * (int64_t)crop_h * crop_w + (int64_t)cy * crop_w + cx] = v;
 }
 
-__device__ __forceinline__ float cubic1(float x, float A) { return ((A + 2.f) * x - (A + 3.f)) * x * x + 1.f; }
-__device__ __forceinline__ float cubic2(float x, float A) { return ((A * x - 5.f * A) * x + 8.f * A) * x - 4.f * A; }
-
 template <typename T>
 __global__ void __launch_bounds__(256)
 resize_noaa_kernel(const T* __restrict__ in, T* __restrict__ out, int64_t total, int in_h, int in_w, int out_h,
@@ -214,20 +212,20 @@ resize_noaa_kernel(const T* __restrict__ in, T* __restrict__ out, int64_t total,
       const float v10 = to_acc(src[(int64_t)y1 * in_w + x0]), v11 = to_acc(src[(int64_t)y1 * in_w + x1]);
       r = l0y * (l0x * v00 + l1x * v01) + l1y * (l0x * v10 + l1x * v11);
     } else {
-      const float A = -0.75f;
-      const float ry = sh * ((float)oy + 0.5f) - 0.5f, rx = sw * ((float)ox + 0.5f) - 0.5f;
-      const int iy = (int)floorf(ry), ix = (int)floorf(rx);
-      const float ty = ry - (float)iy, tx = rx - (float)ix;
-      const float cy[4] = {cubic2(ty + 1.f, A), cubic1(ty, A), cubic1(1.f - ty, A), cubic2(1.f - ty + 1.f, A)};
-      const float cx[4] = {cubic2(tx + 1.f, A), cubic1(tx, A), cubic1(1.f - tx, A), cubic2(1.f - tx + 1.f, A)};
+      const float ry = cubic_source(sh, oy), rx = cubic_source(sw, ox);
+      int iy, ix;
+      const float ty = cubic_frac(ry, &iy), tx = cubic_frac(rx, &ix);
+      float cy[4], cx[4];
+      cubic_coeffs(ty, cy);
+      cubic_coeffs(tx, cx);
       r = 0.f;
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        const int yy = max(min(iy - 1 + k, in_h - 1), 0);
+        const int yy = cubic_clamp(iy - 1 + k, in_h);
         float v[4];
 #pragma unroll
-        for (int m = 0; m < 4; ++m) v[m] = to_acc(src[(int64_t)yy * in_w + max(min(ix - 1 + m, in_w - 1), 0)]);
-        const float rowv = v[0] * cx[0] + v[1] * cx[1] + v[2] * cx[2] + v[3] * cx[3];
+        for (int m = 0; m < 4; ++m) v[m] = to_acc(src[(int64_t)yy * in_w + cubic_clamp(ix - 1 + m, in_w)]);
+        const float rowv = cubic_interp(v[0], v[1], v[2], v[3], cx);
         r = (k == 0) ? rowv * cy[0] : r + rowv * cy[k];
       }
     }

@@ -491,6 +491,33 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> single_stage_postproc
   return std::make_tuple(ob.narrow(0, 0, total), os.narrow(0, 0, total), ol.narrow(0, 0, total), counts);
 }
 
+// ---- Keypoint R-CNN keypoints from heatmaps (roi_heads.py:237-307) ----------------------------------------------------
+// Returns the reference's (xy_preds.permute(0, 2, 1), end_scores): a [K, 3, N] buffer viewed as [K, N, 3], and [K, N].
+std::tuple<at::Tensor, at::Tensor> heatmaps_to_keypoints(const at::Tensor& maps, const at::Tensor& rois) {
+  TORCH_CHECK(maps.is_cuda() && rois.is_cuda(), "heatmaps_to_keypoints: maps and rois must be CUDA tensors");
+  TORCH_CHECK(maps.get_device() == rois.get_device(), "heatmaps_to_keypoints: maps and rois must be on the same GPU");
+  TORCH_CHECK(maps.dim() == 4, "heatmaps_to_keypoints: maps must be [K, N, H, W]");
+  TORCH_CHECK(rois.dim() == 2 && rois.size(1) == 4 && rois.size(0) == maps.size(0),
+              "heatmaps_to_keypoints: rois must be [K, 4], one box per map");
+  TORCH_CHECK(rois.scalar_type() == at::kFloat, "heatmaps_to_keypoints: rois must be float32");
+  const auto dt = maps.scalar_type();
+  TORCH_CHECK(dt == at::kFloat || dt == at::kHalf || dt == at::kBFloat16, "heatmaps_to_keypoints: maps must be float32, float16 or bfloat16");
+  const int64_t K = maps.size(0), N = maps.size(1), H = maps.size(2), W = maps.size(3);
+  TORCH_CHECK(N >= 1 && H >= 1 && W >= 1 && H <= VB200_KP_MAX_SIDE && W <= VB200_KP_MAX_SIDE,
+              "heatmaps_to_keypoints: 1..", VB200_KP_MAX_SIDE, " heatmap rows and columns and at least one keypoint");
+  at::cuda::CUDAGuard guard(maps.device());
+  at::Tensor xy = at::empty({K, 3, N}, rois.options()), scores = at::empty({K, N}, rois.options());
+  if (K > 0) {
+    at::Tensor m = maps.contiguous(), r = rois.contiguous();
+    const size_t wsb = vb200_heatmaps_to_keypoints_workspace_bytes(K, (int)N);
+    at::Tensor ws = workspace(wsb, maps);
+    check_rc(vb200_heatmaps_to_keypoints(m.data_ptr(), dtype_code(dt, "heatmaps_to_keypoints"), r.data_ptr<float>(), K, (int)N, (int)H,
+                                         (int)W, xy.data_ptr<float>(), scores.data_ptr<float>(), ws.data_ptr(), wsb, cur_stream()),
+             "heatmaps_to_keypoints");
+  }
+  return std::make_tuple(xy.permute({0, 2, 1}), scores);
+}
+
 // ---- deform_conv2d ---------------------------------------------------------
 // Packed weights are cached per weight tensor: the key is the TensorImpl (held weakly, so a recycled address cannot
 // alias) plus its version counter (an in-place update of the parameter invalidates the entry).  The packed layout follows
@@ -847,6 +874,7 @@ TORCH_LIBRARY(vision_b200, m) {
   m.def("box_iou_rotated(Tensor boxes1, Tensor boxes2) -> Tensor");
   m.def("detection_postprocess(Tensor boxes, Tensor scores, Tensor labels, float img_h, float img_w, float score_thresh, bool score_inclusive, float min_size, float nms_thresh, int topk) -> (Tensor, Tensor, Tensor)");
   m.def("single_stage_postprocess(int kind, Tensor[] logits, Tensor[] ctrness, Tensor[] regression, Tensor[] anchors, int[] image_sizes, float score_thresh, int topk_candidates, float nms_thresh, int detections_per_img, float[] weights, float bbox_xform_clip) -> (Tensor, Tensor, Tensor, Tensor)");
+  m.def("heatmaps_to_keypoints(Tensor maps, Tensor rois) -> (Tensor, Tensor)");
   m.def("multiscale_roi_align(Tensor[] features, Tensor rois, float[] scales, int pooled_height, int pooled_width, int sampling_ratio, int k_min, int k_max, float canonical_scale, float canonical_level, float eps) -> (Tensor, Tensor)");
   m.def("_roi_align_backward(Tensor grad, Tensor rois, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width, int sampling_ratio, bool aligned) -> Tensor");
   m.def("_roi_pool_backward(Tensor grad, Tensor rois, Tensor argmax, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width) -> Tensor");
@@ -879,6 +907,7 @@ TORCH_LIBRARY_IMPL(vision_b200, CUDA, m) {
   m.impl("_ps_roi_pool_backward", TORCH_FN(ps_roi_pool_backward));
   m.impl("detection_postprocess", TORCH_FN(detection_postprocess));
   m.impl("single_stage_postprocess", TORCH_FN(single_stage_postprocess));
+  m.impl("heatmaps_to_keypoints", TORCH_FN(heatmaps_to_keypoints));
   m.impl("resize_crop_normalize", TORCH_FN(resize_crop_normalize));
   m.impl("box_iou_rotated", TORCH_FN(box_iou_rotated));
   m.impl("_deform_conv2d_backward", TORCH_FN(deform_conv2d_backward));

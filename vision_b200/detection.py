@@ -6,7 +6,10 @@ batched_nms, top-k, gathers - is ONE call of ``vision_b200::detection_postproces
 
 The single-stage detectors' ``postprocess_detections`` (RetinaNet retinanet.py:509-571, FCOS fcos.py:489-556, SSD / SSDLite
 ssd.py:414-463) are ONE call of ``vision_b200::single_stage_postprocess`` for all images: score, threshold, per-level (or
-per-class) top-k, decode, clip, batched_nms and the top detections.  SSD keeps its softmax prologue as torch code."""
+per-class) top-k, decode, clip, batched_nms and the top detections.  SSD keeps its softmax prologue as torch code.
+
+Keypoint R-CNN's ``keypointrcnn_inference`` / ``heatmaps_to_keypoints`` (roi_heads.py:237-354), a per-detection loop of
+bicubic resize, argmax and coordinate arithmetic, are ONE call of ``vision_b200::heatmaps_to_keypoints`` for all images."""
 from __future__ import annotations
 
 import torch
@@ -166,3 +169,50 @@ def ssd_postprocess_detections(self, head_outputs, image_anchors, image_shapes, 
     coder = self.box_coder
     return single_stage_postprocess(_SS_SSD, [pred_scores], [], [regression], image_anchors, image_shapes, self.score_thresh,
                                     self.topk_candidates, self.nms_thresh, self.detections_per_img, coder.weights, coder.bbox_xform_clip)
+
+
+# largest heatmap side the keypoint kernel stages in shared memory (VB200_KP_MAX_SIDE in include/vision_b200.h)
+KEYPOINTS_MAX_SIDE = 128
+
+
+def keypoints_supported(maps, rois) -> bool:
+    """Inputs the keypoint kernel takes: CUDA fp32 / fp16 / bf16 maps [K, N, H, W] with H, W <= KEYPOINTS_MAX_SIDE, fp32 rois
+    [K, 4] on the same device, outside scripting and tracing (the reference keeps its ONNX loop there)."""
+    return (isinstance(maps, Tensor) and isinstance(rois, Tensor) and maps.is_cuda and rois.is_cuda and maps.device == rois.device
+            and maps.dtype in (torch.float32, torch.float16, torch.bfloat16) and maps.dim() == 4 and rois.dtype == torch.float32
+            and rois.dim() == 2 and rois.shape[1] == 4 and maps.shape[0] == rois.shape[0] and maps.shape[1] >= 1
+            and 1 <= maps.shape[2] <= KEYPOINTS_MAX_SIDE and 1 <= maps.shape[3] <= KEYPOINTS_MAX_SIDE and not _traced())
+
+
+def _boxes_sized(rois: Tensor) -> bool:
+    """The one host read-back of a call: every box's resized map has a finite size below 2^31 pixels.  The others go to the
+    reference body, which raises (a NaN or infinite size) or behaves as it does today.  fp32 rounds the product up, never
+    down, across 2^31, so no box past the limit passes."""
+    wh = (rois[:, 2:] - rois[:, :2]).clamp(min=1).ceil()
+    return bool((wh[:, 0] * wh[:, 1] < 2.0**31).all())
+
+
+def heatmaps_to_keypoints_op(maps: Tensor, rois: Tensor):
+    _lib.load_ops()
+    return torch.ops.vision_b200.heatmaps_to_keypoints(maps, rois)
+
+
+def heatmaps_to_keypoints(maps, rois, _orig=None):
+    """roi_heads.heatmaps_to_keypoints as one fused call (same outputs, shapes and strides)."""
+    if not (keypoints_supported(maps, rois) and _boxes_sized(rois)):
+        return _orig(maps, rois)
+    return heatmaps_to_keypoints_op(maps, rois)
+
+
+def keypointrcnn_inference(x, boxes, _orig=None):
+    """roi_heads.keypointrcnn_inference with every image's heatmaps_to_keypoints in ONE call: the boxes concatenated, one op,
+    per-image views of its outputs."""
+    if not (isinstance(boxes, (list, tuple)) and boxes
+            and all(isinstance(b, Tensor) and b.is_cuda and b.dtype == torch.float32 for b in boxes)):
+        return _orig(x, boxes)
+    rois = torch.cat(list(boxes)) if len(boxes) > 1 else boxes[0]
+    if not (keypoints_supported(x, rois) and _boxes_sized(rois)):
+        return _orig(x, boxes)
+    xy, scores = heatmaps_to_keypoints_op(x, rois)
+    counts = [b.size(0) for b in boxes]
+    return list(xy.split(counts)), list(scores.split(counts))
