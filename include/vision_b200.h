@@ -288,6 +288,44 @@ VB200_API int vb200_heatmaps_to_keypoints(const void* maps, int dtype, const flo
                                           int height, int width, float* xy_out, float* scores_out, void* workspace,
                                           size_t workspace_bytes, vb200_stream stream);
 
+/* ---- detection model input batching ---------------------------------------------------------------------------------
+ * Replaces GeneralizedRCNNTransform.forward's inference loop, torchvision/models/detection/transform.py:119-158 with
+ * normalize (:160-169), _resize_image_and_masks (:25-83) and batch_images (:237-255), for all images at once.
+ * Image i is [channels, in_h, in_w] at `data` with element strides (stride_c, stride_h, stride_w), read in place.  Each
+ * element of the padded batch output [num_images, channels, pad_h, pad_w] (contiguous, `dtype` = F32 / F16 / BF16 for
+ * every image) is either +0.0 or pixel (y, x) of image i normalized and resized to out_h x out_w: (v - mean[c]) and then
+ * / std[c], each computed in fp32 and rounded to the dtype, then ATen's CUDA upsample_bilinear2d (align_corners=False,
+ * scale (float)in / out, fp32 blend; an image whose size does not change is copied, as ATen's kernel does) of those
+ * values, rounded to the dtype.  mean_host / std_host: HOST arrays of
+ * `channels` floats (<= 8 channels), already rounded to the dtype.  One launch per VB200_RCNN_MAX_IMAGES images. */
+#define VB200_RCNN_MAX_IMAGES 256
+typedef struct vb200_rcnn_image {
+  const void* data;
+  int64_t stride_c, stride_h, stride_w;
+  int in_h, in_w, out_h, out_w;
+} vb200_rcnn_image;
+VB200_API int vb200_rcnn_batch_images(const vb200_rcnn_image* images, int num_images, int channels, int dtype, int pad_h,
+                                      int pad_w, const float* mean_host, const float* std_host, void* output,
+                                      vb200_stream stream);
+
+/* ---- detection output rescaling ---------------------------------------------------------------------------------------
+ * Replaces GeneralizedRCNNTransform.postprocess's resize_boxes and resize_keypoints, transform.py:257-277, 288-319, for
+ * all images at once.  Item k is a fp32 [rows, cols, width] array (boxes: cols 1, width 4; keypoints: width 3) read with
+ * in_stride and written with out_stride (elements): columns 0 and 2 of a box and column 0 of a keypoint are multiplied
+ * by ratio_w, columns 1 and 3 of a box and column 1 of a keypoint by ratio_h (each a single fp32 product), a keypoint's
+ * column 2 is copied.  ratio_w / ratio_h: the fp32 quotient new / original size.  One launch per VB200_RCNN_MAX_RESCALE
+ * items. */
+#define VB200_RCNN_MAX_RESCALE 128
+typedef struct vb200_rcnn_rescale_item {
+  const float* input;
+  float* output;
+  int64_t in_stride[3], out_stride[3];
+  int64_t rows;
+  int cols, width;
+  float ratio_w, ratio_h;
+} vb200_rcnn_rescale_item;
+VB200_API int vb200_rcnn_rescale(const vb200_rcnn_rescale_item* items, int num_items, vb200_stream stream);
+
 /* ---- deform_conv2d -----------------------------------------------------
  * Replaces deform_conv2d_forward_kernel, csrc/ops/cuda/deform_conv2d_kernel.cu:1035-1255
  * (schema torchvision::deform_conv2d, csrc/ops/deform_conv2d.cpp:101-102).

@@ -4,7 +4,9 @@
                              roi_align_bwd_p2[14][_f16][_det]|multiscale|postprocess|preprocess [iters]
     python tools/prof_ops.py retinanet_post|fcos_post|ssd_post [iters]     fused vs. reference postprocess_detections,
                              batch 1 and 8, logits N(-4.595, 1) and N(-4.595, 0.5); select-kernel time from torch.profiler
-    python tools/prof_ops.py keypoints_post [iters]     fused vs. reference keypointrcnn_inference, batch 1 and 8"""
+    python tools/prof_ops.py keypoints_post [iters]     fused vs. reference keypointrcnn_inference, batch 1 and 8
+    python tools/prof_ops.py rcnn_transform [iters]     fused vs. reference GeneralizedRCNNTransform forward + postprocess,
+                             batch 1 and 8, fp32 and fp16"""
 import os
 import sys
 
@@ -176,6 +178,88 @@ def keypoints_post(iters: int) -> None:
               f"outputs identical: {same}")
 
 
+def rcnn_transform(iters: int) -> None:
+    """GeneralizedRCNNTransform (Faster R-CNN settings) forward + postprocess at batch 1 and 8 of COCO-like sizes, fp32 and fp16,
+    100 boxes per image: the fused methods against the uninstalled ones.  Wall time per call ending in a synchronize, CUDA-event
+    time, rcnn_batch_kernel time from torch.profiler and its share of the HBM bound (input plus padded output bytes)."""
+    import subprocess
+    import time
+
+    from torch.profiler import ProfilerActivity, profile
+    from torchvision.models.detection.transform import GeneralizedRCNNTransform
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+    print(f"rcnn_transform: {gpu.strip().splitlines()[0] if gpu.strip() else 'unknown GPU'}")
+    t = GeneralizedRCNNTransform(800, 1333, [0.485, 0.456, 0.406], [0.229, 0.224, 0.225]).eval()
+    shapes = [(480, 640), (427, 640), (640, 480), (480, 640), (500, 375), (612, 612), (480, 640), (333, 500)]
+    for dtype in (torch.float32, torch.float16):
+        for batch in (1, 8):
+            gen = torch.Generator(device=dev).manual_seed(0)
+            images = [torch.rand(3, h, w, generator=gen, device=dev).to(dtype) for h, w in shapes[:batch]]
+            result = []
+            for _ in range(batch):
+                xy = torch.rand(100, 2, generator=gen, device=dev) * 700
+                result.append({"boxes": torch.cat([xy, xy + torch.rand(100, 2, generator=gen, device=dev) * 300], 1),
+                               "scores": torch.rand(100, generator=gen, device=dev),
+                               "labels": torch.ones(100, dtype=torch.int64, device=dev)})
+            orig = [tuple(img.shape[-2:]) for img in images]
+
+            def fn():
+                image_list, _ = t(images)
+                return image_list, t.postprocess([dict(r) for r in result], image_list.image_sizes, orig)
+
+            def timed(n):
+                for _ in range(3):
+                    fn()
+                torch.cuda.synchronize()
+                wall = []
+                for _ in range(n):
+                    t0 = time.perf_counter()
+                    fn()
+                    torch.cuda.synchronize()
+                    wall.append(time.perf_counter() - t0)
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for _ in range(n):
+                    fn()
+                e1.record()
+                torch.cuda.synchronize()
+                return sorted(wall)[n // 2] * 1e3, e0.elapsed_time(e1) / n
+
+            vb.uninstall()
+            ref_out = fn()
+            ref_wall, ref_ev = timed(iters)
+            vb.install()
+            try:
+                got = fn()
+                wall, ev = timed(iters)
+                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                    for _ in range(iters):
+                        fn()
+                    torch.cuda.synchronize()
+            finally:
+                vb.uninstall()
+            kern_us = {}
+            for e in prof.key_averages():
+                for name in ("rcnn_batch_kernel", "rcnn_rescale_kernel"):
+                    if name in e.key:
+                        kern_us[name] = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / iters
+            nbytes = sum(img.numel() for img in images) * images[0].element_size() + got[0].tensors.numel() * got[0].tensors.element_size()
+            bound_us = nbytes / 3.35e12 * 1e6
+            bk = kern_us.get("rcnn_batch_kernel", 0.0)
+            bits = lambda x: x.reshape(-1).view(torch.int16 if x.element_size() == 2 else torch.int32)  # noqa: E731
+            same = (ref_out[0].image_sizes == got[0].image_sizes and torch.equal(bits(ref_out[0].tensors), bits(got[0].tensors))
+                    and all(torch.equal(bits(a["boxes"]), bits(b["boxes"])) for a, b in zip(ref_out[1], got[1])))
+            kernels = ", ".join(f"{k} {v:.1f} us" for k, v in kern_us.items())
+            print(f"  {str(dtype).split('.')[-1]} batch {batch} -> {tuple(got[0].tensors.shape)}: reference wall {ref_wall:.3f} ms, "
+                  f"events {ref_ev:.3f} ms; fused wall {wall:.3f} ms, events {ev:.3f} ms ({ref_wall / wall:.1f}x wall); {kernels}; "
+                  f"{nbytes / 1e6:.0f} MB at 3.35 TB/s = {bound_us:.1f} us ({bound_us / bk if bk else 0:.0%} of the batch kernel); "
+                  f"outputs identical: {same}")
+
+
+if op == "rcnn_transform":
+    rcnn_transform(iters)
+    raise SystemExit(0)
 if op in ("retinanet_post", "fcos_post", "ssd_post"):
     single_stage_post(op, iters)
     raise SystemExit(0)

@@ -173,6 +173,10 @@ def register() -> None:
     def _(inp, out_h, out_w, mode, antialias):
         return inp.new_empty(tuple(inp.shape[:-2]) + (out_h, out_w))
 
+    @lib.register_fake("vision_b200::rcnn_batch_images")
+    def _(images, out_h, out_w, pad_h, pad_w, mean, std):
+        return images[0].new_empty((len(images), images[0].shape[0], pad_h, pad_w))
+
     # ---- deform_conv2d ----
     def dcn_setup(ctx, inputs, output):
         inp, weight, offset, mask, bias = inputs[:5]

@@ -15,6 +15,9 @@
    ``RetinaNet``, ``FCOS`` and ``SSD`` (and so SSDLite) ``postprocess_detections`` run as one fused call for all images;
    the module globals ``roi_heads.keypointrcnn_inference`` and ``roi_heads.heatmaps_to_keypoints`` (Keypoint R-CNN) are
    rebound to one keypoint-extraction call for all images.
+   ``GeneralizedRCNNTransform.forward`` and ``.postprocess``, which every detection model enters and leaves through, are
+   rebound on the class: normalize, resize and padding of all images in one call, the rescaling of every image's boxes and
+   keypoints in another.
 5. ``resize`` has no torchvision kernel (transforms/v2/functional/_geometry.py:283-362 calls
    F.interpolate): the entries of ``_KERNEL_REGISTRY[resize]`` for Tensor / Image / Video are swapped.
 CPU tensors and unsupported dtypes/modes keep flowing to the reference implementation.
@@ -129,6 +132,24 @@ def install() -> None:
     tv_roi_heads.keypointrcnn_inference = keypointrcnn_inference
     tv_roi_heads.heatmaps_to_keypoints = heatmaps_to_keypoints
 
+    # ---- detection model inputs and outputs (transform.py:119-158, 257-277): bound on the class, so every model's
+    # self.transform (Faster / Mask / Keypoint R-CNN, RetinaNet, FCOS, SSD, SSDLite) picks them up ----
+    from torchvision.models.detection import transform as tv_transform
+
+    rcnn_transform = tv_transform.GeneralizedRCNNTransform
+    orig_tf_forward, orig_tf_post = rcnn_transform.forward, rcnn_transform.postprocess
+
+    @functools.wraps(orig_tf_forward)
+    def transform_forward(self, images, targets=None):
+        return _det.rcnn_transform_forward(self, images, targets, _orig=orig_tf_forward)
+
+    @functools.wraps(orig_tf_post)
+    def transform_postprocess(self, result, image_shapes, original_image_sizes):
+        return _det.rcnn_transform_postprocess(self, result, image_shapes, original_image_sizes, _orig=orig_tf_post)
+
+    rcnn_transform.forward = transform_forward
+    rcnn_transform.postprocess = transform_postprocess
+
     # ---- single-stage detectors (retinanet.py:509-571, fcos.py:489-556, ssd.py:414-463) ----
     from torchvision.models.detection import fcos as tv_fcos, retinanet as tv_retinanet, ssd as tv_ssd
 
@@ -178,7 +199,8 @@ def install() -> None:
                        registry=registry, saved_registry=saved, tv_poolers=tv_poolers, orig_msra=orig_msra,
                        tv_roi_align_mod=tv_roi_align_mod, orig_det_roi_align=orig_det_roi_align,
                        tv_roi_heads=tv_roi_heads, tv_rpn=tv_rpn, orig_pp=orig_pp, orig_fp=orig_fp, orig_kri=orig_kri, orig_h2k=orig_h2k,
-                       tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage))
+                       tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage,
+                       rcnn_transform=rcnn_transform, orig_tf_forward=orig_tf_forward, orig_tf_post=orig_tf_post))
 
 
 def uninstall() -> None:
@@ -194,6 +216,8 @@ def uninstall() -> None:
     _state["tv_rpn"].RegionProposalNetwork.filter_proposals = _state["orig_fp"]
     _state["tv_roi_heads"].keypointrcnn_inference = _state["orig_kri"]
     _state["tv_roi_heads"].heatmaps_to_keypoints = _state["orig_h2k"]
+    _state["rcnn_transform"].forward = _state["orig_tf_forward"]
+    _state["rcnn_transform"].postprocess = _state["orig_tf_post"]
     for cls, orig in _state["single_stage"].items():
         cls.postprocess_detections = orig
     reg = _state["registry"]

@@ -83,4 +83,5 @@ ABI_SYMBOLS = (
     "vb200_deform_conv2d_backward_inputs_workspace_bytes", "vb200_deform_conv2d_backward_inputs_ex",
     "vb200_ps_roi_pool_backward_ex", "vb200_roi_backward_deterministic_supported",
     "vb200_heatmaps_to_keypoints_workspace_bytes", "vb200_heatmaps_to_keypoints",
+    "vb200_rcnn_batch_images", "vb200_rcnn_rescale",
 )

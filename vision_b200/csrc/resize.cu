@@ -15,6 +15,7 @@
 //   resize_aa_stream_kernel    bilinear-AA downscale fast path (see below).
 //   resize_noaa_kernel         antialias=False bilinear / bicubic gather.
 #include "bicubic.cuh"
+#include "bilinear.cuh"
 #include "common.cuh"
 
 namespace vb200 {
@@ -174,15 +175,7 @@ resize_crop_norm_kernel(const T* __restrict__ in, float* __restrict__ out, int C
   } else {
     // upsample_bilinear2d (align_corners=False), as resize_noaa_kernel
     const float sh = (float)in_h / (float)rs_h, sw = (float)in_w / (float)rs_w;
-    float ry = sh * ((float)oy + 0.5f) - 0.5f; if (ry < 0.f) ry = 0.f;
-    float rx = sw * ((float)ox + 0.5f) - 0.5f; if (rx < 0.f) rx = 0.f;
-    const int y0 = min((int)ry, in_h - 1), x0 = min((int)rx, in_w - 1);
-    const int y1 = y0 + (y0 < in_h - 1 ? 1 : 0), x1 = x0 + (x0 < in_w - 1 ? 1 : 0);
-    const float l1y = fminf(fmaxf(ry - (float)y0, 0.f), 1.f), l1x = fminf(fmaxf(rx - (float)x0, 0.f), 1.f);
-    const float l0y = 1.f - l1y, l0x = 1.f - l1x;
-    const float v00 = to_acc(src[(int64_t)y0 * in_w + x0]), v01 = to_acc(src[(int64_t)y0 * in_w + x1]);
-    const float v10 = to_acc(src[(int64_t)y1 * in_w + x0]), v11 = to_acc(src[(int64_t)y1 * in_w + x1]);
-    acc = l0y * (l0x * v00 + l1x * v01) + l1y * (l0x * v10 + l1x * v11);
+    acc = bilinear_sample(sh, sw, oy, ox, in_h, in_w, [=](int y, int x) { return to_acc(src[(int64_t)y * in_w + x]); });
   }
   float v = storage_round<T>(acc, mode);                       // the resized image exists in the storage dtype in the reference
   v = __fmul_rn(v, np.int_scale);                              // convert_image_dtype: uint8 -> x / 255 (CUDA tensor / scalar = x * (1/255))
@@ -202,15 +195,7 @@ resize_noaa_kernel(const T* __restrict__ in, T* __restrict__ out, int64_t total,
     float r;
     if (mode == VB200_RESIZE_BILINEAR) {
       // upsample_bilinear2d: area_pixel_compute_source_index (align_corners=False, clamp at 0)
-      float ry = sh * ((float)oy + 0.5f) - 0.5f; if (ry < 0.f) ry = 0.f;
-      float rx = sw * ((float)ox + 0.5f) - 0.5f; if (rx < 0.f) rx = 0.f;
-      const int y0 = min((int)ry, in_h - 1), x0 = min((int)rx, in_w - 1);
-      const int y1 = y0 + (y0 < in_h - 1 ? 1 : 0), x1 = x0 + (x0 < in_w - 1 ? 1 : 0);
-      const float l1y = fminf(fmaxf(ry - (float)y0, 0.f), 1.f), l1x = fminf(fmaxf(rx - (float)x0, 0.f), 1.f);
-      const float l0y = 1.f - l1y, l0x = 1.f - l1x;
-      const float v00 = to_acc(src[(int64_t)y0 * in_w + x0]), v01 = to_acc(src[(int64_t)y0 * in_w + x1]);
-      const float v10 = to_acc(src[(int64_t)y1 * in_w + x0]), v11 = to_acc(src[(int64_t)y1 * in_w + x1]);
-      r = l0y * (l0x * v00 + l1x * v01) + l1y * (l0x * v10 + l1x * v11);
+      r = bilinear_sample(sh, sw, oy, ox, in_h, in_w, [=](int y, int x) { return to_acc(src[(int64_t)y * in_w + x]); });
     } else {
       const float ry = cubic_source(sh, oy), rx = cubic_source(sw, ox);
       int iy, ix;

@@ -809,6 +809,77 @@ at::Tensor resize_crop_normalize(const at::Tensor& input, int64_t resize_h, int6
   return out;
 }
 
+// ---- detection model inputs and outputs (models/detection/transform.py:119-158, 257-277) ----------------------------
+// images: B tensors [C, H_i, W_i] of one dtype on one GPU, any strides; out_h / out_w: each image's resized size; mean / std:
+// C values already rounded to the images' dtype.  Returns the padded batch [B, C, pad_h, pad_w].
+at::Tensor rcnn_batch_images(at::TensorList images, at::IntArrayRef out_h, at::IntArrayRef out_w, int64_t pad_h, int64_t pad_w,
+                             at::ArrayRef<double> mean, at::ArrayRef<double> std) {
+  const int64_t B = (int64_t)images.size();
+  TORCH_CHECK(B >= 1 && (int64_t)out_h.size() == B && (int64_t)out_w.size() == B, "rcnn_batch_images: one output size per image");
+  const at::Tensor& i0 = images[0];
+  TORCH_CHECK(i0.is_cuda() && i0.dim() == 3, "rcnn_batch_images: images must be CUDA tensors [C, H, W]");
+  const int64_t C = i0.size(0);
+  TORCH_CHECK(C >= 1 && C <= 8 && (int64_t)mean.size() == C && (int64_t)std.size() == C,
+              "rcnn_batch_images: 1..8 channels, one mean / std per channel");
+  const auto dt = i0.scalar_type();
+  TORCH_CHECK(dt == at::kFloat || dt == at::kHalf || dt == at::kBFloat16, "rcnn_batch_images: images must be float32, float16 or bfloat16");
+  std::vector<vb200_rcnn_image> desc((size_t)B);
+  for (int64_t i = 0; i < B; ++i) {
+    const at::Tensor& t = images[i];
+    TORCH_CHECK(t.is_cuda() && t.get_device() == i0.get_device() && t.scalar_type() == dt && t.dim() == 3 && t.size(0) == C,
+                "rcnn_batch_images: every image must be a [C, H, W] tensor of the first one's dtype, channels and GPU");
+    TORCH_CHECK(t.size(1) >= 1 && t.size(2) >= 1 && t.size(1) * t.size(2) < ((int64_t)1 << 31) && out_h[i] >= 1 && out_w[i] >= 1 &&
+                    out_h[i] <= pad_h && out_w[i] <= pad_w,
+                "rcnn_batch_images: image ", i, " of ", t.size(1), " x ", t.size(2), " resized to ", out_h[i], " x ", out_w[i],
+                " does not fit ", pad_h, " x ", pad_w);
+    desc[i] = {t.data_ptr(), t.stride(0), t.stride(1), t.stride(2), (int)t.size(1), (int)t.size(2), (int)out_h[i], (int)out_w[i]};
+  }
+  TORCH_CHECK(pad_h * pad_w < ((int64_t)1 << 31), "rcnn_batch_images: padded planes of 2^31 or more elements");
+  at::cuda::CUDAGuard guard(i0.device());
+  at::Tensor out = at::empty({B, C, pad_h, pad_w}, i0.options());
+  float m[8], sd[8];
+  for (int64_t c = 0; c < C; ++c) { m[c] = (float)mean[c]; sd[c] = (float)std[c]; }
+  check_rc(vb200_rcnn_batch_images(desc.data(), (int)B, (int)C, dtype_code(dt, "rcnn_batch_images"), (int)pad_h, (int)pad_w, m, sd,
+                                   out.data_ptr(), cur_stream()),
+           "rcnn_batch_images");
+  return out;
+}
+
+// inputs: fp32 boxes [N, 4] (returned contiguous, as the reference's stack) or keypoints [N, K, 3] (returned with the input's
+// strides, as the reference's clone), all on one GPU; ratio_w / ratio_h: one fp32 new / original quotient pair per input.
+std::vector<at::Tensor> rcnn_rescale(at::TensorList inputs, at::ArrayRef<double> ratio_w, at::ArrayRef<double> ratio_h) {
+  const size_t n = inputs.size();
+  TORCH_CHECK(ratio_w.size() == n && ratio_h.size() == n, "rcnn_rescale: one ratio pair per input");
+  std::vector<at::Tensor> outs;
+  if (n == 0) return outs;
+  at::cuda::CUDAGuard guard(inputs[0].device());
+  std::vector<vb200_rcnn_rescale_item> items(n);
+  for (size_t k = 0; k < n; ++k) {
+    const at::Tensor& t = inputs[k];
+    TORCH_CHECK(t.is_cuda() && t.get_device() == inputs[0].get_device() && t.scalar_type() == at::kFloat,
+                "rcnn_rescale: inputs must be float32 tensors on one GPU");
+    const bool boxes = t.dim() == 2 && t.size(1) == 4;
+    TORCH_CHECK(boxes || (t.dim() == 3 && t.size(2) == 3), "rcnn_rescale: inputs must be boxes [N, 4] or keypoints [N, K, 3]");
+    at::Tensor o = boxes ? at::empty({t.size(0), 4}, t.options()) : at::empty_like(t);
+    vb200_rcnn_rescale_item& it = items[k];
+    it.input = t.data_ptr<float>();
+    it.output = o.data_ptr<float>();
+    it.rows = t.numel() ? t.size(0) : 0;
+    it.cols = boxes ? 1 : std::max<int>((int)t.size(1), 1);
+    it.width = boxes ? 4 : 3;
+    for (int d = 0; d < 3; ++d) {
+      const int s = boxes ? (d == 0 ? 0 : d == 1 ? -1 : 1) : d;   // boxes: (row, -, column)
+      it.in_stride[d] = s < 0 ? 0 : t.stride(s);
+      it.out_stride[d] = s < 0 ? 0 : o.stride(s);
+    }
+    it.ratio_w = (float)ratio_w[k];
+    it.ratio_h = (float)ratio_h[k];
+    outs.push_back(o);
+  }
+  check_rc(vb200_rcnn_rescale(items.data(), (int)n, cur_stream()), "rcnn_rescale");
+  return outs;
+}
+
 // ---- box_iou_rotated (csrc/ops/box_iou_rotated.cpp; checks as cuda/box_iou_rotated_kernel.cu:92-118) ----------------
 at::Tensor box_iou_rotated(const at::Tensor& boxes1, const at::Tensor& boxes2) {
   TORCH_CHECK(boxes1.is_cuda() && boxes2.is_cuda(), "boxes1 and boxes2 must be CUDA tensors");
@@ -875,6 +946,8 @@ TORCH_LIBRARY(vision_b200, m) {
   m.def("detection_postprocess(Tensor boxes, Tensor scores, Tensor labels, float img_h, float img_w, float score_thresh, bool score_inclusive, float min_size, float nms_thresh, int topk) -> (Tensor, Tensor, Tensor)");
   m.def("single_stage_postprocess(int kind, Tensor[] logits, Tensor[] ctrness, Tensor[] regression, Tensor[] anchors, int[] image_sizes, float score_thresh, int topk_candidates, float nms_thresh, int detections_per_img, float[] weights, float bbox_xform_clip) -> (Tensor, Tensor, Tensor, Tensor)");
   m.def("heatmaps_to_keypoints(Tensor maps, Tensor rois) -> (Tensor, Tensor)");
+  m.def("rcnn_batch_images(Tensor[] images, int[] out_h, int[] out_w, int pad_h, int pad_w, float[] mean, float[] std) -> Tensor");
+  m.def("rcnn_rescale(Tensor[] inputs, float[] ratio_w, float[] ratio_h) -> Tensor[]");
   m.def("multiscale_roi_align(Tensor[] features, Tensor rois, float[] scales, int pooled_height, int pooled_width, int sampling_ratio, int k_min, int k_max, float canonical_scale, float canonical_level, float eps) -> (Tensor, Tensor)");
   m.def("_roi_align_backward(Tensor grad, Tensor rois, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width, int sampling_ratio, bool aligned) -> Tensor");
   m.def("_roi_pool_backward(Tensor grad, Tensor rois, Tensor argmax, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width) -> Tensor");
@@ -908,6 +981,8 @@ TORCH_LIBRARY_IMPL(vision_b200, CUDA, m) {
   m.impl("detection_postprocess", TORCH_FN(detection_postprocess));
   m.impl("single_stage_postprocess", TORCH_FN(single_stage_postprocess));
   m.impl("heatmaps_to_keypoints", TORCH_FN(heatmaps_to_keypoints));
+  m.impl("rcnn_batch_images", TORCH_FN(rcnn_batch_images));
+  m.impl("rcnn_rescale", TORCH_FN(rcnn_rescale));
   m.impl("resize_crop_normalize", TORCH_FN(resize_crop_normalize));
   m.impl("box_iou_rotated", TORCH_FN(box_iou_rotated));
   m.impl("_deform_conv2d_backward", TORCH_FN(deform_conv2d_backward));

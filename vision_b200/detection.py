@@ -9,9 +9,16 @@ ssd.py:414-463) are ONE call of ``vision_b200::single_stage_postprocess`` for al
 per-class) top-k, decode, clip, batched_nms and the top detections.  SSD keeps its softmax prologue as torch code.
 
 Keypoint R-CNN's ``keypointrcnn_inference`` / ``heatmaps_to_keypoints`` (roi_heads.py:237-354), a per-detection loop of
-bicubic resize, argmax and coordinate arithmetic, are ONE call of ``vision_b200::heatmaps_to_keypoints`` for all images."""
+bicubic resize, argmax and coordinate arithmetic, are ONE call of ``vision_b200::heatmaps_to_keypoints`` for all images.
+
+``GeneralizedRCNNTransform.forward`` (transform.py:119-158), which every detection model enters through, is ONE call of
+``vision_b200::rcnn_batch_images`` (normalize, bilinear resize and zero padding of all images); its ``postprocess``
+(:257-277) rescales every image's boxes and keypoints with ONE call of ``vision_b200::rcnn_rescale``."""
 from __future__ import annotations
 
+import math
+
+import numpy as np
 import torch
 import torch.nn.functional as F
 from torch import Tensor
@@ -216,3 +223,125 @@ def keypointrcnn_inference(x, boxes, _orig=None):
     xy, scores = heatmaps_to_keypoints_op(x, rois)
     counts = [b.size(0) for b in boxes]
     return list(xy.split(counts)), list(scores.split(counts))
+
+
+_RCNN_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+_RCNN_MAX_CHANNELS = 8
+_RCNN_MAX_PAD_H = 65535 * 8          # rows of the batch kernel's grid: 65535 tiles of 8
+
+
+def rcnn_output_size(h: int, w: int, min_size, max_size, fixed_size):
+    """The size _resize_image_and_masks (transform.py:25-72) resizes an h x w image to in eval mode: fixed_size reversed, or
+    F.interpolate's recompute_scale_factor rule, int(side * scale) with the scale in Python double."""
+    if fixed_size is not None:
+        return int(fixed_size[1]), int(fixed_size[0])
+    scale = min(min_size / min(h, w), max_size / max(h, w))
+    return int(h * scale), int(w * scale)
+
+
+def _rcnn_batch_plan(self, images):
+    """The per-image output sizes and the padded size when the batch kernel reproduces the reference's forward for these
+    images, else None.  Inference only, outside deterministic mode (F.interpolate decomposes there), scripting and
+    tracing; CUDA images [C, H, W] of one dtype (fp32, or fp16 / bf16 with autocast off), device and channel count, one
+    mean and std per channel (the reference broadcasts others), output sides >= 1 and planes below 2^31 elements."""
+    if (self.training or torch.are_deterministic_algorithms_enabled() or _traced() or not images
+            or not all(isinstance(img, Tensor) for img in images)):
+        return None
+    i0 = images[0]
+    if not (i0.is_cuda and i0.dtype in _RCNN_DTYPES and i0.dim() == 3):
+        return None
+    if i0.dtype != torch.float32 and torch.is_autocast_enabled("cuda"):
+        return None
+    C = i0.shape[0]
+    if not (1 <= C <= _RCNN_MAX_CHANNELS and len(self.image_mean) == C and len(self.image_std) == C):
+        return None
+    sizes = []
+    for img in images:
+        if not (img.device == i0.device and img.dtype == i0.dtype and img.dim() == 3 and img.shape[0] == C):
+            return None
+        h, w = img.shape[-2:]
+        if h < 1 or w < 1 or h * w >= 2**31:
+            return None
+        oh, ow = rcnn_output_size(h, w, self.min_size[-1], self.max_size, self.fixed_size)
+        if oh < 1 or ow < 1 or oh * ow >= 2**31:
+            return None
+        sizes.append((oh, ow))
+    stride = float(self.size_divisible)          # batch_images (transform.py:243-247)
+    pad_h = int(math.ceil(float(max(s[0] for s in sizes)) / stride) * stride)
+    pad_w = int(math.ceil(float(max(s[1] for s in sizes)) / stride) * stride)
+    if pad_h > _RCNN_MAX_PAD_H or pad_h * pad_w >= 2**31:
+        return None
+    return sizes, pad_h, pad_w
+
+
+def rcnn_batch_images_op(images, out_sizes, pad_h: int, pad_w: int, mean, std) -> Tensor:
+    _lib.load_ops()
+    return torch.ops.vision_b200.rcnn_batch_images(list(images), [s[0] for s in out_sizes], [s[1] for s in out_sizes], pad_h, pad_w,
+                                                   list(mean), list(std))
+
+
+def rcnn_transform_forward(self, images, targets=None, _orig=None):
+    """GeneralizedRCNNTransform.forward in eval mode as one fused call: the same ImageList (padded batch and image_sizes as
+    tuples of Python ints) and targets None.  Training, targets and inputs the kernel does not cover run the reference."""
+    from torchvision.models.detection.image_list import ImageList
+
+    imgs = [img for img in images] if isinstance(images, (list, tuple, Tensor)) else None
+    plan = _rcnn_batch_plan(self, imgs) if targets is None and imgs is not None else None
+    if plan is None:
+        return _orig(self, images, targets)
+    sizes, pad_h, pad_w = plan
+    # mean and std exactly as normalize's torch.as_tensor(list, dtype=dtype) rounds them (transform.py:167-168)
+    mean = torch.as_tensor(self.image_mean, dtype=imgs[0].dtype).tolist()
+    std = torch.as_tensor(self.image_std, dtype=imgs[0].dtype).tolist()
+    batched = rcnn_batch_images_op(imgs, sizes, pad_h, pad_w, mean, std)
+    return ImageList(batched, [(int(h), int(w)) for h, w in sizes]), None
+
+
+def _rcnn_ratios(new_size, original_size):
+    """resize_boxes / resize_keypoints' ratios (transform.py:289-294, 307-312): fp32 new / original, (height, width)."""
+    q = np.float32(new_size) / np.float32(original_size) if all(o != 0 for o in original_size) else None
+    return None if q is None else (float(q[0]), float(q[1]))
+
+
+def rcnn_rescale_op(inputs, ratio_w, ratio_h):
+    _lib.load_ops()
+    return torch.ops.vision_b200.rcnn_rescale(list(inputs), list(ratio_w), list(ratio_h))
+
+
+def rcnn_transform_postprocess(self, result, image_shapes, original_image_sizes, _orig=None):
+    """GeneralizedRCNNTransform.postprocess in eval mode with every image's boxes and keypoints rescaled by one fused call;
+    masks are pasted by the reference's paste_masks_in_image with the rescaled boxes.  Same dicts, updated in place."""
+    from torchvision.models.detection import transform as tv_transform
+
+    if self.training or _traced() or not isinstance(result, (list, tuple)):
+        return _orig(self, result, image_shapes, original_image_sizes)
+    triples = list(zip(result, image_shapes, original_image_sizes))
+    inputs, rw, rh, slots = [], [], [], []
+    for i, (pred, im_s, o_im_s) in enumerate(triples):
+        boxes = pred.get("boxes") if isinstance(pred, dict) else None
+        ratios = _rcnn_ratios(o_im_s, im_s) if len(im_s) == 2 and len(o_im_s) == 2 else None
+        if not (isinstance(boxes, Tensor) and boxes.is_cuda and boxes.dtype == torch.float32 and boxes.dim() == 2
+                and boxes.shape[1] == 4 and ratios is not None):
+            return _orig(self, result, image_shapes, original_image_sizes)
+        named = [("boxes", boxes)]
+        if "keypoints" in pred:
+            kp = pred["keypoints"]
+            if not (isinstance(kp, Tensor) and kp.is_cuda and kp.dtype == torch.float32 and kp.dim() == 3 and kp.shape[2] == 3):
+                return _orig(self, result, image_shapes, original_image_sizes)
+            named.append(("keypoints", kp))
+        for key, t in named:
+            if t.device != boxes.device or (inputs and t.device != inputs[0].device):
+                return _orig(self, result, image_shapes, original_image_sizes)
+            inputs.append(t)
+            rh.append(ratios[0])
+            rw.append(ratios[1])
+            slots.append((i, key))
+    if not inputs:
+        return result
+    outs = rcnn_rescale_op(inputs, rw, rh)
+    for (i, key), out in zip(slots, outs):
+        result[i][key] = out
+    for i, (pred, im_s, o_im_s) in enumerate(triples):
+        if "masks" in pred:
+            result[i]["masks"] = tv_transform.paste_masks_in_image(pred["masks"], result[i]["boxes"], o_im_s)
+    return result
