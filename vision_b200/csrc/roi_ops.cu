@@ -372,6 +372,10 @@ __device__ __forceinline__ uint4 lds_u128(uint32_t addr) {
 // multicast address `mc` (multimem.st: the switch replicates the store to every rank, the local one included).
 struct PeerDst { float* dst[7]; float* mc; int n; };
 
+// Which of those destinations the line kernel stores to, fixed at compile time so the single-GPU kernel carries no
+// per-item destination tests and no PeerDst array: `output` alone, `output` plus the pd.n peer copies, or pd.mc alone.
+enum LineDst { kLineLocal = 0, kLinePeers = 1, kLineMulticast = 2 };
+
 constexpr int kLineThreads = 1024;
 constexpr int kLineStageBytes = (kLineThreads / 32) * 2 * 128;   // per warp: two 128-byte slots (loop entries + header)
 
@@ -380,7 +384,7 @@ __host__ __device__ inline size_t line_plane_bytes(int H, int pitch) { return ((
 // MULTI: fused MultiScaleRoIAlign - the work list runs over the planes of ALL feature levels (each level has its own
 // H, W, pitch and RoI bucket, filled by the geometry kernel's device-side LevelMapper); outputs are addressed by RoI id,
 // so there is no per-level gather / scatter / zero-fill pass.
-template <int P, int SR, bool MULTI>
+template <int P, int SR, bool MULTI, int DST>
 __global__ void __launch_bounds__(kLineThreads, 1)
 roi_align_line_kernel(const float* __restrict__ input, const LineTab* __restrict__ tab, float* __restrict__ output,
                       int B, int C, int H, int W, int K, int pitch, LevelSet L, const int* __restrict__ lvl_count,
@@ -391,7 +395,10 @@ roi_align_line_kernel(const float* __restrict__ input, const LineTab* __restrict
   float* plane = reinterpret_cast<float*>(smem_raw);
   const uint32_t plane_s = smem_u32(plane);
 
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, NW = blockDim.x >> 5;
+  // blockDim.x == kLineThreads.  The warp index is read through a shuffle from lane 0 so that the compiler knows it is
+  // warp-uniform: the item loop's trip count then is too, and its __syncwarp / shuffles need no divergence checks.
+  constexpr int NW = kLineThreads / 32;
+  const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
   // the per-warp staging slots sit behind the LARGEST plane of the call
   int Hmax = H, pmax = pitch;
   if (MULTI) {
@@ -401,14 +408,22 @@ roi_align_line_kernel(const float* __restrict__ input, const LineTab* __restrict
       if (bts > best) { best = bts; Hmax = L.lv[l].H; pmax = L.lv[l].pitch; }
     }
   }
+  // this warp's two 128-byte staging slots; `slot` is the current one, slot ^ slot_x the other
   const uint32_t stage_s = plane_s + (uint32_t)line_plane_bytes(Hmax, pmax) + (uint32_t)warp * 256u;
+  const uint32_t slot_x = stage_s ^ (stage_s + 128u);
+  const uint32_t lane4 = __shfl_sync(0xffffffffu, (uint32_t)lane * 4u, lane);   // opaque for the same reason as lane_code
+  const bool multi_batch = B > 1;
 
   const int q = lane & 3, grp = lane >> 2;
   const bool hi = (q & 2) != 0, lo = (q & 1) != 0;
   const float inv_count = 1.0f / (float)(SR * SR);
   // output offsets of this lane's two finished bins (loop-axis bins 2q, 2q+1 of lane group grp)
-  const int off_x = 2 * q * P + grp, off_y = 2 * q + grp * P;       // lane axis x: bin = k * P + grp; y: the transpose
+  const uint32_t off_x = 2 * q * P + grp, off_y = 2 * q + grp * P;   // lane axis x: bin = k * P + grp; y: the transpose
   const bool st0 = grp < P && 2 * q < P, st1 = grp < P && 2 * q + 1 < P;
+  // ... packed into one register, which the item loop keeps instead of re-deriving them from the lane index per item:
+  // byte 0 / 1 = the first bin's offset with the lanes along x / y, bit 16 / 17 = the lane stores its first / second bin
+  // (passed through an identity shuffle: otherwise the compiler re-derives it from threadIdx.x in every item)
+  const uint32_t lane_code = __shfl_sync(0xffffffffu, off_x | off_y << 8 | (uint32_t)st0 << 16 | (uint32_t)st1 << 17, lane);
 
   // Work is split evenly in COST units.  Single level: cost = (plane, RoI) pairs.  MULTI: a plane of level l costs
   // K_l + O_l, O_l = the fixed price of switching to it (two barriers, the load latency, its bytes) expressed in pairs -
@@ -455,7 +470,8 @@ roi_align_line_kernel(const float* __restrict__ input, const LineTab* __restrict
     const int r1 = min(Kc, f + span - ovh);
     const int b = pl / C;
     if (r1 <= r0) { w += span; continue; }          // this CTA's share of the plane is switch cost only
-    const int64_t ostep = (int64_t)NW * C * NB;
+    // output element offsets fit 32 bits: the launchers require K * C * P * P < 2^31
+    const uint32_t ostep = (uint32_t)(NW * C * NB), oplane = (uint32_t)((pl - b * C) * NB);
     __syncthreads();                           // everyone is done with the previous plane
     if (H != cur_H || pitch != cur_pitch) {    // (re)zero the pads: columns [W, pitch) of every row and the two zero rows
       for (int r = warp; r < H; r += NW)
@@ -478,36 +494,38 @@ roi_align_line_kernel(const float* __restrict__ input, const LineTab* __restrict
     int n = r0 + warp;
     int id = 0, id_next = 0;
     uint2 le = make_uint2(0u, 0u);
-    uint32_t slot = 0;
+    uint32_t slot = stage_s;
     if (n < r1) {
       id = MULTI ? __ldg(ids + n) : n;
       if (n + NW < r1) id_next = MULTI ? __ldg(ids + n + NW) : n + NW;
       le = __ldg(&tab[id].lane[lane]);
-      if (lane < 8) cp_async16(stage_s + lane * 16u, reinterpret_cast<const uint4*>(tab + id) + 16 + lane);
+      cp_async4(slot + lane4, reinterpret_cast<const float*>(tab + id) + 64 + lane);
     }
     asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 1;" ::: "memory");   // the plane has landed
     __syncthreads();
 
-    float* __restrict__ outp_lin = output + ((int64_t)n * C + (pl - b * C)) * NB;   // single level: RoI id == n, rows advance by a fixed step
-    for (; n < r1; n += NW, outp_lin += ostep) {
+    uint32_t o_lin = (uint32_t)n * (uint32_t)(C * NB) + oplane;   // single level: RoI id == n, rows advance by a fixed step
+    const char* __restrict__ tab_lin = reinterpret_cast<const char*>(tab + (n + NW));   // ... and so does the next RoI's table
+    for (; n < r1; n += NW, o_lin += ostep, tab_lin += NW * sizeof(LineTab)) {
       const int nn = n + NW;
+      const uint32_t slot_next = slot ^ slot_x;
       uint2 le_next = make_uint2(0u, 0u);
       int id_next2 = 0;
       __syncwarp();
       if (nn < r1) {
         if (MULTI && nn + NW < r1) id_next2 = __ldg(ids + nn + NW);
-        const int idn = MULTI ? id_next : nn;
-        le_next = __ldg(&tab[idn].lane[lane]);
-        if (lane < 8) cp_async16(stage_s + (slot ^ 128u) + lane * 16u, reinterpret_cast<const uint4*>(tab + idn) + 16 + lane);
+        const char* __restrict__ tn = MULTI ? reinterpret_cast<const char*>(tab + id_next) : tab_lin;
+        le_next = __ldg(reinterpret_cast<const uint2*>(tn + 2 * lane4));                          // lane[lane]
+        cp_async4(slot_next + lane4, reinterpret_cast<const float*>(tn + offsetof(LineTab, loop) + lane4));
       }
       asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 1;" ::: "memory");
       __syncwarp();
-      const uint32_t st = stage_s + slot;
+      const uint32_t st = slot;
       const bool lane_is_y = (le.x & 1u) != 0;             // bit 0 of every lane offset carries the lane axis
-      bool mine = true;
-      if (B > 1) mine = (int)lds_u32(st + 116u) == b;      // header word 1: the RoI's batch index
-      if (mine) {
-        float* __restrict__ outp = MULTI ? output + ((int64_t)id * C + (pl - b * C)) * NB : outp_lin;
+      // header word 1: the RoI's batch index (the same word in every lane, taken from lane 0 as above)
+      const bool skip = multi_batch && __shfl_sync(0xffffffffu, (int)lds_u32(st + 116u), 0) != b;
+      if (!skip) {
+        const uint32_t obase = MULTI ? (uint32_t)id * (uint32_t)(C * NB) + oplane : o_lin;
         const uint32_t base0 = plane_s + (le.x & ~3u);
         const uint32_t base1 = base0 + (lane_is_y ? 4u : (uint32_t)pitch * 4u);
         const float wl_ = __uint_as_float(le.y);
@@ -535,22 +553,26 @@ roi_align_line_kernel(const float* __restrict__ input, const LineTab* __restrict
           const float send = lo ? r4[m] : r4[2 + m], keep = lo ? r4[2 + m] : r4[m];
           s2[m] = keep + __shfl_xor_sync(0xffffffffu, send, 1);
         }
-        float* __restrict__ o = outp + (lane_is_y ? off_y : off_x);
-        float* __restrict__ o1 = o + (lane_is_y ? 1 : P);
+        const uint32_t o0 = obase + __byte_perm(lane_code, 0u, 0x4440u | (le.x & 1u));   // byte 0 (x) or 1 (y)
+        const uint32_t o1 = o0 + (lane_is_y ? 1u : (uint32_t)P);
+        const bool st0 = (lane_code & 0x10000u) != 0, st1 = (lane_code & 0x20000u) != 0;
         const float v0 = s2[0] * inv_count, v1 = s2[1] * inv_count;
-        if (pd.mc != nullptr) {              // one store each, replicated by the switch into every rank's buffer
-          if (st0) asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(pd.mc + (o - output)), "f"(v0) : "memory");
-          if (st1) asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(pd.mc + (o1 - output)), "f"(v1) : "memory");
+        if (DST == kLineMulticast) {         // one store each, replicated by the switch into every rank's buffer
+          if (st0) asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(pd.mc + o0), "f"(v0) : "memory");
+          if (st1) asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(pd.mc + o1), "f"(v1) : "memory");
         } else {
-          if (st0) o[0] = v0;
-          if (st1) o1[0] = v1;
-          for (int d = 0; d < pd.n; ++d) {   // peer-mapped copies of the same slot (NVLink stores)
-            if (st0) pd.dst[d][o - output] = v0;
-            if (st1) pd.dst[d][o1 - output] = v1;
+          if (st0) output[o0] = v0;
+          if (st1) output[o1] = v1;
+          if (DST == kLinePeers) {
+#pragma unroll
+            for (int d = 0; d < 7; ++d) {    // peer-mapped copies of the same slot (NVLink stores)
+              if (d < pd.n && st0) pd.dst[d][o0] = v0;
+              if (d < pd.n && st1) pd.dst[d][o1] = v1;
+            }
           }
         }
       }
-      slot ^= 128u;
+      slot = slot_next;
       le = le_next;
       id = id_next;
       id_next = id_next2;
@@ -923,7 +945,12 @@ static int roi_align_forward_impl(const void* input, const void* rois, void* out
       if (rc) return rc;
       const int64_t pairs = (int64_t)batch * channels * num_rois;
       const int grid = (int)(pairs < sm_count() ? pairs : sm_count());
-      VB200_CUDA_TRY(ensure_dyn_smem<roi_align_line_kernel<7, 2, false>>(smem));
+      constexpr auto local = roi_align_line_kernel<7, 2, false, kLineLocal>;
+      constexpr auto to_peers = roi_align_line_kernel<7, 2, false, kLinePeers>;
+      constexpr auto multicast = roi_align_line_kernel<7, 2, false, kLineMulticast>;
+      const auto kernel = peers.mc ? multicast : peers.n > 0 ? to_peers : local;
+      VB200_CUDA_TRY(peers.mc ? ensure_dyn_smem<multicast>(smem) : peers.n > 0 ? ensure_dyn_smem<to_peers>(smem)
+                                                                                : ensure_dyn_smem<local>(smem));
       if (peers_done) *peers_done = true;        // this kernel writes the peer destinations itself
       // programmatic dependent launch: the gather kernel zeroes its pads and stages its first plane while
       // the geometry kernel is still running, and waits (griddepcontrol.wait) before it reads the table
@@ -933,7 +960,7 @@ static int roi_align_forward_impl(const void* input, const void* rois, void* out
       attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
       attr[0].val.programmaticStreamSerializationAllowed = 1;
       cfg.attrs = attr; cfg.numAttrs = 1;
-      VB200_CUDA_TRY(cudaLaunchKernelEx(&cfg, roi_align_line_kernel<7, 2, false>, (const float*)input, (const LineTab*)tab,
+      VB200_CUDA_TRY(cudaLaunchKernelEx(&cfg, kernel, (const float*)input, (const LineTab*)tab,
                                         (float*)output, batch, channels, height, width, num_rois, pitch, none,
                                         (const int*)nullptr, (const int*)nullptr, peers));
       return check_launch("roi_align_line_kernel");
@@ -1079,8 +1106,8 @@ extern "C" int vb200_multiscale_roi_align_forward(const void* const* level_ptrs,
   if (rc) return rc;
   const int64_t pairs = (int64_t)batch * channels * num_rois;
   const int grid = (int)(pairs < sm_count() ? pairs : sm_count());
-  VB200_CUDA_TRY(ensure_dyn_smem<roi_align_line_kernel<7, 2, true>>(smem));
-  roi_align_line_kernel<7, 2, true><<<grid, kLineThreads, smem, st>>>(nullptr, ws.tab, (float*)output, batch, channels, 0, 0, num_rois, 0,
+  VB200_CUDA_TRY(ensure_dyn_smem<roi_align_line_kernel<7, 2, true, kLineLocal>>(smem));
+  roi_align_line_kernel<7, 2, true, kLineLocal><<<grid, kLineThreads, smem, st>>>(nullptr, ws.tab, (float*)output, batch, channels, 0, 0, num_rois, 0,
                                                                      L, ws.lvl_count, ws.bucket, PeerDst{});
   return check_launch("roi_align_line_kernel");
 }
