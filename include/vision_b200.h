@@ -326,6 +326,44 @@ typedef struct vb200_rcnn_rescale_item {
 } vb200_rcnn_rescale_item;
 VB200_API int vb200_rcnn_rescale(const vb200_rcnn_rescale_item* items, int num_items, vb200_stream stream);
 
+/* ---- training-target assignment (box matching) ------------------------------------------------------------------------
+ * Replaces the per-image loops of RegionProposalNetwork.assign_targets_to_anchors (torchvision/models/detection/rpn.py:193-229),
+ * RoIHeads.assign_targets_to_proposals (roi_heads.py:580-613) and the top of RetinaNet.compute_loss (retinanet.py:494-507):
+ * box_iou(gt, predictions) (ops/boxes.py:308-370), Matcher.__call__ and set_low_quality_matches_ (_utils.py:357-416) and
+ * the callers' masked writes, for all images of a call, without the M x N IoU matrix.
+ * Image i: gt [num_gt, 4] of gt_dtype and predictions [num_pred, 4] of pred_dtype (x1, y1, x2, y2; element strides
+ * (row, column)).  IoU follows box_iou op by op: fp32 for any mix of F32 / F16 / BF16 (rb - lt rounded to the dtype when
+ * both sides are F16, or both BF16), fp64 when both are F64.  Each prediction's best gt is Tensor.max(dim=0)'s (ascending gt
+ * order, ties to the lowest index, the first NaN wins); it becomes -1 below low_threshold and -2 in [low, high), compared
+ * with the threshold rounded to float (double for F64); with allow_low_quality a prediction whose IoU equals some gt's max
+ * over the image's predictions keeps its best gt.  Outputs, per mode (num_pred entries each, dense):
+ *   VB200_MATCH_RAW        out0 int64 matches (all -1 when num_gt == 0)
+ *   VB200_MATCH_RPN        out0 float labels (1 matched, 0 for -1, -1 for -2), out1 [num_pred, 4] of gt_dtype =
+ *                          gt[max(match, 0)]; when num_gt == 0 both are fp32 zeros
+ *   VB200_MATCH_ROI_HEADS  out0 int64 max(match, 0), out1 int64 gt_labels[max(match, 0)], 0 for -1, -1 for -2 (gt_labels
+ *                          int64 with element stride label_stride); when num_gt == 0 both are zeros
+ * An image with num_gt > 0 and num_pred == 0 is an error (the reference raises "No proposal boxes available").
+ * workspace: vb200_match_boxes_workspace_bytes(total gt boxes of the call, VB200_F64 when both sides are F64 else
+ * VB200_F32, allow_low_quality) bytes, a function of the shapes only (the per-gt max keys; 0 without allow_low_quality).
+ * Per VB200_MATCH_MAX_IMAGES images: two kernel launches with allow_low_quality (the gt maxima, then the matches), one
+ * without, plus one memset of the keys per call.  Asynchronous. */
+#define VB200_MATCH_MAX_IMAGES 64
+enum { VB200_MATCH_RAW = 0, VB200_MATCH_RPN = 1, VB200_MATCH_ROI_HEADS = 2 };
+typedef struct vb200_match_image {
+  const void* gt;
+  const void* pred;
+  const int64_t* gt_labels;
+  void* out0;
+  void* out1;
+  int64_t gt_stride[2], pred_stride[2], label_stride;
+  int64_t num_pred;
+  int num_gt;
+} vb200_match_image;
+VB200_API size_t vb200_match_boxes_workspace_bytes(int64_t total_gt, int dtype, int allow_low_quality);
+VB200_API int vb200_match_boxes(const vb200_match_image* images, int num_images, int gt_dtype, int pred_dtype, int mode,
+                                double high_threshold, double low_threshold, int allow_low_quality, void* workspace,
+                                size_t workspace_bytes, vb200_stream stream);
+
 /* ---- deform_conv2d -----------------------------------------------------
  * Replaces deform_conv2d_forward_kernel, csrc/ops/cuda/deform_conv2d_kernel.cu:1035-1255
  * (schema torchvision::deform_conv2d, csrc/ops/deform_conv2d.cpp:101-102).

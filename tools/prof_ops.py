@@ -6,7 +6,9 @@
                              batch 1 and 8, logits N(-4.595, 1) and N(-4.595, 0.5); select-kernel time from torch.profiler
     python tools/prof_ops.py keypoints_post [iters]     fused vs. reference keypointrcnn_inference, batch 1 and 8
     python tools/prof_ops.py rcnn_transform [iters]     fused vs. reference GeneralizedRCNNTransform forward + postprocess,
-                             batch 1 and 8, fp32 and fp16"""
+                             batch 1 and 8, fp32 and fp16
+    python tools/prof_ops.py matching [iters]     fused vs. reference training-target assignment (RPN, RoIHeads,
+                             RetinaNet), batch 2 and 8, 7 and 50 gt boxes per image"""
 import os
 import sys
 
@@ -257,6 +259,86 @@ def rcnn_transform(iters: int) -> None:
                   f"outputs identical: {same}")
 
 
+def matching(iters: int) -> None:
+    """Training-target assignment at batch 2 and 8: RegionProposalNetwork.assign_targets_to_anchors on the 217,413 RPN anchors
+    of 800 x 1088 inputs with M in {7, 50} gt boxes, RoIHeads.assign_targets_to_proposals on 2000 + M proposals and the
+    matching of RetinaNet.compute_loss on its 163,206 anchors; the fused methods against the uninstalled ones.  Wall time
+    per call ending in a synchronize (median), and whether the outputs are identical."""
+    import subprocess
+    import time
+    import types
+
+    from torchvision.models.detection import _utils as det_utils, retinanet, roi_heads, rpn
+    from torchvision.models.detection.anchor_utils import AnchorGenerator
+    from torchvision.models.detection.image_list import ImageList
+    from torchvision.ops import boxes as box_ops
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+    print(f"matching: {gpu.strip().splitlines()[0] if gpu.strip() else 'unknown GPU'}")
+
+    def anchors_for(batch, sizes, ratios, strides):
+        gen = AnchorGenerator(sizes, (ratios,) * len(sizes))
+        il = ImageList(torch.empty(batch, 3, 800, 1088, device=dev), [(800, 1088)] * batch)
+        feats = [torch.empty(batch, 1, -(-800 // s), -(-1088 // s), device=dev) for s in strides]
+        return gen(il, feats)
+
+    head = types.SimpleNamespace(compute_loss=lambda targets, outputs, anchors, matched: matched)
+    owners = {"rpn": types.SimpleNamespace(box_similarity=box_ops.box_iou, proposal_matcher=det_utils.Matcher(0.7, 0.3, True)),
+              "roi_heads": types.SimpleNamespace(proposal_matcher=det_utils.Matcher(0.5, 0.5, False)),
+              "retinanet": types.SimpleNamespace(proposal_matcher=det_utils.Matcher(0.5, 0.4, True), head=head)}
+
+    def timed(fn, n):
+        for _ in range(2):
+            fn()
+        torch.cuda.synchronize()
+        wall = []
+        for _ in range(n):
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            wall.append(time.perf_counter() - t0)
+        return sorted(wall)[n // 2] * 1e3
+
+    for batch in (2, 8):
+        rpn_anchors = anchors_for(batch, ((32,), (64,), (128,), (256,), (512,)), (0.5, 1.0, 2.0), (4, 8, 16, 32, 64))
+        ret_sizes = tuple((x, int(x * 2 ** (1.0 / 3)), int(x * 2 ** (2.0 / 3))) for x in (32, 64, 128, 256, 512))
+        ret_anchors = anchors_for(batch, ret_sizes, (0.5, 1.0, 2.0), (8, 16, 32, 64, 128))
+        for M in (7, 50):
+            gen = torch.Generator(device=dev).manual_seed(M)
+
+            def boxes(n):
+                xy = torch.rand(n, 2, generator=gen, device=dev) * torch.tensor([900.0, 650.0], device=dev)
+                return torch.cat([xy, xy + torch.rand(n, 2, generator=gen, device=dev) * 300 + 8], 1)
+
+            gts = [boxes(M) for _ in range(batch)]
+            labels = [torch.randint(1, 91, (M,), generator=gen, device=dev) for _ in range(batch)]
+            proposals = [torch.cat([boxes(2000), g]) for g in gts]
+            targets = [{"boxes": g} for g in gts]
+            calls = {
+                "rpn": lambda: rpn.RegionProposalNetwork.assign_targets_to_anchors(owners["rpn"], rpn_anchors, targets),
+                "roi_heads": lambda: roi_heads.RoIHeads.assign_targets_to_proposals(owners["roi_heads"], proposals, gts, labels),
+                "retinanet": lambda: retinanet.RetinaNet.compute_loss(owners["retinanet"], targets, {}, ret_anchors),
+            }
+            for name, fn in calls.items():
+                vb.uninstall()
+                want = fn()
+                t_ref = timed(fn, iters)
+                vb.install()
+                try:
+                    got = fn()
+                    t_ours = timed(fn, iters)
+                finally:
+                    vb.uninstall()
+                flat = lambda x: [t for part in x for t in (part if isinstance(part, (list, tuple)) else [part])]  # noqa: E731
+                same = all(a.dtype == b.dtype and torch.equal(a, b) for a, b in zip(flat(want), flat(got)))
+                n_pred = (rpn_anchors if name == "rpn" else ret_anchors if name == "retinanet" else proposals)[0].shape[0]
+                print(f"  batch {batch}, M {M}, {name} ({n_pred} predictions per image): reference {t_ref:.3f} ms, fused {t_ours:.3f} ms "
+                      f"({t_ref / t_ours:.1f}x); outputs identical: {same}")
+
+
+if op == "matching":
+    matching(iters)
+    raise SystemExit(0)
 if op == "rcnn_transform":
     rcnn_transform(iters)
     raise SystemExit(0)

@@ -1,5 +1,6 @@
 """One small call of every kernel path, meant to run under compute-sanitizer (memcheck / racecheck):
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py
+    compute-sanitizer --tool memcheck python tools/sanitize_smoke.py matching     (the box-matching kernels: memcheck only)
 No numerics are checked here (tests/ does that); the point is out-of-bounds / hazard reports."""
 import os
 import sys
@@ -130,7 +131,28 @@ def gather():
     torch.ops.vision_b200.deform_conv2d_gather(xi, w, off, m, bias, [t.data_ptr() for t in d], 1, 1, 1, 1, 1, 1, 1, 1, True)
 
 
-for name, fn in (("roi", roi), ("bwd", bwd), ("nms", nms), ("resize", resize), ("dcn", dcn), ("gather", gather)):
+def matching():
+    """the box-matching kernels, memcheck only: every mode, a background image, a gt count past one shared-memory chunk, a
+    partial last tile, fp16 / fp64 inputs and strided (non-contiguous) boxes"""
+    from torchvision.models.detection import _utils as det_utils
+
+    from vision_b200 import detection as det
+
+    def boxes(n, dt=torch.float32):
+        xy = torch.rand(n, 2, device=dev) * 500
+        return torch.cat([xy, xy + torch.rand(n, 2, device=dev) * 100], 1).to(dt)
+
+    gts = [boxes(300), torch.zeros(0, 4, device=dev), boxes(3)]
+    preds = [boxes(1500), boxes(77), boxes(2049).t().contiguous().t()]
+    labels = [torch.randint(1, 9, (g.shape[0],), device=dev) for g in gts]
+    for mode, matcher in ((det.MATCH_RAW, det_utils.Matcher(0.5, 0.4, True)), (det.MATCH_RPN, det_utils.Matcher(0.7, 0.3, True)),
+                          (det.MATCH_ROI_HEADS, det_utils.Matcher(0.5, 0.5, False))):
+        det.match_boxes_op(gts, preds, labels if mode == det.MATCH_ROI_HEADS else None, matcher, mode)
+    det.match_boxes_op([g.half() for g in gts], [p.half() for p in preds], None, det_utils.Matcher(0.7, 0.3, True), det.MATCH_RPN)
+    det.match_boxes_op([g.double() for g in gts], [p.double() for p in preds], None, det_utils.Matcher(0.7, 0.3, True), det.MATCH_RPN)
+
+
+for name, fn in (("roi", roi), ("bwd", bwd), ("nms", nms), ("resize", resize), ("dcn", dcn), ("gather", gather), ("matching", matching)):
     if only in ("all", name):
         fn()
         torch.cuda.synchronize()

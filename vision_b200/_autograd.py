@@ -177,6 +177,15 @@ def register() -> None:
     def _(images, out_h, out_w, pad_h, pad_w, mean, std):
         return images[0].new_empty((len(images), images[0].shape[0], pad_h, pad_w))
 
+    @lib.register_fake("vision_b200::match_boxes")
+    def _(gt_boxes, predictions, gt_labels, high_threshold, low_threshold, allow_low_quality_matches, mode):
+        n = [p.shape[0] for p in predictions]
+        if mode == 1:          # VB200_MATCH_RPN: fp32 labels, matched boxes of the gt dtype (fp32 zeros without gt)
+            return ([p.new_empty((k,), dtype=torch.float32) for p, k in zip(predictions, n)],
+                    [p.new_empty((k, 4), dtype=g.dtype if g.numel() else torch.float32) for p, g, k in zip(predictions, gt_boxes, n)])
+        out0 = [p.new_empty((k,), dtype=torch.int64) for p, k in zip(predictions, n)]
+        return out0, ([p.new_empty((k,), dtype=torch.int64) for p, k in zip(predictions, n)] if mode == 2 else [])
+
     # ---- deform_conv2d ----
     def dcn_setup(ctx, inputs, output):
         inp, weight, offset, mask, bias = inputs[:5]

@@ -18,6 +18,8 @@
    ``GeneralizedRCNNTransform.forward`` and ``.postprocess``, which every detection model enters and leaves through, are
    rebound on the class: normalize, resize and padding of all images in one call, the rescaling of every image's boxes and
    keypoints in another.
+   Training targets: ``RegionProposalNetwork.assign_targets_to_anchors``, ``RoIHeads.assign_targets_to_proposals`` and
+   ``RetinaNet.compute_loss`` are rebound on their classes; the per-image box_iou + Matcher loop becomes one call.
 5. ``resize`` has no torchvision kernel (transforms/v2/functional/_geometry.py:283-362 calls
    F.interpolate): the entries of ``_KERNEL_REGISTRY[resize]`` for Tensor / Image / Video are swapped.
 CPU tensors and unsupported dtypes/modes keep flowing to the reference implementation.
@@ -132,6 +134,22 @@ def install() -> None:
     tv_roi_heads.keypointrcnn_inference = keypointrcnn_inference
     tv_roi_heads.heatmaps_to_keypoints = heatmaps_to_keypoints
 
+    # ---- training-target assignment (rpn.py:193-229, roi_heads.py:580-613, retinanet.py:494-507): bound on the classes ----
+    from torchvision.models.detection import retinanet as tv_retinanet
+
+    matching = {}
+    for cls, name, body in ((tv_rpn.RegionProposalNetwork, "assign_targets_to_anchors", _det.rpn_assign_targets_to_anchors),
+                            (tv_roi_heads.RoIHeads, "assign_targets_to_proposals", _det.roi_heads_assign_targets_to_proposals),
+                            (tv_retinanet.RetinaNet, "compute_loss", _det.retinanet_compute_loss)):
+        orig = getattr(cls, name)
+
+        def fused(self, *args, _body=body, _orig=orig, **kwargs):
+            return _body(self, *args, _orig=_orig, **kwargs)
+
+        functools.update_wrapper(fused, orig)
+        matching[(cls, name)] = orig
+        setattr(cls, name, fused)
+
     # ---- detection model inputs and outputs (transform.py:119-158, 257-277): bound on the class, so every model's
     # self.transform (Faster / Mask / Keypoint R-CNN, RetinaNet, FCOS, SSD, SSDLite) picks them up ----
     from torchvision.models.detection import transform as tv_transform
@@ -199,7 +217,7 @@ def install() -> None:
                        registry=registry, saved_registry=saved, tv_poolers=tv_poolers, orig_msra=orig_msra,
                        tv_roi_align_mod=tv_roi_align_mod, orig_det_roi_align=orig_det_roi_align,
                        tv_roi_heads=tv_roi_heads, tv_rpn=tv_rpn, orig_pp=orig_pp, orig_fp=orig_fp, orig_kri=orig_kri, orig_h2k=orig_h2k,
-                       tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage,
+                       tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage, matching=matching,
                        rcnn_transform=rcnn_transform, orig_tf_forward=orig_tf_forward, orig_tf_post=orig_tf_post))
 
 
@@ -220,6 +238,8 @@ def uninstall() -> None:
     _state["rcnn_transform"].postprocess = _state["orig_tf_post"]
     for cls, orig in _state["single_stage"].items():
         cls.postprocess_detections = orig
+    for (cls, name), orig in _state["matching"].items():
+        setattr(cls, name, orig)
     reg = _state["registry"]
     reg.clear()
     reg.update(_state["saved_registry"])

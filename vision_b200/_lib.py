@@ -44,7 +44,8 @@ def core() -> ctypes.CDLL:
                          "vb200_roi_backward_workspace_bytes", "vb200_multiscale_roi_align_workspace_bytes",
                          "vb200_detection_postprocess_workspace_bytes", "vb200_deform_conv2d_packed_weight_bytes",
                          "vb200_single_stage_postprocess_workspace_bytes",
-                         "vb200_deform_conv2d_backward_inputs_workspace_bytes", "vb200_heatmaps_to_keypoints_workspace_bytes"):
+                         "vb200_deform_conv2d_backward_inputs_workspace_bytes", "vb200_heatmaps_to_keypoints_workspace_bytes",
+                         "vb200_match_boxes_workspace_bytes"):
                 getattr(lib, name).restype = ctypes.c_size_t
             _core = lib
         return _core
@@ -83,5 +84,5 @@ ABI_SYMBOLS = (
     "vb200_deform_conv2d_backward_inputs_workspace_bytes", "vb200_deform_conv2d_backward_inputs_ex",
     "vb200_ps_roi_pool_backward_ex", "vb200_roi_backward_deterministic_supported",
     "vb200_heatmaps_to_keypoints_workspace_bytes", "vb200_heatmaps_to_keypoints",
-    "vb200_rcnn_batch_images", "vb200_rcnn_rescale",
+    "vb200_rcnn_batch_images", "vb200_rcnn_rescale", "vb200_match_boxes_workspace_bytes", "vb200_match_boxes",
 )

@@ -20,7 +20,7 @@ OBJDIR = os.path.join(HERE, "build")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 CU_SOURCES = ["runtime.cu", "box_iou_rotated.cu", "roi_ops.cu", "roi_backward.cu", "nms.cu", "resize.cu", "resize_stream.cu", "deform_conv2d.cu", "deform_conv2d_bwd.cu",
-              "deform_conv2d_tc.cu", "keypoints.cu", "rcnn_transform.cu"]
+              "deform_conv2d_tc.cu", "keypoints.cu", "rcnn_transform.cu", "matching.cu"]
 CORE_LIB = os.path.join(LIBDIR, "libvision_b200.so")
 SHIM_LIB = os.path.join(LIBDIR, "libvision_b200_torch.so")
 

@@ -880,6 +880,82 @@ std::vector<at::Tensor> rcnn_rescale(at::TensorList inputs, at::ArrayRef<double>
   return outs;
 }
 
+// ---- training-target assignment (rpn.py:193-229, roi_heads.py:580-613, retinanet.py:494-507) -------------------------
+// gt_boxes / predictions: one [M_i, 4] / [N_i, 4] tensor per image on one GPU (a gt with no elements is a background image);
+// every gt that has elements shares one dtype, every prediction another.  gt_labels: one int64 [M_i] per image for mode
+// VB200_MATCH_ROI_HEADS, else empty.  Returns per-image (matches) for VB200_MATCH_RAW with an empty second list,
+// (labels, matched gt boxes) for VB200_MATCH_RPN and (clamped matches, labels) for VB200_MATCH_ROI_HEADS.
+std::tuple<std::vector<at::Tensor>, std::vector<at::Tensor>> match_boxes(at::TensorList gt_boxes, at::TensorList predictions,
+                                                                         at::TensorList gt_labels, double high_threshold,
+                                                                         double low_threshold, bool allow_low_quality_matches,
+                                                                         int64_t mode) {
+  const size_t B = predictions.size();
+  TORCH_CHECK(B >= 1 && gt_boxes.size() == B, "match_boxes: one gt tensor per prediction tensor");
+  TORCH_CHECK(mode == VB200_MATCH_RAW || mode == VB200_MATCH_RPN || mode == VB200_MATCH_ROI_HEADS, "match_boxes: unknown mode ", mode);
+  const bool roi = mode == VB200_MATCH_ROI_HEADS;
+  TORCH_CHECK(gt_labels.size() == (roi ? B : 0), "match_boxes: gt labels are taken with mode ", VB200_MATCH_ROI_HEADS, " only, one per image");
+  const at::Tensor& p0 = predictions[0];
+  TORCH_CHECK(p0.is_cuda(), "match_boxes: predictions must be CUDA tensors");
+  const auto pdt = p0.scalar_type();
+  c10::optional<at::ScalarType> gdt;
+  std::vector<vb200_match_image> desc(B);
+  for (size_t i = 0; i < B; ++i) {
+    const at::Tensor &g = gt_boxes[i], &p = predictions[i];
+    TORCH_CHECK(p.is_cuda() && p.get_device() == p0.get_device() && p.scalar_type() == pdt && p.dim() == 2 && p.size(1) == 4,
+                "match_boxes: predictions must be [N, 4] tensors of one dtype on one GPU");
+    TORCH_CHECK(p.size(0) < ((int64_t)1 << 31), "match_boxes: 2^31 or more predictions in one image");
+    vb200_match_image& d = desc[i];
+    d = {};
+    d.pred = p.data_ptr();
+    d.pred_stride[0] = p.stride(0);
+    d.pred_stride[1] = p.stride(1);
+    d.num_pred = p.size(0);
+    if (g.numel() == 0) continue;
+    TORCH_CHECK(g.is_cuda() && g.get_device() == p0.get_device() && g.dim() == 2 && g.size(1) == 4,
+                "match_boxes: gt boxes must be [M, 4] tensors on the predictions' GPU");
+    TORCH_CHECK(!gdt || g.scalar_type() == *gdt, "match_boxes: gt boxes must share one dtype");
+    gdt = g.scalar_type();
+    TORCH_CHECK(p.size(0) > 0, "No proposal boxes available for one of the images during training");
+    TORCH_CHECK(g.size(0) < ((int64_t)1 << 31), "match_boxes: 2^31 or more gt boxes in one image");
+    d.gt = g.data_ptr();
+    d.gt_stride[0] = g.stride(0);
+    d.gt_stride[1] = g.stride(1);
+    d.num_gt = (int)g.size(0);
+    if (roi) {
+      const at::Tensor& l = gt_labels[i];
+      TORCH_CHECK(l.is_cuda() && l.get_device() == p0.get_device() && l.scalar_type() == at::kLong && l.dim() == 1 && l.size(0) == g.size(0),
+                  "match_boxes: gt labels must be int64 [M] tensors on the predictions' GPU");
+      d.gt_labels = l.data_ptr<int64_t>();
+      d.label_stride = l.stride(0);
+    }
+  }
+  at::cuda::CUDAGuard guard(p0.device());
+  std::vector<at::Tensor> out0, out1;
+  for (size_t i = 0; i < B; ++i) {
+    const int64_t N = desc[i].num_pred;
+    const bool bg = desc[i].num_gt == 0;
+    if (mode == VB200_MATCH_RPN) {
+      out0.push_back(at::empty({N}, p0.options().dtype(at::kFloat)));
+      out1.push_back(at::empty({N, 4}, p0.options().dtype(bg ? at::kFloat : *gdt)));
+    } else {
+      out0.push_back(at::empty({N}, p0.options().dtype(at::kLong)));
+      if (roi) out1.push_back(at::empty({N}, p0.options().dtype(at::kLong)));
+    }
+    desc[i].out0 = out0.back().data_ptr();
+    desc[i].out1 = mode == VB200_MATCH_RAW ? nullptr : out1.back().data_ptr();
+  }
+  const int gdc = dtype_code(gdt ? *gdt : pdt, "match_boxes"), pdc = dtype_code(pdt, "match_boxes");
+  int64_t total_gt = 0;
+  for (const auto& d : desc) total_gt += d.num_gt;
+  const size_t wsb = vb200_match_boxes_workspace_bytes(total_gt, gdc == VB200_F64 && pdc == VB200_F64 ? VB200_F64 : VB200_F32,
+                                                       allow_low_quality_matches);
+  at::Tensor ws = workspace(wsb, p0);
+  check_rc(vb200_match_boxes(desc.data(), (int)B, gdc, pdc, (int)mode, high_threshold, low_threshold, allow_low_quality_matches ? 1 : 0,
+                             ws.data_ptr(), wsb, cur_stream()),
+           "match_boxes");
+  return std::make_tuple(out0, out1);
+}
+
 // ---- box_iou_rotated (csrc/ops/box_iou_rotated.cpp; checks as cuda/box_iou_rotated_kernel.cu:92-118) ----------------
 at::Tensor box_iou_rotated(const at::Tensor& boxes1, const at::Tensor& boxes2) {
   TORCH_CHECK(boxes1.is_cuda() && boxes2.is_cuda(), "boxes1 and boxes2 must be CUDA tensors");
@@ -948,6 +1024,7 @@ TORCH_LIBRARY(vision_b200, m) {
   m.def("heatmaps_to_keypoints(Tensor maps, Tensor rois) -> (Tensor, Tensor)");
   m.def("rcnn_batch_images(Tensor[] images, int[] out_h, int[] out_w, int pad_h, int pad_w, float[] mean, float[] std) -> Tensor");
   m.def("rcnn_rescale(Tensor[] inputs, float[] ratio_w, float[] ratio_h) -> Tensor[]");
+  m.def("match_boxes(Tensor[] gt_boxes, Tensor[] predictions, Tensor[] gt_labels, float high_threshold, float low_threshold, bool allow_low_quality_matches, int mode) -> (Tensor[], Tensor[])");
   m.def("multiscale_roi_align(Tensor[] features, Tensor rois, float[] scales, int pooled_height, int pooled_width, int sampling_ratio, int k_min, int k_max, float canonical_scale, float canonical_level, float eps) -> (Tensor, Tensor)");
   m.def("_roi_align_backward(Tensor grad, Tensor rois, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width, int sampling_ratio, bool aligned) -> Tensor");
   m.def("_roi_pool_backward(Tensor grad, Tensor rois, Tensor argmax, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width) -> Tensor");
@@ -983,6 +1060,7 @@ TORCH_LIBRARY_IMPL(vision_b200, CUDA, m) {
   m.impl("heatmaps_to_keypoints", TORCH_FN(heatmaps_to_keypoints));
   m.impl("rcnn_batch_images", TORCH_FN(rcnn_batch_images));
   m.impl("rcnn_rescale", TORCH_FN(rcnn_rescale));
+  m.impl("match_boxes", TORCH_FN(match_boxes));
   m.impl("resize_crop_normalize", TORCH_FN(resize_crop_normalize));
   m.impl("box_iou_rotated", TORCH_FN(box_iou_rotated));
   m.impl("_deform_conv2d_backward", TORCH_FN(deform_conv2d_backward));

@@ -13,7 +13,11 @@ bicubic resize, argmax and coordinate arithmetic, are ONE call of ``vision_b200:
 
 ``GeneralizedRCNNTransform.forward`` (transform.py:119-158), which every detection model enters through, is ONE call of
 ``vision_b200::rcnn_batch_images`` (normalize, bilinear resize and zero padding of all images); its ``postprocess``
-(:257-277) rescales every image's boxes and keypoints with ONE call of ``vision_b200::rcnn_rescale``."""
+(:257-277) rescales every image's boxes and keypoints with ONE call of ``vision_b200::rcnn_rescale``.
+
+The training targets of ``RegionProposalNetwork.assign_targets_to_anchors`` (rpn.py:193-229),
+``RoIHeads.assign_targets_to_proposals`` (roi_heads.py:580-613) and the matching loop of ``RetinaNet.compute_loss``
+(retinanet.py:494-507), a per-image box_iou + Matcher, are ONE call of ``vision_b200::match_boxes`` for all images."""
 from __future__ import annotations
 
 import math
@@ -345,3 +349,77 @@ def rcnn_transform_postprocess(self, result, image_shapes, original_image_sizes,
         if "masks" in pred:
             result[i]["masks"] = tv_transform.paste_masks_in_image(pred["masks"], result[i]["boxes"], o_im_s)
     return result
+
+
+MATCH_RAW, MATCH_RPN, MATCH_ROI_HEADS = 0, 1, 2          # VB200_MATCH_* in include/vision_b200.h
+_MATCH_DTYPES = (torch.float16, torch.bfloat16, torch.float32, torch.float64)
+
+
+def match_supported(matcher, gt_boxes, predictions, gt_labels=None) -> bool:
+    """Inputs the matching kernel reproduces the reference on: a plain ``det_utils.Matcher`` (not SSD's SSDMatcher or a
+    subclass) with its -1 / -2 codes, outside scripting and tracing; one [M, 4] gt (or an empty one: a background image)
+    and one [N, 4] prediction tensor per image, N below 2^31, all CUDA on one device; the gt boxes that have elements of one
+    dtype and the predictions of one dtype, both fp64 or both among fp16 / bf16 / fp32; for RoIHeads, int64 [M] labels."""
+    from torchvision.models.detection import _utils as det_utils
+
+    if (_traced() or type(matcher) is not det_utils.Matcher or matcher.BELOW_LOW_THRESHOLD != -1 or matcher.BETWEEN_THRESHOLDS != -2
+            or not isinstance(gt_boxes, (list, tuple)) or not isinstance(predictions, (list, tuple)) or not predictions
+            or len(gt_boxes) != len(predictions) or (gt_labels is not None and len(gt_labels) != len(predictions))):
+        return False
+    p0 = predictions[0]
+    if not (isinstance(p0, Tensor) and p0.is_cuda and p0.dtype in _MATCH_DTYPES):
+        return False
+    gdt = None
+    for i, (g, p) in enumerate(zip(gt_boxes, predictions)):
+        if not (isinstance(g, Tensor) and isinstance(p, Tensor) and p.is_cuda and p.device == p0.device and p.dtype == p0.dtype
+                and p.dim() == 2 and p.shape[1] == 4 and p.shape[0] < 2**31):
+            return False
+        if g.numel() == 0:
+            continue
+        if not (g.is_cuda and g.device == p0.device and g.dim() == 2 and g.shape[1] == 4 and g.dtype in _MATCH_DTYPES
+                and g.dtype == (gdt or g.dtype) and (g.dtype == torch.float64) == (p.dtype == torch.float64)):
+            return False
+        gdt = g.dtype
+        if gt_labels is not None:
+            lb = gt_labels[i]
+            if not (isinstance(lb, Tensor) and lb.is_cuda and lb.device == p0.device and lb.dtype == torch.int64
+                    and tuple(lb.shape) == (g.shape[0],)):
+                return False
+    return True
+
+
+def match_boxes_op(gt_boxes, predictions, gt_labels, matcher, mode: int):
+    """Every image's box_iou + Matcher + the caller's epilogue as one op.  An image with gt boxes and no predictions raises
+    the Matcher's error from the shapes, before anything is launched."""
+    for g, p in zip(gt_boxes, predictions):
+        if g.numel() != 0 and p.shape[0] == 0:
+            raise ValueError("No proposal boxes available for one of the images during training")
+    _lib.load_ops()
+    return torch.ops.vision_b200.match_boxes(list(gt_boxes), list(predictions), list(gt_labels or []), float(matcher.high_threshold),
+                                             float(matcher.low_threshold), bool(matcher.allow_low_quality_matches), mode)
+
+
+def rpn_assign_targets_to_anchors(self, anchors, targets, _orig=None):
+    """RegionProposalNetwork.assign_targets_to_anchors as one fused call: the same fp32 labels and matched gt boxes."""
+    from torchvision.ops import boxes as box_ops
+
+    gt_boxes = [t["boxes"] for t in targets] if isinstance(targets, (list, tuple)) else None
+    if self.box_similarity is not box_ops.box_iou or gt_boxes is None or not match_supported(self.proposal_matcher, gt_boxes, anchors):
+        return _orig(self, anchors, targets)
+    return match_boxes_op(gt_boxes, anchors, None, self.proposal_matcher, MATCH_RPN)
+
+
+def roi_heads_assign_targets_to_proposals(self, proposals, gt_boxes, gt_labels, _orig=None):
+    """RoIHeads.assign_targets_to_proposals as one fused call: the same clamped matches and int64 labels."""
+    if not match_supported(self.proposal_matcher, gt_boxes, proposals, gt_labels):
+        return _orig(self, proposals, gt_boxes, gt_labels)
+    return match_boxes_op(gt_boxes, proposals, gt_labels, self.proposal_matcher, MATCH_ROI_HEADS)
+
+
+def retinanet_compute_loss(self, targets, head_outputs, anchors, _orig=None):
+    """RetinaNet.compute_loss with its matching loop as one fused call; self.head.compute_loss is the reference's."""
+    gt_boxes = [t["boxes"] for t in targets] if isinstance(targets, (list, tuple)) else None
+    if gt_boxes is None or not match_supported(self.proposal_matcher, gt_boxes, anchors):
+        return _orig(self, targets, head_outputs, anchors)
+    matched_idxs, _ = match_boxes_op(gt_boxes, anchors, None, self.proposal_matcher, MATCH_RAW)
+    return self.head.compute_loss(targets, head_outputs, anchors, matched_idxs)
