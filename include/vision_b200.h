@@ -364,6 +364,35 @@ VB200_API int vb200_match_boxes(const vb200_match_image* images, int num_images,
                                 double high_threshold, double low_threshold, int allow_low_quality, void* workspace,
                                 size_t workspace_bytes, vb200_stream stream);
 
+/* ---- FCOS training-target assignment (centre sampling) ------------------------------------------------------------------
+ * Replaces the per-image matching loop of FCOS.compute_loss (torchvision/models/detection/fcos.py:440-487, the [N, M]
+ * tensors of :455-483) for all images of a call, without any N x M intermediate.
+ * Image i: gt [num_gt, 4] of gt_dtype and anchors [num_anchors, 4] of anchor_dtype (x1, y1, x2, y2; element strides
+ * (row, column)); out int64 [num_anchors], dense.  Per anchor, op by op as the reference: centres, sizes, radius * size and
+ * the level bounds size * 4 / size * 8 rounded to anchor_dtype, gt centres and areas rounded to gt_dtype, anchor - gt
+ * differences rounded to the promoted type (the dtype when both sides share it, fp32 for any other mix of F32 / F16 / BF16,
+ * fp64 when both are F64), scalars rounded to float unless both are F64; the strict comparisons with NaN failing them;
+ * value = (float)match * (1e8 - area) in promote(fp32, gt_dtype); the best gt as Tensor.max(dim=1) picks it (ascending gt
+ * order, ties to the lowest index, the first NaN wins), -1 where that value is below 1e-5.  An image with num_gt == 0 gets
+ * all -1.  The lower bound is 0 for the first and the upper bound inf from the last anchors that
+ * vb200_fcos_level_bounds(num_anchors, first_level, last_level) names, first_level / last_level being
+ * num_anchors_per_level[0] / [-1].  One kernel launch per VB200_MATCH_MAX_IMAGES images, no workspace.  Asynchronous. */
+typedef struct vb200_fcos_image {
+  const void* gt;
+  const void* anchors;
+  int64_t* out;
+  int64_t gt_stride[2], anchor_stride[2];
+  int64_t num_anchors;
+  int num_gt;
+} vb200_fcos_image;
+/* Python's slicing of lower_bound[:first_level] = 0 and upper_bound[-last_level:] = inf (fcos.py:472-475) over num_anchors
+ * anchors: *lower_end_host anchors from the front get lower bound 0, anchors from *upper_begin_host on get upper bound inf
+ * (a last_level of 0 makes [-0:] the whole tensor; counts beyond num_anchors clamp; negative counts index from the end). */
+VB200_API void vb200_fcos_level_bounds(int64_t num_anchors, int64_t first_level, int64_t last_level, int64_t* lower_end_host,
+                                       int64_t* upper_begin_host);
+VB200_API int vb200_fcos_match(const vb200_fcos_image* images, int num_images, int gt_dtype, int anchor_dtype, double radius,
+                               int64_t first_level, int64_t last_level, vb200_stream stream);
+
 /* ---- deform_conv2d -----------------------------------------------------
  * Replaces deform_conv2d_forward_kernel, csrc/ops/cuda/deform_conv2d_kernel.cu:1035-1255
  * (schema torchvision::deform_conv2d, csrc/ops/deform_conv2d.cpp:101-102).

@@ -8,7 +8,9 @@
     python tools/prof_ops.py rcnn_transform [iters]     fused vs. reference GeneralizedRCNNTransform forward + postprocess,
                              batch 1 and 8, fp32 and fp16
     python tools/prof_ops.py matching [iters]     fused vs. reference training-target assignment (RPN, RoIHeads,
-                             RetinaNet), batch 2 and 8, 7 and 50 gt boxes per image"""
+                             RetinaNet), batch 2 and 8, 7 and 50 gt boxes per image
+    python tools/prof_ops.py fcos [iters]     fused vs. reference FCOS.compute_loss matching, batch 2, 8 and 16, 7 and 50
+                             gt boxes per image"""
 import os
 import sys
 
@@ -336,8 +338,70 @@ def matching(iters: int) -> None:
                       f"({t_ref / t_ours:.1f}x); outputs identical: {same}")
 
 
+def fcos_matching(iters: int) -> None:
+    """FCOS.compute_loss at batch 2, 8 and 16 with M in {7, 50} gt boxes per image, on the 18,134 FCOS anchors of an 800 x 1088
+    batch, with a head whose compute_loss returns the matched indices: the fused method against the uninstalled one.  Wall
+    time per call ending in a synchronize (median), and whether the outputs are identical."""
+    import subprocess
+    import time
+    import types
+
+    from torchvision.models.detection import fcos
+    from torchvision.models.detection.anchor_utils import AnchorGenerator
+    from torchvision.models.detection.image_list import ImageList
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+    print(f"fcos: {gpu.strip().splitlines()[0] if gpu.strip() else 'unknown GPU'}")
+    owner = types.SimpleNamespace(center_sampling_radius=1.5,
+                                  head=types.SimpleNamespace(compute_loss=lambda targets, outputs, anchors, matched: matched))
+    strides = (8, 16, 32, 64, 128)
+
+    def timed(fn, n):
+        for _ in range(2):
+            fn()
+        torch.cuda.synchronize()
+        wall = []
+        for _ in range(n):
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            wall.append(time.perf_counter() - t0)
+        return sorted(wall)[n // 2] * 1e3
+
+    for batch in (2, 8, 16):
+        gen = AnchorGenerator(tuple((s,) for s in strides), ((1.0,),) * len(strides))       # FCOS's own generator
+        il = ImageList(torch.empty(batch, 3, 800, 1088, device=dev), [(800, 1088)] * batch)
+        feats = [torch.empty(batch, 1, -(-800 // s), -(-1088 // s), device=dev) for s in strides]
+        anchors = gen(il, feats)
+        levels = [f.shape[2] * f.shape[3] for f in feats]
+        for M in (7, 50):
+            g = torch.Generator(device=dev).manual_seed(M)
+
+            def boxes(n):
+                xy = torch.rand(n, 2, generator=g, device=dev) * torch.tensor([900.0, 650.0], device=dev)
+                return torch.cat([xy, xy + torch.rand(n, 2, generator=g, device=dev) * 300 + 8], 1)
+
+            targets = [{"boxes": boxes(M)} for _ in range(batch)]
+            fn = lambda: fcos.FCOS.compute_loss(owner, targets, {}, anchors, levels)  # noqa: E731
+            vb.uninstall()
+            want = fn()
+            t_ref = timed(fn, iters)
+            vb.install()
+            try:
+                got = fn()
+                t_ours = timed(fn, iters)
+            finally:
+                vb.uninstall()
+            same = all(a.dtype == b.dtype and a.stride() == b.stride() and torch.equal(a, b) for a, b in zip(want, got))
+            print(f"  batch {batch}, M {M} ({anchors[0].shape[0]} anchors per image): reference {t_ref:.3f} ms, fused {t_ours:.3f} ms "
+                  f"({t_ref / t_ours:.1f}x); outputs identical: {same}")
+
+
 if op == "matching":
     matching(iters)
+    raise SystemExit(0)
+if op == "fcos":
+    fcos_matching(iters)
     raise SystemExit(0)
 if op == "rcnn_transform":
     rcnn_transform(iters)

@@ -1,6 +1,7 @@
 """One small call of every kernel path, meant to run under compute-sanitizer (memcheck / racecheck):
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py matching     (the box-matching kernels: memcheck only)
+    compute-sanitizer --tool memcheck python tools/sanitize_smoke.py fcos         (the FCOS matching kernel: memcheck only)
 No numerics are checked here (tests/ does that); the point is out-of-bounds / hazard reports."""
 import os
 import sys
@@ -152,7 +153,25 @@ def matching():
     det.match_boxes_op([g.double() for g in gts], [p.double() for p in preds], None, det_utils.Matcher(0.7, 0.3, True), det.MATCH_RPN)
 
 
-for name, fn in (("roi", roi), ("bwd", bwd), ("nms", nms), ("resize", resize), ("dcn", dcn), ("gather", gather), ("matching", matching)):
+def fcos():
+    """the FCOS matching kernel, memcheck only: a background image, an image without anchors, a gt count past one
+    shared-memory chunk, partial last tiles, fp16 / bf16 / fp64 inputs and strided (non-contiguous) boxes"""
+    from vision_b200 import detection as det
+
+    def boxes(n, dt=torch.float32):
+        xy = torch.rand(n, 2, device=dev) * 500
+        return torch.cat([xy, xy + torch.rand(n, 2, device=dev) * 100], 1).to(dt)
+
+    gts = [boxes(300), torch.zeros(0, 4, device=dev), boxes(3), boxes(5)]
+    anchors = [boxes(1500), boxes(77), boxes(2049).t().contiguous().t(), boxes(0)]
+    levels = [1000, 400, 100]
+    det.fcos_match_op(gts, anchors, 1.5, levels)
+    det.fcos_match_op([g.half() for g in gts], [a.bfloat16() for a in anchors], 1.5, levels)
+    det.fcos_match_op([g.double() for g in gts], [a.double() for a in anchors], 2.5, [10**6, 0])
+
+
+for name, fn in (("roi", roi), ("bwd", bwd), ("nms", nms), ("resize", resize), ("dcn", dcn), ("gather", gather), ("matching", matching),
+                 ("fcos", fcos)):
     if only in ("all", name):
         fn()
         torch.cuda.synchronize()

@@ -186,6 +186,10 @@ def register() -> None:
         out0 = [p.new_empty((k,), dtype=torch.int64) for p, k in zip(predictions, n)]
         return out0, ([p.new_empty((k,), dtype=torch.int64) for p, k in zip(predictions, n)] if mode == 2 else [])
 
+    @lib.register_fake("vision_b200::fcos_match")
+    def _(gt_boxes, anchors, radius, first_level, last_level):
+        return [a.new_empty((a.shape[0],), dtype=torch.int64) for a in anchors]
+
     # ---- deform_conv2d ----
     def dcn_setup(ctx, inputs, output):
         inp, weight, offset, mask, bias = inputs[:5]

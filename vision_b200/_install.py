@@ -20,6 +20,7 @@
    keypoints in another.
    Training targets: ``RegionProposalNetwork.assign_targets_to_anchors``, ``RoIHeads.assign_targets_to_proposals`` and
    ``RetinaNet.compute_loss`` are rebound on their classes; the per-image box_iou + Matcher loop becomes one call.
+   ``FCOS.compute_loss`` likewise: its per-image centre-sampling loop becomes one call.
 5. ``resize`` has no torchvision kernel (transforms/v2/functional/_geometry.py:283-362 calls
    F.interpolate): the entries of ``_KERNEL_REGISTRY[resize]`` for Tensor / Image / Video are swapped.
 CPU tensors and unsupported dtypes/modes keep flowing to the reference implementation.
@@ -134,13 +135,15 @@ def install() -> None:
     tv_roi_heads.keypointrcnn_inference = keypointrcnn_inference
     tv_roi_heads.heatmaps_to_keypoints = heatmaps_to_keypoints
 
-    # ---- training-target assignment (rpn.py:193-229, roi_heads.py:580-613, retinanet.py:494-507): bound on the classes ----
-    from torchvision.models.detection import retinanet as tv_retinanet
+    # ---- training-target assignment (rpn.py:193-229, roi_heads.py:580-613, retinanet.py:494-507, fcos.py:440-487): bound on
+    # the classes ----
+    from torchvision.models.detection import fcos as tv_fcos, retinanet as tv_retinanet
 
     matching = {}
     for cls, name, body in ((tv_rpn.RegionProposalNetwork, "assign_targets_to_anchors", _det.rpn_assign_targets_to_anchors),
                             (tv_roi_heads.RoIHeads, "assign_targets_to_proposals", _det.roi_heads_assign_targets_to_proposals),
-                            (tv_retinanet.RetinaNet, "compute_loss", _det.retinanet_compute_loss)):
+                            (tv_retinanet.RetinaNet, "compute_loss", _det.retinanet_compute_loss),
+                            (tv_fcos.FCOS, "compute_loss", _det.fcos_compute_loss)):
         orig = getattr(cls, name)
 
         def fused(self, *args, _body=body, _orig=orig, **kwargs):

@@ -85,4 +85,5 @@ ABI_SYMBOLS = (
     "vb200_ps_roi_pool_backward_ex", "vb200_roi_backward_deterministic_supported",
     "vb200_heatmaps_to_keypoints_workspace_bytes", "vb200_heatmaps_to_keypoints",
     "vb200_rcnn_batch_images", "vb200_rcnn_rescale", "vb200_match_boxes_workspace_bytes", "vb200_match_boxes",
+    "vb200_fcos_level_bounds", "vb200_fcos_match",
 )

@@ -10,6 +10,8 @@
 //            CTA and gt.  Max is order-independent, so the keys are the same whatever the schedule.
 //   final    every IoU again (the same function, so the same bits): each prediction's best gt as Tensor.max(dim=0) picks it,
 //            the thresholds, the low-quality rule against the pass-1 maxima, and the caller's epilogue.
+// FCOS's centre-sampling matcher (fcos.py:440-487) is a different algorithm on the same layout: one pass, each anchor's
+// best gt found while scanning the gt boxes, no N x M tensor (fcos_match_kernel below).
 // The per-image descriptors travel as a __grid_constant__ kernel parameter.
 #include <vector>
 
@@ -69,14 +71,20 @@ template <typename A> __device__ __forceinline__ A nan_min(A a, A b) { return a 
 // clamp(min=0), which keeps a NaN
 template <typename A> __device__ __forceinline__ A clamp0(A v) { return v < A(0) ? A(0) : v; }
 
+// A value computed in fp32 (as ATen computes fp16 / bf16 ops) and stored in a tensor of type S: rounded to S.  fp32 and fp64
+// values are stored as computed.
+template <typename S> __device__ __forceinline__ float round_as(float v) { return v; }
+template <> __device__ __forceinline__ float round_as<__half>(float v) { return __half2float(__float2half_rn(v)); }
+template <> __device__ __forceinline__ float round_as<__nv_bfloat16>(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+template <typename S> __device__ __forceinline__ double round_as(double v) { return v; }
+// ... for a dtype known only at run time (one tensor of the call)
+template <typename A> __device__ __forceinline__ A round_as(A v, int dtype) {
+  return dtype == VB200_F16 ? round_as<__half>(v) : dtype == VB200_BF16 ? round_as<__nv_bfloat16>(v) : v;
+}
+
 // rb - lt: computed in the type of the operands.  When both sides are fp16 (or both bf16) lt and rb are fp16 tensors and the
 // difference is rounded to fp16 before _upcast; every other mix promotes to fp32 (or is fp64 throughout).
-template <typename S> __device__ __forceinline__ float round_sub(float a, float b) { return sub_rn(a, b); }
-template <> __device__ __forceinline__ float round_sub<__half>(float a, float b) { return __half2float(__float2half_rn(sub_rn(a, b))); }
-template <> __device__ __forceinline__ float round_sub<__nv_bfloat16>(float a, float b) {
-  return __bfloat162float(__float2bfloat16_rn(sub_rn(a, b)));
-}
-template <typename S> __device__ __forceinline__ double round_sub(double a, double b) { return sub_rn(a, b); }
+template <typename S, typename A> __device__ __forceinline__ A round_sub(A a, A b) { return round_as<S>(sub_rn(a, b)); }
 
 template <typename A> struct MBox { A x1, y1, x2, y2, area; };
 
@@ -257,6 +265,121 @@ int launch_matching(MatchPlan& plan, const vb200_match_image* images, int num_im
 
 size_t match_key_bytes(int64_t total_gt, int dtype) { return align256((size_t)total_gt * (dtype == VB200_F64 ? 8 : 4)); }
 
+// ---- FCOS centre sampling (fcos.py:455-483) ------------------------------------------------------------------------------
+// A thread holds kFcosAnchorsPerThread anchors' anchor-side values in registers and scans the image's gt boxes, staged in
+// shared memory kGtChunk at a time with their gt-side values, in ascending index order: the running best is
+// Tensor.max(dim=1)'s, so no N x M value is ever stored.
+constexpr int kFcosThreads = 256;
+constexpr int kFcosAnchorsPerThread = 2;
+constexpr int kFcosTile = kFcosThreads * kFcosAnchorsPerThread;   // anchors per CTA
+
+struct FcosPlan {
+  vb200_fcos_image img[VB200_MATCH_MAX_IMAGES];
+  int64_t lower_end[VB200_MATCH_MAX_IMAGES], upper_begin[VB200_MATCH_MAX_IMAGES];   // vb200_fcos_level_bounds of each image
+  int gt_dtype, anchor_dtype;
+  float radius_f;            // center_sampling_radius as ATen's CUDA scalar ops take it for a non-fp64 tensor
+  double radius_d;
+};
+
+// The gt side, rounded to the gt dtype: gt_centers = (gt[:, :2] + gt[:, 2:]) / 2, the boxes, and 1e8 - gt_areas.
+template <typename A> struct FcosGt { A cx, cy, x1, y1, x2, y2, term; };
+// The anchor side, rounded to the anchor dtype: anchor_centers, center_sampling_radius * anchor_sizes and the level bounds.
+template <typename A> struct FcosAnchor { A cx, cy, reach, lower, upper; };
+
+// (a + b) / 2 of two coordinates of a tensor of `dtype`: the sum rounded to it, then the division, which ATen's CUDA kernel
+// computes as a product with the scalar's reciprocal
+template <typename A> __device__ __forceinline__ A fcos_center(A a, A b, int dtype) {
+  return round_as(mul_rn(round_as(add_rn(a, b), dtype), A(0.5)), dtype);
+}
+
+// Run under S, the type anchor - gt differences are rounded to: the dtype when both sides share it, else fp32 (or fp64).
+template <typename A, typename S>
+__global__ void __launch_bounds__(kFcosThreads)
+fcos_match_kernel(const __grid_constant__ FcosPlan plan) {
+  const vb200_fcos_image& d = plan.img[blockIdx.y];
+  const int M = d.num_gt;
+  const int64_t N = d.num_anchors, base = (int64_t)blockIdx.x * kFcosTile;
+  if (base >= N) return;                              // uniform over the CTA
+  __shared__ FcosGt<A> sg[kGtChunk];
+  const int ad = plan.anchor_dtype, gd = plan.gt_dtype;
+  const A radius = sizeof(A) == 8 ? (A)plan.radius_d : (A)plan.radius_f;
+
+  FcosAnchor<A> a[kFcosAnchorsPerThread];
+  A best[kFcosAnchorsPerThread];
+  int best_idx[kFcosAnchorsPerThread];
+#pragma unroll
+  for (int k = 0; k < kFcosAnchorsPerThread; ++k) {
+    const int64_t n = base + threadIdx.x + k * kFcosThreads;
+    const MBox<A> b = n < N ? load_box<A>(d.anchors, ad, n, d.anchor_stride) : MBox<A>{};    // (.area is box_iou's, unused)
+    const A size = round_as(sub_rn(b.x2, b.x1), ad);                                           // anchor_sizes
+    a[k].cx = fcos_center(b.x1, b.x2, ad);
+    a[k].cy = fcos_center(b.y1, b.y2, ad);
+    a[k].reach = round_as(mul_rn(radius, size), ad);
+    a[k].lower = n < plan.lower_end[blockIdx.y] ? A(0) : round_as(mul_rn(size, A(4)), ad);
+    a[k].upper = n >= plan.upper_begin[blockIdx.y] ? A(INFINITY) : round_as(mul_rn(size, A(8)), ad);
+    best[k] = A(0);
+    best_idx[k] = -1;
+  }
+
+  for (int c0 = 0; c0 < M; c0 += kGtChunk) {
+    const int cnt = M - c0 < kGtChunk ? M - c0 : kGtChunk;
+    __syncthreads();                                  // the previous chunk is consumed
+    for (int j = threadIdx.x; j < cnt; j += kFcosThreads) {
+      const MBox<A> b = load_box<A>(d.gt, gd, c0 + j, d.gt_stride);
+      const A area = round_as(mul_rn(round_as(sub_rn(b.x2, b.x1), gd), round_as(sub_rn(b.y2, b.y1), gd)), gd);
+      // 1e8 - gt_areas: the scalar as a float (exact), the difference rounded to the gt dtype (inf for fp16)
+      sg[j] = FcosGt<A>{fcos_center(b.x1, b.x2, gd), fcos_center(b.y1, b.y2, gd), b.x1, b.y1, b.x2, b.y2,
+                        round_as(sub_rn(A(1e8), area), gd)};
+    }
+    __syncthreads();
+    for (int j = 0; j < cnt; ++j) {
+      const FcosGt<A> g = sg[j];
+#pragma unroll
+      for (int k = 0; k < kFcosAnchorsPerThread; ++k) {
+        // |anchor_centers - gt_centers|.max(dim=2) < radius * size; pairwise_dist's min > 0, its max in (lower, upper).
+        // max / min over the stacked dimension propagate a NaN, and every comparison with a NaN is false.
+        const A cdist = nan_max(fabs(round_sub<S>(a[k].cx, g.cx)), fabs(round_sub<S>(a[k].cy, g.cy)));
+        const A l = round_sub<S>(a[k].cx, g.x1), t = round_sub<S>(a[k].cy, g.y1);
+        const A r = round_sub<S>(g.x2, a[k].cx), btm = round_sub<S>(g.y2, a[k].cy);
+        const A dmin = nan_min(nan_min(l, t), nan_min(r, btm)), dmax = nan_max(nan_max(l, t), nan_max(r, btm));
+        const bool match = cdist < a[k].reach && dmin > A(0) && dmax > a[k].lower && dmax < a[k].upper;
+        // match.to(float32) * (1e8 - area), multiplied literally: 0 * inf is NaN, 0 * a negative term is -0
+        const A v = mul_rn(match ? A(1) : A(0), g.term);
+        // Tensor.max(dim=1): ascending gt order, strict >, the first NaN wins and stays
+        if (best_idx[k] < 0 || (best[k] == best[k] && (v != v || v > best[k]))) { best[k] = v; best_idx[k] = c0 + j; }
+      }
+    }
+  }
+
+  // matched_idx[min_values < 1e-5] = -1, the scalar rounded to the value's type; a NaN keeps its index.  An image without gt
+  // keeps best 0 and index -1.
+  const A min_value = sizeof(A) == 8 ? (A)1e-5 : (A)1e-5f;
+#pragma unroll
+  for (int k = 0; k < kFcosAnchorsPerThread; ++k) {
+    const int64_t n = base + threadIdx.x + k * kFcosThreads;
+    if (n < N) d.out[n] = best[k] < min_value ? -1 : best_idx[k];
+  }
+}
+
+template <typename A, typename S>
+int launch_fcos(FcosPlan& plan, const vb200_fcos_image* images, int num_images, int64_t first_level, int64_t last_level,
+                cudaStream_t st) {
+  for (int done = 0; done < num_images; done += VB200_MATCH_MAX_IMAGES) {
+    const int chunk = num_images - done < VB200_MATCH_MAX_IMAGES ? num_images - done : VB200_MATCH_MAX_IMAGES;
+    int64_t most = 0;
+    for (int i = 0; i < chunk; ++i) {
+      plan.img[i] = images[done + i];
+      vb200_fcos_level_bounds(images[done + i].num_anchors, first_level, last_level, &plan.lower_end[i], &plan.upper_begin[i]);
+      most = images[done + i].num_anchors > most ? images[done + i].num_anchors : most;
+    }
+    if (most == 0) continue;
+    fcos_match_kernel<A, S><<<dim3((unsigned)ceil_div64(most, kFcosTile), (unsigned)chunk), kFcosThreads, 0, st>>>(plan);
+    const int rc = check_launch("fcos_match_kernel");
+    if (rc) return rc;
+  }
+  return 0;
+}
+
 }  // namespace
 }  // namespace vb200
 
@@ -313,4 +436,44 @@ extern "C" int vb200_match_boxes(const vb200_match_image* images, int num_images
   if (gt_dtype == VB200_BF16 && pred_dtype == VB200_BF16)
     return launch_matching<float, __nv_bfloat16>(plan, images, num_images, key_offset.data(), st);
   return launch_matching<float, float>(plan, images, num_images, key_offset.data(), st);
+}
+
+extern "C" void vb200_fcos_level_bounds(int64_t num_anchors, int64_t first_level, int64_t last_level, int64_t* lower_end_host,
+                                        int64_t* upper_begin_host) {
+  // Python's slice bounds: a negative index counts from the end, then both clamp to [0, num_anchors]
+  const auto index = [num_anchors](int64_t i) {
+    if (i < 0) i += num_anchors;
+    return i < 0 ? 0 : i > num_anchors ? num_anchors : i;
+  };
+  *lower_end_host = index(first_level);     // lower_bound[:first_level]
+  *upper_begin_host = index(-last_level);   // upper_bound[-last_level:]; [-0:] starts at 0
+}
+
+extern "C" int vb200_fcos_match(const vb200_fcos_image* images, int num_images, int gt_dtype, int anchor_dtype, double radius,
+                                int64_t first_level, int64_t last_level, vb200_stream stream) {
+  VB200_REQUIRE(num_images >= 0, "fcos_match: bad image count");
+  const bool wide = gt_dtype == VB200_F64 && anchor_dtype == VB200_F64;
+  const auto narrow_float = [](int t) { return t == VB200_F32 || t == VB200_F16 || t == VB200_BF16; };
+  VB200_REQUIRE(wide || (narrow_float(gt_dtype) && narrow_float(anchor_dtype)),
+                "fcos_match: gt and anchors must both be float64, or both float32 / float16 / bfloat16 (dtypes %d, %d)", gt_dtype,
+                anchor_dtype);
+  VB200_REQUIRE(first_level > INT64_MIN && last_level > INT64_MIN, "fcos_match: bad level sizes");
+  if (num_images == 0) return 0;
+  VB200_REQUIRE(images, "fcos_match: null images");
+  for (int i = 0; i < num_images; ++i) {
+    const vb200_fcos_image& d = images[i];
+    VB200_REQUIRE(d.num_gt >= 0 && d.num_anchors >= 0 && d.num_anchors < ((int64_t)1 << 31), "fcos_match: image %d: bad sizes", i);
+    VB200_REQUIRE(d.num_anchors == 0 || (d.anchors && d.out && (d.num_gt == 0 || d.gt)), "fcos_match: image %d: null pointer", i);
+  }
+  FcosPlan plan;
+  plan.gt_dtype = gt_dtype;
+  plan.anchor_dtype = anchor_dtype;
+  plan.radius_f = (float)radius;
+  plan.radius_d = radius;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (wide) return launch_fcos<double, double>(plan, images, num_images, first_level, last_level, st);
+  if (gt_dtype == VB200_F16 && anchor_dtype == VB200_F16) return launch_fcos<float, __half>(plan, images, num_images, first_level, last_level, st);
+  if (gt_dtype == VB200_BF16 && anchor_dtype == VB200_BF16)
+    return launch_fcos<float, __nv_bfloat16>(plan, images, num_images, first_level, last_level, st);
+  return launch_fcos<float, float>(plan, images, num_images, first_level, last_level, st);
 }

@@ -956,6 +956,51 @@ std::tuple<std::vector<at::Tensor>, std::vector<at::Tensor>> match_boxes(at::Ten
   return std::make_tuple(out0, out1);
 }
 
+// ---- FCOS training-target assignment (fcos.py:440-487) -----------------------------------------------------------------
+// gt_boxes / anchors: one [M_i, 4] / [N_i, 4] tensor per image on one GPU (a gt with no elements is a background image); every
+// gt that has elements shares one dtype, every anchor tensor another.  first_level / last_level: num_anchors_per_level[0] and
+// [-1].  Returns each image's int64 [N_i] matched gt index, -1 for an unmatched anchor.
+std::vector<at::Tensor> fcos_match(at::TensorList gt_boxes, at::TensorList anchors, double radius, int64_t first_level,
+                                   int64_t last_level) {
+  const size_t B = anchors.size();
+  TORCH_CHECK(B >= 1 && gt_boxes.size() == B, "fcos_match: one gt tensor per anchor tensor");
+  const at::Tensor& a0 = anchors[0];
+  TORCH_CHECK(a0.is_cuda(), "fcos_match: anchors must be CUDA tensors");
+  const auto adt = a0.scalar_type();
+  c10::optional<at::ScalarType> gdt;
+  std::vector<vb200_fcos_image> desc(B);
+  std::vector<at::Tensor> out;
+  at::cuda::CUDAGuard guard(a0.device());
+  for (size_t i = 0; i < B; ++i) {
+    const at::Tensor &g = gt_boxes[i], &a = anchors[i];
+    TORCH_CHECK(a.is_cuda() && a.get_device() == a0.get_device() && a.scalar_type() == adt && a.dim() == 2 && a.size(1) == 4,
+                "fcos_match: anchors must be [N, 4] tensors of one dtype on one GPU");
+    TORCH_CHECK(a.size(0) < ((int64_t)1 << 31), "fcos_match: 2^31 or more anchors in one image");
+    out.push_back(at::empty({a.size(0)}, a0.options().dtype(at::kLong)));
+    vb200_fcos_image& d = desc[i];
+    d = {};
+    d.anchors = a.data_ptr();
+    d.anchor_stride[0] = a.stride(0);
+    d.anchor_stride[1] = a.stride(1);
+    d.num_anchors = a.size(0);
+    d.out = out.back().data_ptr<int64_t>();
+    if (g.numel() == 0) continue;
+    TORCH_CHECK(g.is_cuda() && g.get_device() == a0.get_device() && g.dim() == 2 && g.size(1) == 4,
+                "fcos_match: gt boxes must be [M, 4] tensors on the anchors' GPU");
+    TORCH_CHECK(!gdt || g.scalar_type() == *gdt, "fcos_match: gt boxes must share one dtype");
+    TORCH_CHECK(g.size(0) < ((int64_t)1 << 31), "fcos_match: 2^31 or more gt boxes in one image");
+    gdt = g.scalar_type();
+    d.gt = g.data_ptr();
+    d.gt_stride[0] = g.stride(0);
+    d.gt_stride[1] = g.stride(1);
+    d.num_gt = (int)g.size(0);
+  }
+  check_rc(vb200_fcos_match(desc.data(), (int)B, dtype_code(gdt ? *gdt : adt, "fcos_match"), dtype_code(adt, "fcos_match"), radius,
+                            first_level, last_level, cur_stream()),
+           "fcos_match");
+  return out;
+}
+
 // ---- box_iou_rotated (csrc/ops/box_iou_rotated.cpp; checks as cuda/box_iou_rotated_kernel.cu:92-118) ----------------
 at::Tensor box_iou_rotated(const at::Tensor& boxes1, const at::Tensor& boxes2) {
   TORCH_CHECK(boxes1.is_cuda() && boxes2.is_cuda(), "boxes1 and boxes2 must be CUDA tensors");
@@ -1025,6 +1070,7 @@ TORCH_LIBRARY(vision_b200, m) {
   m.def("rcnn_batch_images(Tensor[] images, int[] out_h, int[] out_w, int pad_h, int pad_w, float[] mean, float[] std) -> Tensor");
   m.def("rcnn_rescale(Tensor[] inputs, float[] ratio_w, float[] ratio_h) -> Tensor[]");
   m.def("match_boxes(Tensor[] gt_boxes, Tensor[] predictions, Tensor[] gt_labels, float high_threshold, float low_threshold, bool allow_low_quality_matches, int mode) -> (Tensor[], Tensor[])");
+  m.def("fcos_match(Tensor[] gt_boxes, Tensor[] anchors, float radius, int first_level, int last_level) -> Tensor[]");
   m.def("multiscale_roi_align(Tensor[] features, Tensor rois, float[] scales, int pooled_height, int pooled_width, int sampling_ratio, int k_min, int k_max, float canonical_scale, float canonical_level, float eps) -> (Tensor, Tensor)");
   m.def("_roi_align_backward(Tensor grad, Tensor rois, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width, int sampling_ratio, bool aligned) -> Tensor");
   m.def("_roi_pool_backward(Tensor grad, Tensor rois, Tensor argmax, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width) -> Tensor");
@@ -1061,6 +1107,7 @@ TORCH_LIBRARY_IMPL(vision_b200, CUDA, m) {
   m.impl("rcnn_batch_images", TORCH_FN(rcnn_batch_images));
   m.impl("rcnn_rescale", TORCH_FN(rcnn_rescale));
   m.impl("match_boxes", TORCH_FN(match_boxes));
+  m.impl("fcos_match", TORCH_FN(fcos_match));
   m.impl("resize_crop_normalize", TORCH_FN(resize_crop_normalize));
   m.impl("box_iou_rotated", TORCH_FN(box_iou_rotated));
   m.impl("_deform_conv2d_backward", TORCH_FN(deform_conv2d_backward));

@@ -17,7 +17,8 @@ bicubic resize, argmax and coordinate arithmetic, are ONE call of ``vision_b200:
 
 The training targets of ``RegionProposalNetwork.assign_targets_to_anchors`` (rpn.py:193-229),
 ``RoIHeads.assign_targets_to_proposals`` (roi_heads.py:580-613) and the matching loop of ``RetinaNet.compute_loss``
-(retinanet.py:494-507), a per-image box_iou + Matcher, are ONE call of ``vision_b200::match_boxes`` for all images."""
+(retinanet.py:494-507), a per-image box_iou + Matcher, are ONE call of ``vision_b200::match_boxes`` for all images; the
+centre-sampling matching loop of ``FCOS.compute_loss`` (fcos.py:440-487) is ONE call of ``vision_b200::fcos_match``."""
 from __future__ import annotations
 
 import math
@@ -362,8 +363,14 @@ def match_supported(matcher, gt_boxes, predictions, gt_labels=None) -> bool:
     dtype and the predictions of one dtype, both fp64 or both among fp16 / bf16 / fp32; for RoIHeads, int64 [M] labels."""
     from torchvision.models.detection import _utils as det_utils
 
-    if (_traced() or type(matcher) is not det_utils.Matcher or matcher.BELOW_LOW_THRESHOLD != -1 or matcher.BETWEEN_THRESHOLDS != -2
-            or not isinstance(gt_boxes, (list, tuple)) or not isinstance(predictions, (list, tuple)) or not predictions
+    if type(matcher) is not det_utils.Matcher or matcher.BELOW_LOW_THRESHOLD != -1 or matcher.BETWEEN_THRESHOLDS != -2:
+        return False
+    return _box_lists_supported(gt_boxes, predictions, gt_labels)
+
+
+def _box_lists_supported(gt_boxes, predictions, gt_labels=None) -> bool:
+    """The per-image box lists both matching kernels take (see match_supported), outside scripting and tracing."""
+    if (_traced() or not isinstance(gt_boxes, (list, tuple)) or not isinstance(predictions, (list, tuple)) or not predictions
             or len(gt_boxes) != len(predictions) or (gt_labels is not None and len(gt_labels) != len(predictions))):
         return False
     p0 = predictions[0]
@@ -422,4 +429,30 @@ def retinanet_compute_loss(self, targets, head_outputs, anchors, _orig=None):
     if gt_boxes is None or not match_supported(self.proposal_matcher, gt_boxes, anchors):
         return _orig(self, targets, head_outputs, anchors)
     matched_idxs, _ = match_boxes_op(gt_boxes, anchors, None, self.proposal_matcher, MATCH_RAW)
+    return self.head.compute_loss(targets, head_outputs, anchors, matched_idxs)
+
+
+def fcos_match_supported(gt_boxes, anchors, num_anchors_per_level, radius) -> bool:
+    """Inputs the FCOS kernel reproduces the reference on: the box lists of match_supported (one [M, 4] gt, or one without
+    elements, and one [N, 4] anchor tensor per image, N below 2^31, all CUDA on one device, the gt of one dtype and the
+    anchors of one, both fp64 or both among fp16 / bf16 / fp32), outside scripting and tracing; a non-empty
+    num_anchors_per_level whose first and last entries are ints; a real center_sampling_radius."""
+    return (isinstance(num_anchors_per_level, (list, tuple)) and len(num_anchors_per_level) > 0
+            and all(isinstance(k, int) and abs(k) < 2**62 for k in (num_anchors_per_level[0], num_anchors_per_level[-1]))
+            and isinstance(radius, (int, float)) and _box_lists_supported(gt_boxes, anchors))
+
+
+def fcos_match_op(gt_boxes, anchors, radius, num_anchors_per_level):
+    """Every image's matched_idx of FCOS.compute_loss (fcos.py:447-485) as one op: int64 [N] per image, -1 unmatched."""
+    _lib.load_ops()
+    return torch.ops.vision_b200.fcos_match(list(gt_boxes), list(anchors), float(radius), int(num_anchors_per_level[0]),
+                                            int(num_anchors_per_level[-1]))
+
+
+def fcos_compute_loss(self, targets, head_outputs, anchors, num_anchors_per_level, _orig=None):
+    """FCOS.compute_loss with its matching loop as one fused call; self.head.compute_loss is the reference's."""
+    gt_boxes = [t["boxes"] for t in targets] if isinstance(targets, (list, tuple)) else None
+    if gt_boxes is None or not fcos_match_supported(gt_boxes, anchors, num_anchors_per_level, self.center_sampling_radius):
+        return _orig(self, targets, head_outputs, anchors, num_anchors_per_level)
+    matched_idxs = fcos_match_op(gt_boxes, anchors, self.center_sampling_radius, num_anchors_per_level)
     return self.head.compute_loss(targets, head_outputs, anchors, matched_idxs)
