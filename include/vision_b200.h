@@ -393,6 +393,54 @@ VB200_API void vb200_fcos_level_bounds(int64_t num_anchors, int64_t first_level,
 VB200_API int vb200_fcos_match(const vb200_fcos_image* images, int num_images, int gt_dtype, int anchor_dtype, double radius,
                                int64_t first_level, int64_t last_level, vb200_stream stream);
 
+/* ---- RetinaNet head losses ---------------------------------------------------------------------------------------------
+ * Replace the per-image loops of RetinaNetClassificationHead.compute_loss (torchvision/models/detection/retinanet.py:158-189,
+ * with sigmoid_focal_loss, ops/focal_loss.py:41-56, alpha 0.25, gamma 2) and of RetinaNetRegressionHead.compute_loss
+ * (retinanet.py:272-302 with _box_loss "l1", models/detection/_utils.py:524-526, and encode_boxes, :103-118), forward and
+ * backward, for all images of a call, with no host sync and no full-size intermediate.
+ * Image i, all fp32: pred is the image's dense rows of cls_logits [A, C] or bbox_regression [A, 4] (unit stride, rows of C
+ * or 4); matched int64 [A] (element stride matched_stride), the Matcher's indices: >= 0 foreground, -2 ignored, other
+ * negatives background; classification: labels int64 [num_gt] (stride label_stride), the target class of a foreground
+ * anchor is labels[matched], a label in [-C, 0) wrapping as indexing does; regression: gt [num_gt, 4] and anchors [A, 4]
+ * (element strides (row, column)); grad (backward only) the image's dense rows of the gradient, written exactly once.
+ * A matched index >= num_gt or a label outside [-C, C) (the reference raises a device-side assert) makes the image's loss
+ * NaN and its gradient rows NaN; nothing outside labels, gt or the pred rows is read.
+ * Forward: *loss (device fp32) = (sum_i L_i) * fl(1 / B) with the images added in order, L_i = S_i / max(1, n_i) as the
+ * heads divide (a true division in the classification head, the product with fl(1 / n_i) in the regression head), S_i the
+ * image's sum, n_i its foreground count (written to num_foreground[i], device int64).  Classification elements follow the
+ * focal loss in stable fp32 forms, the regression targets are encode_single's bits.  Backward: grad_loss (device fp32, 0-dim)
+ * times the per-image scale fl(fl(g * fl(1 / B)) / max(1, n_i)) (the product with fl(1 / n_i) for regression) times the
+ * element's derivative; 0 for ignored and background-regression rows, sign(pred - target) as torch.sign (0 for ±0 and NaN).
+ * Every sum is in a fixed order, no floating-point atomics: results are bit-reproducible.  workspace: the query's bytes, a
+ * function of (B, A) only.  Per VB200_LOSS_MAX_IMAGES images one kernel launch, plus one finalize launch per forward.
+ * A * C (A * 4) must be below 2^31.  Asynchronous. */
+#define VB200_LOSS_MAX_IMAGES 64
+typedef struct vb200_retinanet_loss_image {
+  const float* pred;
+  const int64_t* matched;
+  const int64_t* labels;       /* classification only */
+  const float* gt;             /* regression only */
+  const float* anchors;        /* regression only */
+  float* grad;                 /* backward only */
+  int64_t matched_stride, label_stride, gt_stride[2], anchor_stride[2];
+  int64_t num_gt;
+} vb200_retinanet_loss_image;
+VB200_API size_t vb200_retinanet_cls_loss_workspace_bytes(int num_images, int64_t num_anchors);
+VB200_API int vb200_retinanet_cls_loss(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors, int num_classes,
+                                       float* loss, int64_t* num_foreground, void* workspace, size_t workspace_bytes,
+                                       vb200_stream stream);
+VB200_API int vb200_retinanet_cls_loss_backward(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
+                                                int num_classes, const float* grad_loss, const int64_t* num_foreground,
+                                                vb200_stream stream);
+/* weights_host: the box coder's weights as torch.as_tensor(weights, dtype=float32) rounds them */
+VB200_API size_t vb200_retinanet_box_loss_workspace_bytes(int num_images, int64_t num_anchors);
+VB200_API int vb200_retinanet_box_loss(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
+                                       const float* weights_host, float* loss, int64_t* num_foreground, void* workspace,
+                                       size_t workspace_bytes, vb200_stream stream);
+VB200_API int vb200_retinanet_box_loss_backward(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
+                                                const float* weights_host, const float* grad_loss, const int64_t* num_foreground,
+                                                vb200_stream stream);
+
 /* ---- deform_conv2d -----------------------------------------------------
  * Replaces deform_conv2d_forward_kernel, csrc/ops/cuda/deform_conv2d_kernel.cu:1035-1255
  * (schema torchvision::deform_conv2d, csrc/ops/deform_conv2d.cpp:101-102).

@@ -10,7 +10,9 @@
     python tools/prof_ops.py matching [iters]     fused vs. reference training-target assignment (RPN, RoIHeads,
                              RetinaNet), batch 2 and 8, 7 and 50 gt boxes per image
     python tools/prof_ops.py fcos [iters]     fused vs. reference FCOS.compute_loss matching, batch 2, 8 and 16, 7 and 50
-                             gt boxes per image"""
+                             gt boxes per image
+    python tools/prof_ops.py retinanet_loss [iters]     fused vs. reference RetinaNet head losses, forward + backward,
+                             batch 2 and 8, 7 and 50 gt boxes per image"""
 import os
 import sys
 
@@ -397,6 +399,111 @@ def fcos_matching(iters: int) -> None:
                   f"({t_ref / t_ours:.1f}x); outputs identical: {same}")
 
 
+def retinanet_loss(iters: int) -> None:
+    """RetinaNet's two head losses, forward + backward, on its 163,206 anchors of an 800 x 1088 batch with C = 91, batch 2 and
+    8, M in {7, 50} gt boxes per image, matches from the real Matcher: the fused methods against the uninstalled ones on the
+    same inputs.  Wall time per step ending in a synchronize (median), GPU kernel time per step from torch.profiler (a
+    separate run), the peak-memory delta over the step and the HBM bound of the fused step computed from the shapes (the
+    logits read once forward, read once and their gradient written once backward, at the data-sheet 3.35 TB/s)."""
+    import re
+    import subprocess
+    import time
+
+    from torch.profiler import ProfilerActivity, profile
+    from torchvision.models.detection import _utils as det_utils, retinanet
+    from torchvision.models.detection.anchor_utils import AnchorGenerator
+    from torchvision.models.detection.image_list import ImageList
+    from torchvision.ops import boxes as box_ops
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+    print(f"retinanet_loss: {gpu.strip().splitlines()[0] if gpu.strip() else 'unknown GPU'}")
+    C = 91
+    cls_head, box_head = retinanet.RetinaNetClassificationHead(8, 9, C), retinanet.RetinaNetRegressionHead(8, 9)
+    matcher = det_utils.Matcher(0.5, 0.4, True)
+
+    def timed(fn, n):
+        for _ in range(2):
+            fn()
+        torch.cuda.synchronize()
+        wall = []
+        for _ in range(n):
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            wall.append(time.perf_counter() - t0)
+        return sorted(wall)[n // 2] * 1e3
+
+    def kernel_ms(fn, n):
+        fn()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(n):
+                fn()
+            torch.cuda.synchronize()
+        events = [e for e in prof.key_averages() if e.device_type == torch.autograd.DeviceType.CUDA]
+        total = sum(e.self_device_time_total for e in events) / n / 1e3
+        top = sorted(events, key=lambda e: -e.self_device_time_total)[:3]
+        short = lambda k: re.sub(r"^void |vb200::|\(anonymous namespace\)::|at::native::|\(.*$", "", k)[:48]  # noqa: E731
+        return total, ", ".join(f"{short(e.key)} {e.self_device_time_total / n / 1e3:.3f}" for e in top)
+
+    def peak_mb(fn, clear):
+        clear()
+        torch.cuda.synchronize()
+        base = torch.cuda.memory_allocated()
+        torch.cuda.reset_peak_memory_stats()
+        fn()
+        torch.cuda.synchronize()
+        return (torch.cuda.max_memory_allocated() - base) / 2**20
+
+    sizes = tuple((x, int(x * 2 ** (1.0 / 3)), int(x * 2 ** (2.0 / 3))) for x in (32, 64, 128, 256, 512))
+    for batch in (2, 8):
+        gen = AnchorGenerator(sizes, ((0.5, 1.0, 2.0),) * len(sizes))
+        il = ImageList(torch.empty(batch, 3, 800, 1088, device=dev), [(800, 1088)] * batch)
+        anchors = gen(il, [torch.empty(batch, 1, -(-800 // s), -(-1088 // s), device=dev) for s in (8, 16, 32, 64, 128)])
+        A = anchors[0].shape[0]
+        for M in (7, 50):
+            g = torch.Generator(device=dev).manual_seed(M)
+            targets, matched = [], []
+            for a in anchors:
+                xy = torch.rand(M, 2, generator=g, device=dev) * torch.tensor([900.0, 650.0], device=dev)
+                boxes = torch.cat([xy, xy + torch.rand(M, 2, generator=g, device=dev) * 300 + 8], 1)
+                targets.append({"boxes": boxes, "labels": torch.randint(1, C, (M,), generator=g, device=dev)})
+                matched.append(matcher(box_ops.box_iou(boxes, a)))
+            logits = (torch.randn(batch, A, C, generator=g, device=dev) - 4.595).requires_grad_(True)
+            regression = (torch.randn(batch, A, 4, generator=g, device=dev) * 0.1).requires_grad_(True)
+
+            def clear():
+                logits.grad = regression.grad = None
+
+            def step():
+                clear()
+                loss = (cls_head.compute_loss(targets, {"cls_logits": logits}, matched)
+                        + box_head.compute_loss(targets, {"bbox_regression": regression}, anchors, matched))
+                loss.backward()
+                return loss.detach()
+
+            rows = {}
+            for name in ("reference", "fused"):
+                if name == "fused":
+                    vb.install()
+                try:
+                    loss = step()
+                    rows[name] = (loss, logits.grad.clone(), regression.grad.clone(), timed(step, iters), kernel_ms(step, 5),
+                                  peak_mb(step, clear))
+                finally:
+                    vb.uninstall()
+            bound_us = batch * A * C * 4 * 3 / 3.35e12 * 1e6
+            (l0, gc0, gr0, *_), (l1, gc1, gr1, *_) = rows["reference"], rows["fused"]
+            print(f"  batch {batch}, M {M} ({A} anchors per image, {int(sum((m >= 0).sum() for m in matched))} foreground): "
+                  f"HBM bound of the fused step {bound_us:.0f} us; loss {l0.item():.6f} vs {l1.item():.6f}, "
+                  f"max |d grad| cls {(gc0 - gc1).abs().max().item():.2e}, box {(gr0 - gr1).abs().max().item():.2e}")
+            for name, (_, _, _, wall, (kern, top), peak) in rows.items():
+                print(f"    {name:9s} wall {wall:.3f} ms per step, kernels {kern:.3f} ms ({top}), peak +{peak:.0f} MiB")
+
+
+if op == "retinanet_loss":
+    retinanet_loss(iters)
+    raise SystemExit(0)
 if op == "matching":
     matching(iters)
     raise SystemExit(0)

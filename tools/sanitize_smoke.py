@@ -2,6 +2,7 @@
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py matching     (the box-matching kernels: memcheck only)
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py fcos         (the FCOS matching kernel: memcheck only)
+    compute-sanitizer --tool memcheck python tools/sanitize_smoke.py retinanet_loss   (the head-loss kernels: memcheck only)
 No numerics are checked here (tests/ does that); the point is out-of-bounds / hazard reports."""
 import os
 import sys
@@ -170,8 +171,35 @@ def fcos():
     det.fcos_match_op([g.double() for g in gts], [a.double() for a in anchors], 2.5, [10**6, 0])
 
 
+def retinanet_loss():
+    """the head-loss kernels forward and backward, memcheck only: logits not 16-byte aligned, a row count not a multiple of
+    the tile, a background image, an image with every anchor ignored, negative labels, out-of-range labels and match
+    indices (which must read nothing outside labels, gt or the logits), strided anchors and gt boxes, and more images than
+    one launch's descriptors"""
+    from vision_b200 import detection as det
+
+    def boxes(n):
+        xy = torch.rand(n, 2, device=dev) * 500
+        return torch.cat([xy, xy + torch.rand(n, 2, device=dev) * 100 + 1], 1)
+
+    for B, A, C in ((3, 777, 91), (70, 33, 2)):
+        ms = [4 if i % 3 != 1 else 0 for i in range(B)]
+        gts = [boxes(m).t().contiguous().t() for m in ms]
+        labels = [torch.randint(-C, C, (m,), device=dev) for m in ms]
+        matched = [torch.randint(-2, max(m, 1), (A,), device=dev) for m in ms]
+        matched[-1] = torch.full((A,), -2, dtype=torch.int64, device=dev)
+        if ms[0]:
+            labels[0][0] = C + 5
+            matched[0][5] = ms[0] + 100
+        logits = torch.randn(B * A * C + 1, device=dev)[1:].view(B, A, C).requires_grad_(True)
+        regression = torch.randn(B, A, 4, device=dev, requires_grad=True)
+        anchors = [boxes(A).t().contiguous().t() for _ in range(B)]
+        (det.retinanet_cls_loss_op(logits, matched, labels) + det.retinanet_box_loss_op(regression, anchors, gts, matched,
+                                                                                         [1.0, 1.0, 1.0, 1.0])).backward()
+
+
 for name, fn in (("roi", roi), ("bwd", bwd), ("nms", nms), ("resize", resize), ("dcn", dcn), ("gather", gather), ("matching", matching),
-                 ("fcos", fcos)):
+                 ("fcos", fcos), ("retinanet_loss", retinanet_loss)):
     if only in ("all", name):
         fn()
         torch.cuda.synchronize()

@@ -190,6 +190,50 @@ def register() -> None:
     def _(gt_boxes, anchors, radius, first_level, last_level):
         return [a.new_empty((a.shape[0],), dtype=torch.int64) for a in anchors]
 
+    # ---- RetinaNet head losses: cls_logits and bbox_regression are the only differentiable inputs; the counts are not ----
+    def cls_loss_setup(ctx, inputs, output):
+        logits, matched, labels = inputs
+        ctx.mark_non_differentiable(output[1])
+        ctx.save_for_backward(logits, output[1])
+        ctx.lists = (list(matched), list(labels))
+
+    def cls_loss_backward(ctx, grad, _grad_counts):
+        logits, counts = ctx.saved_tensors
+        matched, labels = ctx.lists
+        return ops.retinanet_cls_loss_backward(grad, logits, matched, labels, counts), [None] * len(matched), [None] * len(labels)
+
+    lib.register_autograd("vision_b200::retinanet_cls_loss", cls_loss_backward, setup_context=cls_loss_setup)
+
+    def box_loss_setup(ctx, inputs, output):
+        regression, anchors, gt_boxes, matched, weights = inputs
+        ctx.mark_non_differentiable(output[1])
+        ctx.save_for_backward(regression, output[1])
+        ctx.lists = (list(anchors), list(gt_boxes), list(matched), list(weights))
+
+    def box_loss_backward(ctx, grad, _grad_counts):
+        regression, counts = ctx.saved_tensors
+        anchors, gt_boxes, matched, weights = ctx.lists
+        return (ops.retinanet_box_loss_backward(grad, regression, anchors, gt_boxes, matched, weights, counts), [None] * len(anchors),
+                [None] * len(gt_boxes), [None] * len(matched), None)
+
+    lib.register_autograd("vision_b200::retinanet_box_loss", box_loss_backward, setup_context=box_loss_setup)
+
+    @lib.register_fake("vision_b200::retinanet_cls_loss")
+    def _(cls_logits, matched_idxs, labels):
+        return cls_logits.new_empty(()), cls_logits.new_empty((cls_logits.shape[0],), dtype=torch.int64)
+
+    @lib.register_fake("vision_b200::retinanet_cls_loss_backward")
+    def _(grad, cls_logits, matched_idxs, labels, num_foreground):
+        return cls_logits.new_empty(cls_logits.shape)
+
+    @lib.register_fake("vision_b200::retinanet_box_loss")
+    def _(bbox_regression, anchors, gt_boxes, matched_idxs, weights):
+        return bbox_regression.new_empty(()), bbox_regression.new_empty((bbox_regression.shape[0],), dtype=torch.int64)
+
+    @lib.register_fake("vision_b200::retinanet_box_loss_backward")
+    def _(grad, bbox_regression, anchors, gt_boxes, matched_idxs, weights, num_foreground):
+        return bbox_regression.new_empty(bbox_regression.shape)
+
     # ---- deform_conv2d ----
     def dcn_setup(ctx, inputs, output):
         inp, weight, offset, mask, bias = inputs[:5]

@@ -21,6 +21,8 @@
    Training targets: ``RegionProposalNetwork.assign_targets_to_anchors``, ``RoIHeads.assign_targets_to_proposals`` and
    ``RetinaNet.compute_loss`` are rebound on their classes; the per-image box_iou + Matcher loop becomes one call.
    ``FCOS.compute_loss`` likewise: its per-image centre-sampling loop becomes one call.
+   Head losses: ``RetinaNetClassificationHead.compute_loss`` and ``RetinaNetRegressionHead.compute_loss`` are rebound on
+   their classes; each per-image loss loop becomes one call with a fused backward.
 5. ``resize`` has no torchvision kernel (transforms/v2/functional/_geometry.py:283-362 calls
    F.interpolate): the entries of ``_KERNEL_REGISTRY[resize]`` for Tensor / Image / Video are swapped.
 CPU tensors and unsupported dtypes/modes keep flowing to the reference implementation.
@@ -153,6 +155,20 @@ def install() -> None:
         matching[(cls, name)] = orig
         setattr(cls, name, fused)
 
+    # ---- RetinaNet head losses (retinanet.py:158-189, 272-302): bound on the head classes; RetinaNetHead.compute_loss stays
+    # torchvision's and calls them ----
+    losses = {}
+    for cls, body in ((tv_retinanet.RetinaNetClassificationHead, _det.retinanet_cls_compute_loss),
+                      (tv_retinanet.RetinaNetRegressionHead, _det.retinanet_box_compute_loss)):
+        orig = cls.compute_loss
+
+        def fused(self, *args, _body=body, _orig=orig, **kwargs):
+            return _body(self, *args, _orig=_orig, **kwargs)
+
+        functools.update_wrapper(fused, orig)
+        losses[(cls, "compute_loss")] = orig
+        cls.compute_loss = fused
+
     # ---- detection model inputs and outputs (transform.py:119-158, 257-277): bound on the class, so every model's
     # self.transform (Faster / Mask / Keypoint R-CNN, RetinaNet, FCOS, SSD, SSDLite) picks them up ----
     from torchvision.models.detection import transform as tv_transform
@@ -220,7 +236,7 @@ def install() -> None:
                        registry=registry, saved_registry=saved, tv_poolers=tv_poolers, orig_msra=orig_msra,
                        tv_roi_align_mod=tv_roi_align_mod, orig_det_roi_align=orig_det_roi_align,
                        tv_roi_heads=tv_roi_heads, tv_rpn=tv_rpn, orig_pp=orig_pp, orig_fp=orig_fp, orig_kri=orig_kri, orig_h2k=orig_h2k,
-                       tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage, matching=matching,
+                       tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage, matching=matching, losses=losses,
                        rcnn_transform=rcnn_transform, orig_tf_forward=orig_tf_forward, orig_tf_post=orig_tf_post))
 
 
@@ -241,7 +257,7 @@ def uninstall() -> None:
     _state["rcnn_transform"].postprocess = _state["orig_tf_post"]
     for cls, orig in _state["single_stage"].items():
         cls.postprocess_detections = orig
-    for (cls, name), orig in _state["matching"].items():
+    for (cls, name), orig in list(_state["matching"].items()) + list(_state["losses"].items()):
         setattr(cls, name, orig)
     reg = _state["registry"]
     reg.clear()

@@ -85,5 +85,7 @@ ABI_SYMBOLS = (
     "vb200_ps_roi_pool_backward_ex", "vb200_roi_backward_deterministic_supported",
     "vb200_heatmaps_to_keypoints_workspace_bytes", "vb200_heatmaps_to_keypoints",
     "vb200_rcnn_batch_images", "vb200_rcnn_rescale", "vb200_match_boxes_workspace_bytes", "vb200_match_boxes",
-    "vb200_fcos_level_bounds", "vb200_fcos_match",
+    "vb200_fcos_level_bounds", "vb200_fcos_match", "vb200_retinanet_cls_loss_workspace_bytes", "vb200_retinanet_cls_loss",
+    "vb200_retinanet_cls_loss_backward", "vb200_retinanet_box_loss_workspace_bytes", "vb200_retinanet_box_loss",
+    "vb200_retinanet_box_loss_backward",
 )

@@ -18,6 +18,7 @@
 #include <torch/library.h>
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <memory>
 #include <mutex>
@@ -1001,6 +1002,135 @@ std::vector<at::Tensor> fcos_match(at::TensorList gt_boxes, at::TensorList ancho
   return out;
 }
 
+// ---- RetinaNet head losses (retinanet.py:158-189, 272-302) --------------------------------------------------------------
+// pred: cls_logits [B, A, C] or bbox_regression [B, A, 4], fp32 on one GPU with dense rows (unit stride in the last dimension,
+// rows of its width).  matched_idxs: one int64 [A] per image; labels: one int64 [M_i] per image (classification); gt_boxes /
+// anchors: one fp32 [M_i, 4] / [A, 4] per image (regression).  Returns the 0-dim loss and the int64 [B] foreground counts the
+// backward takes; the backward returns the dense gradient of pred.
+std::vector<vb200_retinanet_loss_image> loss_images(const at::Tensor& pred, int64_t width, at::TensorList matched_idxs, at::TensorList labels,
+                                                    at::TensorList anchors, at::TensorList gt_boxes, bool box, const char* op) {
+  TORCH_CHECK(pred.is_cuda() && pred.scalar_type() == at::kFloat && pred.dim() == 3 && pred.size(0) >= 1, op,
+              ": the predictions must be a CUDA float32 [B, A, ", box ? "4" : "C", "] tensor with B >= 1");
+  const int64_t B = pred.size(0), A = pred.size(1);
+  TORCH_CHECK(pred.size(2) == width && pred.stride(2) == 1 && (A <= 1 || pred.stride(1) == width), op,
+              ": each image's predictions must be dense rows");
+  TORCH_CHECK(A * width < ((int64_t)1 << 31), op, ": 2^31 or more predictions in one image");
+  TORCH_CHECK((int64_t)matched_idxs.size() == B && (int64_t)(box ? gt_boxes.size() : labels.size()) == B &&
+                  (!box || (int64_t)anchors.size() == B),
+              op, ": one matched_idxs and one target per image");
+  const auto same_gpu = [&](const at::Tensor& t) { return t.is_cuda() && t.get_device() == pred.get_device(); };
+  std::vector<vb200_retinanet_loss_image> desc((size_t)B);
+  for (int64_t i = 0; i < B; ++i) {
+    vb200_retinanet_loss_image& d = desc[(size_t)i];
+    d = {};
+    d.pred = pred.data_ptr<float>() + i * pred.stride(0);
+    const at::Tensor& m = matched_idxs[i];
+    TORCH_CHECK(same_gpu(m) && m.scalar_type() == at::kLong && m.dim() == 1 && m.size(0) == A, op,
+                ": matched_idxs must be int64 [A] tensors on the predictions' GPU");
+    d.matched = m.data_ptr<int64_t>();
+    d.matched_stride = m.stride(0);
+    if (box) {
+      const at::Tensor &g = gt_boxes[i], &a = anchors[i];
+      TORCH_CHECK(same_gpu(g) && g.scalar_type() == at::kFloat && g.dim() == 2 && g.size(1) == 4, op,
+                  ": gt boxes must be float32 [M, 4] tensors on the predictions' GPU");
+      TORCH_CHECK(same_gpu(a) && a.scalar_type() == at::kFloat && a.dim() == 2 && a.size(0) == A && a.size(1) == 4, op,
+                  ": anchors must be float32 [A, 4] tensors on the predictions' GPU");
+      d.gt = g.data_ptr<float>();
+      d.gt_stride[0] = g.stride(0);
+      d.gt_stride[1] = g.stride(1);
+      d.num_gt = g.size(0);
+      d.anchors = a.data_ptr<float>();
+      d.anchor_stride[0] = a.stride(0);
+      d.anchor_stride[1] = a.stride(1);
+    } else {
+      const at::Tensor& l = labels[i];
+      TORCH_CHECK(same_gpu(l) && l.scalar_type() == at::kLong && l.dim() == 1, op, ": labels must be int64 [M] tensors on the predictions' GPU");
+      d.labels = l.data_ptr<int64_t>();
+      d.label_stride = l.stride(0);
+      d.num_gt = l.size(0);
+    }
+  }
+  return desc;
+}
+
+std::array<float, 4> coder_weights(at::ArrayRef<double> weights, const char* op) {
+  TORCH_CHECK(weights.size() == 4, op, ": four box coder weights");
+  return {(float)weights[0], (float)weights[1], (float)weights[2], (float)weights[3]};
+}
+
+std::tuple<at::Tensor, at::Tensor> retinanet_cls_loss(const at::Tensor& cls_logits, at::TensorList matched_idxs, at::TensorList labels) {
+  TORCH_CHECK(cls_logits.dim() == 3, "retinanet_cls_loss: cls_logits must be [B, A, C]");
+  auto desc = loss_images(cls_logits, cls_logits.size(2), matched_idxs, labels, {}, {}, false, "retinanet_cls_loss");
+  at::cuda::CUDAGuard guard(cls_logits.device());
+  const int B = (int)desc.size();
+  const int64_t A = cls_logits.size(1);
+  at::Tensor loss = at::empty({}, cls_logits.options());
+  at::Tensor counts = at::empty({B}, cls_logits.options().dtype(at::kLong));
+  const size_t wsb = vb200_retinanet_cls_loss_workspace_bytes(B, A);
+  at::Tensor ws = workspace(wsb, cls_logits);
+  check_rc(vb200_retinanet_cls_loss(desc.data(), B, A, (int)cls_logits.size(2), loss.data_ptr<float>(), counts.data_ptr<int64_t>(),
+                                    ws.data_ptr(), wsb, cur_stream()),
+           "retinanet_cls_loss");
+  return std::make_tuple(loss, counts);
+}
+
+at::Tensor retinanet_cls_loss_backward(const at::Tensor& grad, const at::Tensor& cls_logits, at::TensorList matched_idxs, at::TensorList labels,
+                                       const at::Tensor& num_foreground) {
+  TORCH_CHECK(cls_logits.dim() == 3, "retinanet_cls_loss_backward: cls_logits must be [B, A, C]");
+  auto desc = loss_images(cls_logits, cls_logits.size(2), matched_idxs, labels, {}, {}, false, "retinanet_cls_loss_backward");
+  const int B = (int)desc.size();
+  TORCH_CHECK(grad.is_cuda() && grad.get_device() == cls_logits.get_device() && grad.scalar_type() == at::kFloat && grad.numel() == 1,
+              "retinanet_cls_loss_backward: the gradient must be one float32 value on the logits' GPU");
+  TORCH_CHECK(num_foreground.is_cuda() && num_foreground.get_device() == cls_logits.get_device() && num_foreground.scalar_type() == at::kLong &&
+                  num_foreground.dim() == 1 && num_foreground.size(0) == B,
+              "retinanet_cls_loss_backward: num_foreground must be the forward's int64 [B] counts");
+  at::cuda::CUDAGuard guard(cls_logits.device());
+  at::Tensor g = grad.contiguous(), n = num_foreground.contiguous();
+  at::Tensor out = at::empty(cls_logits.sizes(), cls_logits.options());
+  for (int i = 0; i < B; ++i) desc[(size_t)i].grad = out.data_ptr<float>() + (int64_t)i * out.stride(0);
+  check_rc(vb200_retinanet_cls_loss_backward(desc.data(), B, cls_logits.size(1), (int)cls_logits.size(2), g.data_ptr<float>(),
+                                             n.data_ptr<int64_t>(), cur_stream()),
+           "retinanet_cls_loss_backward");
+  return out;
+}
+
+std::tuple<at::Tensor, at::Tensor> retinanet_box_loss(const at::Tensor& bbox_regression, at::TensorList anchors, at::TensorList gt_boxes,
+                                                      at::TensorList matched_idxs, at::ArrayRef<double> weights) {
+  auto desc = loss_images(bbox_regression, 4, matched_idxs, {}, anchors, gt_boxes, true, "retinanet_box_loss");
+  const auto w = coder_weights(weights, "retinanet_box_loss");
+  at::cuda::CUDAGuard guard(bbox_regression.device());
+  const int B = (int)desc.size();
+  const int64_t A = bbox_regression.size(1);
+  at::Tensor loss = at::empty({}, bbox_regression.options());
+  at::Tensor counts = at::empty({B}, bbox_regression.options().dtype(at::kLong));
+  const size_t wsb = vb200_retinanet_box_loss_workspace_bytes(B, A);
+  at::Tensor ws = workspace(wsb, bbox_regression);
+  check_rc(vb200_retinanet_box_loss(desc.data(), B, A, w.data(), loss.data_ptr<float>(), counts.data_ptr<int64_t>(), ws.data_ptr(), wsb,
+                                    cur_stream()),
+           "retinanet_box_loss");
+  return std::make_tuple(loss, counts);
+}
+
+at::Tensor retinanet_box_loss_backward(const at::Tensor& grad, const at::Tensor& bbox_regression, at::TensorList anchors, at::TensorList gt_boxes,
+                                       at::TensorList matched_idxs, at::ArrayRef<double> weights, const at::Tensor& num_foreground) {
+  auto desc = loss_images(bbox_regression, 4, matched_idxs, {}, anchors, gt_boxes, true, "retinanet_box_loss_backward");
+  const auto w = coder_weights(weights, "retinanet_box_loss_backward");
+  const int B = (int)desc.size();
+  TORCH_CHECK(grad.is_cuda() && grad.get_device() == bbox_regression.get_device() && grad.scalar_type() == at::kFloat && grad.numel() == 1,
+              "retinanet_box_loss_backward: the gradient must be one float32 value on the regression's GPU");
+  TORCH_CHECK(num_foreground.is_cuda() && num_foreground.get_device() == bbox_regression.get_device() &&
+                  num_foreground.scalar_type() == at::kLong && num_foreground.dim() == 1 && num_foreground.size(0) == B,
+              "retinanet_box_loss_backward: num_foreground must be the forward's int64 [B] counts");
+  at::cuda::CUDAGuard guard(bbox_regression.device());
+  at::Tensor g = grad.contiguous(), n = num_foreground.contiguous();
+  at::Tensor out = at::empty(bbox_regression.sizes(), bbox_regression.options());
+  for (int i = 0; i < B; ++i) desc[(size_t)i].grad = out.data_ptr<float>() + (int64_t)i * out.stride(0);
+  check_rc(vb200_retinanet_box_loss_backward(desc.data(), B, bbox_regression.size(1), w.data(), g.data_ptr<float>(), n.data_ptr<int64_t>(),
+                                             cur_stream()),
+           "retinanet_box_loss_backward");
+  return out;
+}
+
 // ---- box_iou_rotated (csrc/ops/box_iou_rotated.cpp; checks as cuda/box_iou_rotated_kernel.cu:92-118) ----------------
 at::Tensor box_iou_rotated(const at::Tensor& boxes1, const at::Tensor& boxes2) {
   TORCH_CHECK(boxes1.is_cuda() && boxes2.is_cuda(), "boxes1 and boxes2 must be CUDA tensors");
@@ -1071,6 +1201,10 @@ TORCH_LIBRARY(vision_b200, m) {
   m.def("rcnn_rescale(Tensor[] inputs, float[] ratio_w, float[] ratio_h) -> Tensor[]");
   m.def("match_boxes(Tensor[] gt_boxes, Tensor[] predictions, Tensor[] gt_labels, float high_threshold, float low_threshold, bool allow_low_quality_matches, int mode) -> (Tensor[], Tensor[])");
   m.def("fcos_match(Tensor[] gt_boxes, Tensor[] anchors, float radius, int first_level, int last_level) -> Tensor[]");
+  m.def("retinanet_cls_loss(Tensor cls_logits, Tensor[] matched_idxs, Tensor[] labels) -> (Tensor, Tensor)");
+  m.def("retinanet_cls_loss_backward(Tensor grad, Tensor cls_logits, Tensor[] matched_idxs, Tensor[] labels, Tensor num_foreground) -> Tensor");
+  m.def("retinanet_box_loss(Tensor bbox_regression, Tensor[] anchors, Tensor[] gt_boxes, Tensor[] matched_idxs, float[] weights) -> (Tensor, Tensor)");
+  m.def("retinanet_box_loss_backward(Tensor grad, Tensor bbox_regression, Tensor[] anchors, Tensor[] gt_boxes, Tensor[] matched_idxs, float[] weights, Tensor num_foreground) -> Tensor");
   m.def("multiscale_roi_align(Tensor[] features, Tensor rois, float[] scales, int pooled_height, int pooled_width, int sampling_ratio, int k_min, int k_max, float canonical_scale, float canonical_level, float eps) -> (Tensor, Tensor)");
   m.def("_roi_align_backward(Tensor grad, Tensor rois, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width, int sampling_ratio, bool aligned) -> Tensor");
   m.def("_roi_pool_backward(Tensor grad, Tensor rois, Tensor argmax, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width) -> Tensor");
@@ -1108,6 +1242,10 @@ TORCH_LIBRARY_IMPL(vision_b200, CUDA, m) {
   m.impl("rcnn_rescale", TORCH_FN(rcnn_rescale));
   m.impl("match_boxes", TORCH_FN(match_boxes));
   m.impl("fcos_match", TORCH_FN(fcos_match));
+  m.impl("retinanet_cls_loss", TORCH_FN(retinanet_cls_loss));
+  m.impl("retinanet_cls_loss_backward", TORCH_FN(retinanet_cls_loss_backward));
+  m.impl("retinanet_box_loss", TORCH_FN(retinanet_box_loss));
+  m.impl("retinanet_box_loss_backward", TORCH_FN(retinanet_box_loss_backward));
   m.impl("resize_crop_normalize", TORCH_FN(resize_crop_normalize));
   m.impl("box_iou_rotated", TORCH_FN(box_iou_rotated));
   m.impl("_deform_conv2d_backward", TORCH_FN(deform_conv2d_backward));

@@ -18,7 +18,12 @@ bicubic resize, argmax and coordinate arithmetic, are ONE call of ``vision_b200:
 The training targets of ``RegionProposalNetwork.assign_targets_to_anchors`` (rpn.py:193-229),
 ``RoIHeads.assign_targets_to_proposals`` (roi_heads.py:580-613) and the matching loop of ``RetinaNet.compute_loss``
 (retinanet.py:494-507), a per-image box_iou + Matcher, are ONE call of ``vision_b200::match_boxes`` for all images; the
-centre-sampling matching loop of ``FCOS.compute_loss`` (fcos.py:440-487) is ONE call of ``vision_b200::fcos_match``."""
+centre-sampling matching loop of ``FCOS.compute_loss`` (fcos.py:440-487) is ONE call of ``vision_b200::fcos_match``.
+
+RetinaNet's head losses, ``RetinaNetClassificationHead.compute_loss`` (retinanet.py:158-189, the sigmoid focal loss) and
+``RetinaNetRegressionHead.compute_loss`` (:272-302, the "l1" box loss), per-image loops of full-size masks, gathers and
+elementwise chains, are ONE call each of ``vision_b200::retinanet_cls_loss`` / ``retinanet_box_loss`` for all images, with
+a fused backward (_autograd.py)."""
 from __future__ import annotations
 
 import math
@@ -430,6 +435,94 @@ def retinanet_compute_loss(self, targets, head_outputs, anchors, _orig=None):
         return _orig(self, targets, head_outputs, anchors)
     matched_idxs, _ = match_boxes_op(gt_boxes, anchors, None, self.proposal_matcher, MATCH_RAW)
     return self.head.compute_loss(targets, head_outputs, anchors, matched_idxs)
+
+
+def _same_gpu(t, device, dtype=None, dim=None) -> bool:
+    return (isinstance(t, Tensor) and t.is_cuda and t.device == device and (dtype is None or t.dtype == dtype)
+            and (dim is None or t.dim() == dim))
+
+
+def _loss_inputs_ok(targets, pred, matched_idxs, width) -> bool:
+    """What both fused head losses take: outside scripting and tracing, one target dict and one int64 [A] matched_idxs per
+    image of a fp32 CUDA [B, A, width] prediction tensor whose rows are dense, A * width below 2^31."""
+    if (_traced() or not isinstance(targets, (list, tuple)) or not targets or not isinstance(matched_idxs, (list, tuple))
+            or not isinstance(pred, Tensor) or not pred.is_cuda or pred.dtype != torch.float32 or pred.dim() != 3):
+        return False
+    B, A, C = pred.shape
+    if not (len(targets) == len(matched_idxs) == B and C == width >= 1 and A * C < 2**31 and pred.stride(2) == 1
+            and (A <= 1 or pred.stride(1) == C)):
+        return False
+    return all(isinstance(t, dict) and _same_gpu(m, pred.device, torch.int64, 1) and m.shape[0] == A
+               for t, m in zip(targets, matched_idxs))
+
+
+def retinanet_cls_loss_supported(head, targets, cls_logits, matched_idxs) -> bool:
+    """Inputs the focal-loss kernels reproduce RetinaNetClassificationHead.compute_loss on: those of _loss_inputs_ok with
+    the logits' C, an int64 [M] labels tensor per image on the logits' GPU, and the Matcher's -2 for ignored anchors."""
+    if getattr(head, "BETWEEN_THRESHOLDS", None) != -2 or not isinstance(cls_logits, Tensor) or cls_logits.dim() != 3:
+        return False
+    if not _loss_inputs_ok(targets, cls_logits, matched_idxs, cls_logits.shape[2]):
+        return False
+    return all(_same_gpu(t.get("labels"), cls_logits.device, torch.int64, 1) for t in targets)
+
+
+def retinanet_cls_loss_op(cls_logits, matched_idxs, labels):
+    _lib.load_ops()
+    loss, _ = torch.ops.vision_b200.retinanet_cls_loss(cls_logits, list(matched_idxs), list(labels))
+    return loss
+
+
+def retinanet_cls_compute_loss(self, targets, head_outputs, matched_idxs, _orig=None):
+    """RetinaNetClassificationHead.compute_loss as one fused call for all images: the same loss, and a dense gradient of
+    cls_logits written in one pass."""
+    cls_logits = head_outputs["cls_logits"] if isinstance(head_outputs, dict) else None
+    if not retinanet_cls_loss_supported(self, targets, cls_logits, matched_idxs):
+        return _orig(self, targets, head_outputs, matched_idxs)
+    return retinanet_cls_loss_op(cls_logits, matched_idxs, [t["labels"] for t in targets])
+
+
+def _coder_weights(box_coder):
+    """The coder's weights as encode_single's torch.as_tensor(weights, dtype=float32) rounds them, or None."""
+    w = box_coder.weights
+    if not isinstance(w, (list, tuple)) or len(w) != 4 or not all(isinstance(v, (int, float)) for v in w):
+        return None
+    return [float(v) for v in np.asarray(w, dtype=np.float32)]
+
+
+def retinanet_box_loss_supported(head, targets, bbox_regression, anchors, matched_idxs) -> bool:
+    """Inputs the box-loss kernels reproduce RetinaNetRegressionHead.compute_loss on: the "l1" loss with a plain
+    ``det_utils.BoxCoder`` of four numeric weights, the inputs of _loss_inputs_ok with width 4, and fp32 [A, 4] anchors and
+    [M, 4] gt boxes per image on the regression's GPU."""
+    from torchvision.models.detection import _utils as det_utils
+
+    if getattr(head, "_loss_type", None) != "l1" or type(getattr(head, "box_coder", None)) is not det_utils.BoxCoder:
+        return False
+    if _coder_weights(head.box_coder) is None or not _loss_inputs_ok(targets, bbox_regression, matched_idxs, 4):
+        return False
+    if not isinstance(anchors, (list, tuple)) or len(anchors) != len(targets):
+        return False
+    A, device = bbox_regression.shape[1], bbox_regression.device
+    for t, a in zip(targets, anchors):
+        g = t.get("boxes")
+        if not (_same_gpu(g, device, torch.float32, 2) and g.shape[1] == 4 and _same_gpu(a, device, torch.float32, 2)
+                and tuple(a.shape) == (A, 4)):
+            return False
+    return True
+
+
+def retinanet_box_loss_op(bbox_regression, anchors, gt_boxes, matched_idxs, weights):
+    _lib.load_ops()
+    loss, _ = torch.ops.vision_b200.retinanet_box_loss(bbox_regression, list(anchors), list(gt_boxes), list(matched_idxs), list(weights))
+    return loss
+
+
+def retinanet_box_compute_loss(self, targets, head_outputs, anchors, matched_idxs, _orig=None):
+    """RetinaNetRegressionHead.compute_loss ("l1") as one fused call for all images: the same loss, and a dense gradient of
+    bbox_regression written in one pass."""
+    regression = head_outputs["bbox_regression"] if isinstance(head_outputs, dict) else None
+    if not retinanet_box_loss_supported(self, targets, regression, anchors, matched_idxs):
+        return _orig(self, targets, head_outputs, anchors, matched_idxs)
+    return retinanet_box_loss_op(regression, anchors, [t["boxes"] for t in targets], matched_idxs, _coder_weights(self.box_coder))
 
 
 def fcos_match_supported(gt_boxes, anchors, num_anchors_per_level, radius) -> bool:
