@@ -213,11 +213,8 @@ def dcn_path(dtype, c_in, c_out, kh, kw, groups, offset_groups):
     raise AssertionError(f"unexpected packed-weight size {n}")
 
 
-def launched_forward_kernels(fn):
-    """Runs fn under torch.profiler and names the deform_conv2d forward kernels it launched: "tc256" / "tc128" for
-    deform_conv2d_tc_kernel with BN = 256 / 128 output channels per CTA (its second template argument), "tc3" for
-    deform_conv2d_tc3_kernel, "simt" for deform_conv2d_simt_kernel.  The packed-weight query tells the path class only;
-    BN shows in the kernel's name alone.
+def launched_kernel_names(fn):
+    """Runs fn under torch.profiler: (its result, the names of the events it recorded, device kernels among them).
 
     The profiler now and then delivers no device activity at all for a short session; fn (deterministic) then runs
     again, up to three times.  A session that recorded device kernels is never retried, whatever it found."""
@@ -231,8 +228,17 @@ def launched_forward_kernels(fn):
         events = prof.events()
         if any(e.device_type == DeviceType.CUDA for e in events):
             break
+    return out, {e.name for e in events}
+
+
+def launched_forward_kernels(fn):
+    """Runs fn under torch.profiler and names the deform_conv2d forward kernels it launched: "tc256" / "tc128" for
+    deform_conv2d_tc_kernel with BN = 256 / 128 output channels per CTA (its second template argument), "tc3" for
+    deform_conv2d_tc3_kernel, "simt" for deform_conv2d_simt_kernel.  The packed-weight query tells the path class only;
+    BN shows in the kernel's name alone."""
+    out, names = launched_kernel_names(fn)
     labels = set()
-    for name in {e.name for e in events}:
+    for name in names:
         bn = re.search(r"deform_conv2d_tc_kernel<[^,]*,[^0-9]*(\d+)", name) or re.search(r"deform_conv2d_tc_kernelI\w+?Li(\d+)E", name)
         if bn:
             labels.add("tc" + bn.group(1))

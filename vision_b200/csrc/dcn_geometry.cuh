@@ -50,11 +50,18 @@ struct Sample {
   int hl, wl;        // the sample's cell: floor(y), floor(x)
 };
 
-template <typename A>
+// A position past +-2^31 saturates the conversion to INT_MAX / INT_MIN, and hl + 1 then overflows.  By default the next row /
+// column is a wrapping add (INT_MAX + 1 = INT_MIN, outside the image like the sample).  As a signed add the overflow is
+// undefined and the compiler folds the corner tests through it (hh >= 0 into hl > -2), which passed a corner of such a
+// sample as live: the backward's grad_offset, which has no outer test, then summed it with a fraction y - hl of up to 1e12.
+// INSIDE_ONLY keeps the signed add for callers that read the corners of `inside` samples alone (hl in [-1, H - 1], no
+// overflow; an outside sample's flags are never read): the forward, whose tensor-core kernel measured 2% slower with the
+// wrapping add (the folded tests are shorter in its table fill).
+template <typename A, bool INSIDE_ONLY = false>
 __device__ __forceinline__ Sample<A> make_sample(A y, A x, int H, int W) {
   Sample<A> s;
   const int hl = (int)floor(y), wl = (int)floor(x);
-  const int hh = hl + 1, wh = wl + 1;
+  const int hh = INSIDE_ONLY ? hl + 1 : (int)((unsigned)hl + 1u), wh = INSIDE_ONLY ? wl + 1 : (int)((unsigned)wl + 1u);
   s.hl = hl; s.wl = wl;
   s.lh = y - (A)hl; s.lw = x - (A)wl;
   s.inside = !(y <= (A)-1 || (A)H <= y || x <= (A)-1 || (A)W <= x);
@@ -109,7 +116,7 @@ __device__ __forceinline__ void fill_sample_table(DcnTabEnt* tab, const T* __res
     if (pix < HWo) {
       float y, x, m;
       sample_position<float>(off, msk, p, t0 + tl, pix, y, x, m);
-      const Sample<float> s = make_sample<float>(y, x, p.in_h, p.in_w);
+      const Sample<float> s = make_sample<float, true>(y, x, p.in_h, p.in_w);
       if (s.inside) {
         float w[4];
         corner_weights(s, w);

@@ -183,7 +183,7 @@ deform_conv2d_f64_kernel(const double* __restrict__ in, const double* __restrict
       for (int tap = 0; tap < KK; ++tap) {
         double y, x, m;
         sample_position<double>(off + ob * HWo, mask + ob / 2 * HWo, p, tap, pix, y, x, m);
-        const Sample<double> s = make_sample<double>(y, x, p.in_h, p.in_w);
+        const Sample<double> s = make_sample<double, true>(y, x, p.in_h, p.in_w);
         double val = 0;
         if (s.inside) {
           double wt[4], v[4];
