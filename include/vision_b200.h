@@ -441,6 +441,59 @@ VB200_API int vb200_retinanet_box_loss_backward(const vb200_retinanet_loss_image
                                                 const float* weights_host, const float* grad_loss, const int64_t* num_foreground,
                                                 vb200_stream stream);
 
+/* ---- FCOS head losses --------------------------------------------------------------------------------------------------
+ * Replace FCOSHead.compute_loss (torchvision/models/detection/fcos.py:52-125): its per-image gather loop, the .item() host
+ * sync, sigmoid_focal_loss (ops/focal_loss.py:41-56, alpha 0.25, gamma 2), BoxLinearCoder.decode / .encode
+ * (models/detection/_utils.py:240-310), generalized_box_iou_loss (ops/giou_loss.py with _loss_inter_union, ops/_utils.py:87-105)
+ * and binary_cross_entropy_with_logits on the centre-ness, forward and backward, for all images of a call, with no host sync
+ * and no full-size intermediate.  Two calls: the classification loss, and the GIoU and centre-ness losses together.
+ * Image i, all fp32: pred is the image's dense rows of cls_logits [A, C] or bbox_regression [A, 4] (unit stride, rows of C
+ * or 4); ctrness the image's bbox_ctrness [A] (element stride ctrness_stride, box call only); matched int64 [A] (stride
+ * matched_stride); labels int64 [num_gt] (stride label_stride); gt [num_gt, 4] and anchors [A, 4] (element strides (row,
+ * column), box call only); grad / grad_ctrness (backward only) the image's dense rows of the gradients, written exactly once.
+ * Foreground, as the reference derives it with m = matched[a]: m < 0 (-2 included) is background; an image with no gt and
+ * m >= 0 has target class 0 and the zero gt box; otherwise l = labels[m] is the target class if l >= 0 and background if
+ * l < 0 (not wrapped).  m >= num_gt > 0, or (classification) l >= C, is bad: the reference raises a device-side assert, here
+ * the loss is NaN and the anchor's gradient rows NaN; nothing outside labels, gt or the pred rows is read.
+ * n = the number of foreground anchors of the whole batch (bad ones included), written to *num_foreground (device int64).
+ * Forward: each *loss (device fp32) = fl(S) * fl(1 / max(1, n)), S the sum over the whole batch (the head divides by the
+ * Python int from .item(), which ATen's CUDA division turns into the product with its fp32 reciprocal; no 1 / B).
+ * Classification: the focal loss of every element, in the stable forms of the RetinaNet call.  Box: per foreground anchor
+ * the GIoU loss of decode(bbox_regression, anchor) against the gt box, and BCE-with-logits (1 - t) x - log sigmoid(x) of the
+ * centre-ness logit x against t = sqrt(min(l, r) / max(l, r) * min(t, b) / max(t, b)) of encode(anchor, gt); decode, encode
+ * and the GIoU restated op by op in fp32, so every branch (overlap, min / max) is the reference's fp32 decision.
+ * Backward: s = fl(g * fl(1 / max(1, n))), g read from device memory, times each element's derivative; the GIoU gradient is
+ * analytic through the decode, with torch.max / torch.min's tie rule (equal operands get half the gradient each), and the
+ * centre-ness gradient s (sigmoid(x) - t).  Non-foreground rows are exactly 0; a null grad_box or grad_ctrness (not both)
+ * counts as a zero gradient: its rows are 0.  Every sum is in a fixed order, no floating-point atomics: results are bit-reproducible.
+ * workspace: the query's bytes, a function of (B, A) only.  Per VB200_LOSS_MAX_IMAGES images one kernel launch, plus one
+ * finalize launch per forward.  A * C (A * 4) must be below 2^31.  Asynchronous. */
+typedef struct vb200_fcos_loss_image {
+  const float* pred;
+  const float* ctrness;        /* box call only */
+  const int64_t* matched;
+  const int64_t* labels;
+  const float* gt;             /* box call only */
+  const float* anchors;        /* box call only */
+  float* grad;                 /* backward only */
+  float* grad_ctrness;         /* box backward only */
+  int64_t ctrness_stride, matched_stride, label_stride, gt_stride[2], anchor_stride[2];
+  int64_t num_gt;
+} vb200_fcos_loss_image;
+VB200_API size_t vb200_fcos_cls_loss_workspace_bytes(int num_images, int64_t num_anchors);
+VB200_API int vb200_fcos_cls_loss(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int num_classes, float* loss,
+                                  int64_t* num_foreground, void* workspace, size_t workspace_bytes, vb200_stream stream);
+VB200_API int vb200_fcos_cls_loss_backward(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int num_classes,
+                                           const float* grad_loss, const int64_t* num_foreground, vb200_stream stream);
+/* normalize_by_size: the BoxLinearCoder's flag (nonzero: the codes are relative to the anchor's width and height) */
+VB200_API size_t vb200_fcos_box_loss_workspace_bytes(int num_images, int64_t num_anchors);
+VB200_API int vb200_fcos_box_loss(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int normalize_by_size,
+                                  float* loss_box, float* loss_ctrness, int64_t* num_foreground, void* workspace,
+                                  size_t workspace_bytes, vb200_stream stream);
+VB200_API int vb200_fcos_box_loss_backward(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors,
+                                           int normalize_by_size, const float* grad_box, const float* grad_ctrness,
+                                           const int64_t* num_foreground, vb200_stream stream);
+
 /* ---- deform_conv2d -----------------------------------------------------
  * Replaces deform_conv2d_forward_kernel, csrc/ops/cuda/deform_conv2d_kernel.cu:1035-1255
  * (schema torchvision::deform_conv2d, csrc/ops/deform_conv2d.cpp:101-102).

@@ -12,7 +12,9 @@
     python tools/prof_ops.py fcos [iters]     fused vs. reference FCOS.compute_loss matching, batch 2, 8 and 16, 7 and 50
                              gt boxes per image
     python tools/prof_ops.py retinanet_loss [iters]     fused vs. reference RetinaNet head losses, forward + backward,
-                             batch 2 and 8, 7 and 50 gt boxes per image"""
+                             batch 2 and 8, 7 and 50 gt boxes per image
+    python tools/prof_ops.py fcos_loss [iters]     fused vs. reference FCOSHead.compute_loss, forward + backward, batch 2,
+                             8 and 16, 7 and 50 gt boxes per image"""
 import os
 import sys
 
@@ -501,6 +503,119 @@ def retinanet_loss(iters: int) -> None:
                 print(f"    {name:9s} wall {wall:.3f} ms per step, kernels {kern:.3f} ms ({top}), peak +{peak:.0f} MiB")
 
 
+def fcos_loss(iters: int) -> None:
+    """FCOSHead.compute_loss, forward + backward of its three losses, on FCOS's 18,134 anchors of an 800 x 1088 batch with
+    C = 91, batch 2, 8 and 16, M in {7, 50} gt boxes per image, matches from the fused FCOS matcher (bit-identical to the
+    reference's): the fused method against the uninstalled one on the same inputs.  Wall time per step ending in a
+    synchronize (median), GPU kernel time per step from torch.profiler (a separate run), the peak-memory delta over the step
+    and the HBM bound of the fused step computed from the shapes (the logits read once forward, read once and their gradient
+    written once backward; per anchor its match read by each of the four kernels, its anchor, regression and centre-ness
+    read forward and backward and their gradients written; at the data-sheet 3.35 TB/s)."""
+    import re
+    import subprocess
+    import time
+
+    from torch.profiler import ProfilerActivity, profile
+    from torchvision.models.detection import fcos
+    from torchvision.models.detection.anchor_utils import AnchorGenerator
+    from torchvision.models.detection.image_list import ImageList
+
+    from vision_b200 import detection as det
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+    print(f"fcos_loss: {gpu.strip().splitlines()[0] if gpu.strip() else 'unknown GPU'}")
+    C = 91
+    head = fcos.FCOSHead(256, 1, C).to(dev)
+    strides = (8, 16, 32, 64, 128)
+
+    def timed(fn, n):
+        for _ in range(2):
+            fn()
+        torch.cuda.synchronize()
+        wall = []
+        for _ in range(n):
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            wall.append(time.perf_counter() - t0)
+        return sorted(wall)[n // 2] * 1e3
+
+    def kernel_ms(fn, n):
+        fn()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(n):
+                fn()
+            torch.cuda.synchronize()
+        events = [e for e in prof.key_averages() if e.device_type == torch.autograd.DeviceType.CUDA]
+        total = sum(e.self_device_time_total for e in events) / n / 1e3
+        top = sorted(events, key=lambda e: -e.self_device_time_total)[:4]
+        short = lambda k: re.sub(r"^void |vb200::|\(anonymous namespace\)::|at::native::|\(.*$", "", k)[:48]  # noqa: E731
+        return total, ", ".join(f"{short(e.key)} {e.self_device_time_total / n / 1e3:.3f}" for e in top)
+
+    def peak_mb(fn, clear):
+        clear()
+        torch.cuda.synchronize()
+        base = torch.cuda.memory_allocated()
+        torch.cuda.reset_peak_memory_stats()
+        fn()
+        torch.cuda.synchronize()
+        return (torch.cuda.max_memory_allocated() - base) / 2**20
+
+    for batch in (2, 8, 16):
+        gen = AnchorGenerator(tuple((s,) for s in strides), ((1.0,),) * len(strides))       # FCOS's own generator
+        il = ImageList(torch.empty(batch, 3, 800, 1088, device=dev), [(800, 1088)] * batch)
+        feats = [torch.empty(batch, 1, -(-800 // s), -(-1088 // s), device=dev) for s in strides]
+        anchors = gen(il, feats)
+        levels = [f.shape[2] * f.shape[3] for f in feats]
+        A = anchors[0].shape[0]
+        for M in (7, 50):
+            g = torch.Generator(device=dev).manual_seed(M)
+            targets = []
+            for _ in range(batch):
+                xy = torch.rand(M, 2, generator=g, device=dev) * torch.tensor([900.0, 650.0], device=dev)
+                boxes = torch.cat([xy, xy + torch.rand(M, 2, generator=g, device=dev) * 300 + 8], 1)
+                targets.append({"boxes": boxes, "labels": torch.randint(1, C, (M,), generator=g, device=dev)})
+            matched = det.fcos_match_op([t["boxes"] for t in targets], anchors, 1.5, levels)
+            outputs = {"cls_logits": torch.randn(batch, A, C, generator=g, device=dev) - 4.595,
+                       "bbox_regression": torch.rand(batch, A, 4, generator=g, device=dev) * 3,
+                       "bbox_ctrness": torch.randn(batch, A, 1, generator=g, device=dev)}
+            for v in outputs.values():
+                v.requires_grad_(True)
+
+            def clear():
+                for v in outputs.values():
+                    v.grad = None
+
+            def step():
+                clear()
+                losses = head.compute_loss(targets, outputs, anchors, matched)
+                sum(losses.values()).backward()
+                return {k: v.detach() for k, v in losses.items()}
+
+            rows = {}
+            for name in ("reference", "fused"):
+                if name == "fused":
+                    vb.install()
+                try:
+                    losses = step()
+                    rows[name] = (losses, {k: v.grad.clone() for k, v in outputs.items()}, timed(step, iters), kernel_ms(step, 5),
+                                  peak_mb(step, clear))
+                finally:
+                    vb.uninstall()
+            bound_us = batch * A * (C * 4 * 3 + 4 * 8 + 2 * (16 + 16 + 4) + 16 + 4) / 3.35e12 * 1e6
+            (l0, g0, *_), (l1, g1, *_) = rows["reference"], rows["fused"]
+            rel = ", ".join(f"{k} {abs(l1[k].item() - l0[k].item()) / abs(l0[k].item()):.1e}" for k in l0)
+            grads = ", ".join(f"{k} {((g1[k] - g0[k]).abs().max() / g0[k].abs().max()).item():.1e}" for k in g0)
+            print(f"  batch {batch}, M {M} ({A} anchors per image, {int(sum((m >= 0).sum() for m in matched))} foreground): "
+                  f"HBM bound of the fused step {bound_us:.0f} us; loss rel. diff {rel}; max |d grad| / max |grad| {grads}")
+            for name, (_, _, wall, (kern, top), peak) in rows.items():
+                print(f"    {name:9s} wall {wall:.3f} ms per step, kernels {kern:.3f} ms ({top}), peak +{peak:.0f} MiB")
+
+
+if op == "fcos_loss":
+    fcos_loss(iters)
+    raise SystemExit(0)
 if op == "retinanet_loss":
     retinanet_loss(iters)
     raise SystemExit(0)

@@ -2,7 +2,8 @@
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py matching     (the box-matching kernels: memcheck only)
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py fcos         (the FCOS matching kernel: memcheck only)
-    compute-sanitizer --tool memcheck python tools/sanitize_smoke.py retinanet_loss   (the head-loss kernels: memcheck only)
+    compute-sanitizer --tool memcheck python tools/sanitize_smoke.py retinanet_loss   (the RetinaNet and FCOS head-loss
+                                                                                       kernels: memcheck only)
 No numerics are checked here (tests/ does that); the point is out-of-bounds / hazard reports."""
 import os
 import sys
@@ -196,6 +197,11 @@ def retinanet_loss():
         anchors = [boxes(A).t().contiguous().t() for _ in range(B)]
         (det.retinanet_cls_loss_op(logits, matched, labels) + det.retinanet_box_loss_op(regression, anchors, gts, matched,
                                                                                          [1.0, 1.0, 1.0, 1.0])).backward()
+        # FCOS's calls on the same inputs, with a strided centre-ness view and matches into an image without gt
+        ctrness = torch.randn(B, A, 2, device=dev)[..., :1].requires_grad_(True)
+        for normalize in (True, False):
+            loss_box, loss_ctr = det.fcos_box_loss_op(regression, ctrness, anchors, gts, labels, matched, normalize)
+            (det.fcos_cls_loss_op(logits, matched, labels) + loss_box + loss_ctr).backward()
 
 
 for name, fn in (("roi", roi), ("bwd", bwd), ("nms", nms), ("resize", resize), ("dcn", dcn), ("gather", gather), ("matching", matching),

@@ -234,6 +234,54 @@ def register() -> None:
     def _(grad, bbox_regression, anchors, gt_boxes, matched_idxs, weights, num_foreground):
         return bbox_regression.new_empty(bbox_regression.shape)
 
+    # ---- FCOS head losses: cls_logits, bbox_regression and bbox_ctrness are the only differentiable inputs; the count is
+    # not.  The box op's two losses share one backward, which takes both incoming gradients ----
+    def fcos_cls_setup(ctx, inputs, output):
+        logits, matched, labels = inputs
+        ctx.mark_non_differentiable(output[1])
+        ctx.save_for_backward(logits, output[1])
+        ctx.lists = (list(matched), list(labels))
+
+    def fcos_cls_backward(ctx, grad, _grad_count):
+        logits, count = ctx.saved_tensors
+        matched, labels = ctx.lists
+        return ops.fcos_cls_loss_backward(grad, logits, matched, labels, count), [None] * len(matched), [None] * len(labels)
+
+    lib.register_autograd("vision_b200::fcos_cls_loss", fcos_cls_backward, setup_context=fcos_cls_setup)
+
+    def fcos_box_setup(ctx, inputs, output):
+        regression, ctrness, anchors, gt_boxes, labels, matched, normalize = inputs
+        ctx.mark_non_differentiable(output[2])
+        ctx.save_for_backward(regression, ctrness, output[2])
+        ctx.lists = (list(anchors), list(gt_boxes), list(labels), list(matched))
+        ctx.normalize = normalize
+
+    def fcos_box_backward(ctx, grad_box, grad_ctrness, _grad_count):
+        regression, ctrness, count = ctx.saved_tensors
+        anchors, gt_boxes, labels, matched = ctx.lists
+        g_reg, g_ctr = ops.fcos_box_loss_backward(grad_box, grad_ctrness, regression, ctrness, anchors, gt_boxes, labels, matched,
+                                                  ctx.normalize, count)
+        return g_reg, g_ctr, [None] * len(anchors), [None] * len(gt_boxes), [None] * len(labels), [None] * len(matched), None
+
+    lib.register_autograd("vision_b200::fcos_box_loss", fcos_box_backward, setup_context=fcos_box_setup)
+
+    @lib.register_fake("vision_b200::fcos_cls_loss")
+    def _(cls_logits, matched_idxs, labels):
+        return cls_logits.new_empty(()), cls_logits.new_empty((), dtype=torch.int64)
+
+    @lib.register_fake("vision_b200::fcos_cls_loss_backward")
+    def _(grad, cls_logits, matched_idxs, labels, num_foreground):
+        return cls_logits.new_empty(cls_logits.shape)
+
+    @lib.register_fake("vision_b200::fcos_box_loss")
+    def _(bbox_regression, bbox_ctrness, anchors, gt_boxes, labels, matched_idxs, normalize_by_size):
+        return bbox_regression.new_empty(()), bbox_regression.new_empty(()), bbox_regression.new_empty((), dtype=torch.int64)
+
+    @lib.register_fake("vision_b200::fcos_box_loss_backward")
+    def _(grad_box, grad_ctrness, bbox_regression, bbox_ctrness, anchors, gt_boxes, labels, matched_idxs, normalize_by_size,
+          num_foreground):
+        return bbox_regression.new_empty(bbox_regression.shape), bbox_ctrness.new_empty(bbox_ctrness.shape)
+
     # ---- deform_conv2d ----
     def dcn_setup(ctx, inputs, output):
         inp, weight, offset, mask, bias = inputs[:5]

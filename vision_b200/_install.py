@@ -22,7 +22,8 @@
    ``RetinaNet.compute_loss`` are rebound on their classes; the per-image box_iou + Matcher loop becomes one call.
    ``FCOS.compute_loss`` likewise: its per-image centre-sampling loop becomes one call.
    Head losses: ``RetinaNetClassificationHead.compute_loss`` and ``RetinaNetRegressionHead.compute_loss`` are rebound on
-   their classes; each per-image loss loop becomes one call with a fused backward.
+   their classes; each per-image loss loop becomes one call with a fused backward.  ``FCOSHead.compute_loss`` likewise:
+   its three losses become two calls, each with a fused backward.
 5. ``resize`` has no torchvision kernel (transforms/v2/functional/_geometry.py:283-362 calls
    F.interpolate): the entries of ``_KERNEL_REGISTRY[resize]`` for Tensor / Image / Video are swapped.
 CPU tensors and unsupported dtypes/modes keep flowing to the reference implementation.
@@ -169,6 +170,16 @@ def install() -> None:
         losses[(cls, "compute_loss")] = orig
         cls.compute_loss = fused
 
+    # ---- FCOS head loss (fcos.py:52-125): bound on FCOSHead; FCOS.compute_loss (its matching fused above) calls it ----
+    orig_fcos_head_loss = tv_fcos.FCOSHead.compute_loss
+
+    @functools.wraps(orig_fcos_head_loss)
+    def fcos_head_loss(self, targets, head_outputs, anchors, matched_idxs):
+        return _det.fcos_head_compute_loss(self, targets, head_outputs, anchors, matched_idxs, _orig=orig_fcos_head_loss)
+
+    tv_fcos.FCOSHead.compute_loss = fcos_head_loss
+    fcos_losses = {(tv_fcos.FCOSHead, "compute_loss"): orig_fcos_head_loss}
+
     # ---- detection model inputs and outputs (transform.py:119-158, 257-277): bound on the class, so every model's
     # self.transform (Faster / Mask / Keypoint R-CNN, RetinaNet, FCOS, SSD, SSDLite) picks them up ----
     from torchvision.models.detection import transform as tv_transform
@@ -237,7 +248,7 @@ def install() -> None:
                        tv_roi_align_mod=tv_roi_align_mod, orig_det_roi_align=orig_det_roi_align,
                        tv_roi_heads=tv_roi_heads, tv_rpn=tv_rpn, orig_pp=orig_pp, orig_fp=orig_fp, orig_kri=orig_kri, orig_h2k=orig_h2k,
                        tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage, matching=matching, losses=losses,
-                       rcnn_transform=rcnn_transform, orig_tf_forward=orig_tf_forward, orig_tf_post=orig_tf_post))
+                       fcos_losses=fcos_losses, rcnn_transform=rcnn_transform, orig_tf_forward=orig_tf_forward, orig_tf_post=orig_tf_post))
 
 
 def uninstall() -> None:
@@ -257,7 +268,7 @@ def uninstall() -> None:
     _state["rcnn_transform"].postprocess = _state["orig_tf_post"]
     for cls, orig in _state["single_stage"].items():
         cls.postprocess_detections = orig
-    for (cls, name), orig in list(_state["matching"].items()) + list(_state["losses"].items()):
+    for (cls, name), orig in list(_state["matching"].items()) + list(_state["losses"].items()) + list(_state["fcos_losses"].items()):
         setattr(cls, name, orig)
     reg = _state["registry"]
     reg.clear()

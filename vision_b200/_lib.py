@@ -87,5 +87,6 @@ ABI_SYMBOLS = (
     "vb200_rcnn_batch_images", "vb200_rcnn_rescale", "vb200_match_boxes_workspace_bytes", "vb200_match_boxes",
     "vb200_fcos_level_bounds", "vb200_fcos_match", "vb200_retinanet_cls_loss_workspace_bytes", "vb200_retinanet_cls_loss",
     "vb200_retinanet_cls_loss_backward", "vb200_retinanet_box_loss_workspace_bytes", "vb200_retinanet_box_loss",
-    "vb200_retinanet_box_loss_backward",
+    "vb200_retinanet_box_loss_backward", "vb200_fcos_cls_loss_workspace_bytes", "vb200_fcos_cls_loss", "vb200_fcos_cls_loss_backward",
+    "vb200_fcos_box_loss_workspace_bytes", "vb200_fcos_box_loss", "vb200_fcos_box_loss_backward",
 )

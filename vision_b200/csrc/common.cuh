@@ -105,6 +105,10 @@ __device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigne
   return pack2(__fmaf_rn(lo32(a), lo32(b), lo32(c)), __fmaf_rn(hi32(a), hi32(b), hi32(c)));
 }
 
+// torch.maximum / torch.minimum: a NaN in either operand is the result
+template <typename A> __device__ __forceinline__ A nan_max(A a, A b) { return a != a ? a : b != b ? b : (a > b ? a : b); }
+template <typename A> __device__ __forceinline__ A nan_min(A a, A b) { return a != a ? a : b != b ? b : (a < b ? a : b); }
+
 __host__ __device__ inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 

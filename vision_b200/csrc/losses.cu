@@ -1,17 +1,17 @@
-// losses.cu — RetinaNet's head losses (torchvision/models/detection/retinanet.py:158-189 and 272-302), forward and backward,
-// sm_90a.
+// losses.cu — the single-stage detectors' head losses, forward and backward, sm_90a: RetinaNet's
+// (torchvision/models/detection/retinanet.py:158-189 and 272-302) and FCOS's (fcos.py:52-125).
 //
 // The reference, per image: a full-size zeros_like target with the ones scattered in, boolean indexing of the logits and the
 // target (a nonzero, a host sync), sigmoid_focal_loss (ops/focal_loss.py:41-56) as a chain of full-size elementwise kernels,
-// max(1, num_foreground) on a CUDA tensor (another sync); the regression head adds a torch.where sync and encode_single on the
-// gathered foreground rows.  Autograd keeps the full-size intermediates for a backward of the same shape.  Here every image of a
-// call is one grid layer of (tile of kLossTile anchors, image):
+// max(1, num_foreground) on a CUDA tensor or a .item() (another sync); the box terms add more syncs and chains of small
+// kernels over the gathered foreground rows.  Autograd keeps the full-size intermediates for a backward of the same shape.
+// Here every image of a call is one grid layer of (tile of kLossTile anchors, image):
 //   forward   each CTA stages its anchors' codes (target class, background, ignored or bad) in shared memory, streams its
 //             anchors' logits once with 16-byte loads and writes one partial sum and foreground count to a per-(image, tile)
-//             slot; the box loss does the same per foreground anchor with the reference's encode_single restated op by op.
-//   finalize  one CTA adds each image's partials in a fixed order, divides as the reference does and adds the images in
-//             _sum's order.
-//   backward  the dense gradient written exactly once: the analytic derivative times each image's scale, 0 where the
+//             slot; the box losses do the same per foreground anchor with the reference's box arithmetic restated op by op.
+//   finalize  one CTA adds the partials in a fixed order and divides as the head does: per image then over the images
+//             (RetinaNet), or once for the whole batch (FCOS).
+//   backward  the dense gradient written exactly once: the analytic derivative times the head's scale, 0 where the
 //             reference's indexing leaves it 0.
 // No floating-point atomics and no launch parameter depends on the SM count, so every result is bit-reproducible run to run.
 #include "common.cuh"
@@ -20,36 +20,74 @@ namespace vb200 {
 namespace {
 
 constexpr int kLossThreads = 256;
-constexpr int kLossTile = 256;                      // anchors per CTA, both losses: one anchor per thread when staging
-static_assert(kLossThreads == kLossTile, "the code staging and the box loss give each thread one anchor");
+constexpr int kLossTile = 256;                      // anchors per CTA, every loss: one anchor per thread when staging
+static_assert(kLossThreads == kLossTile, "the code staging and the box losses give each thread one anchor");
 constexpr int kFinalizeThreads = 256;
 
 // anchor codes; a code >= 0 is the anchor's target class
-constexpr int kBad = -3;          // matched >= num_gt, or a label outside [-C, C): the reference raises, the loss is NaN
-constexpr int kIgnored = -2;      // matched == Matcher.BETWEEN_THRESHOLDS: no loss, zero gradient
+constexpr int kBad = -3;          // an index the reference cannot gather with (it raises): the loss is NaN
+constexpr int kIgnored = -2;      // RetinaNet's matched == Matcher.BETWEEN_THRESHOLDS: no loss, zero gradient
 constexpr int kBackground = -1;   // every class's target is 0
 
-struct LossPlan {
-  vb200_retinanet_loss_image img[VB200_LOSS_MAX_IMAGES];
+// How a head turns its sum into the loss (and so the backward's scale):
+//   kImageDiv    per image, a true division by max(1, n_i) (a CUDA tensor), the images summed, times fl(1 / B)
+//   kImageRecip  per image, the product with fl(1 / max(1, n_i)) (a Python int), the images summed, times fl(1 / B)
+//   kBatchRecip  once for the batch, the product with fl(1 / max(1, n)), n from .item()
+enum class Norm { kImageDiv, kImageRecip, kBatchRecip };
+
+template <class Image> struct LossPlan {
+  Image img[VB200_LOSS_MAX_IMAGES];
   int64_t num_anchors;
   int num_classes, tiles, first_image, num_images;     // img[0] is image first_image of the call's num_images
   double* partial;                                      // forward: [num_images, tiles]
+  double* partial2;                                     // FCOS box forward: the centre-ness partials, [num_images, tiles]
   int* tile_fg;                                         // forward: [num_images, tiles]
-  const float* grad_loss;                               // backward: the 0-dim incoming gradient
-  const int64_t* num_fg;                                // backward: the forward's per-image foreground counts
-  float weights[4];                                     // box loss: the coder's weights as fp32
+  const float* grad_loss;                               // backward: the 0-dim incoming gradient (FCOS box: of the GIoU loss)
+  const float* grad_loss2;                              // FCOS box backward: of the centre-ness loss
+  const int64_t* num_fg;                                // backward: the forward's foreground counts
+  float weights[4];                                     // RetinaNet box loss: the coder's weights as fp32
+  bool normalize;                                       // FCOS box loss: BoxLinearCoder.normalize_by_size
 };
 
-__device__ __forceinline__ int anchor_code(const vb200_retinanet_loss_image& d, int64_t a, int C, bool& fg) {
-  const int64_t m = d.matched[a * d.matched_stride];
-  fg = m >= 0;                                          // num_foreground counts matched >= 0, bad indices included
-  if (m == -2) return kIgnored;
+// RetinaNet: the Matcher's -2 is ignored; a label in [-C, 0) wraps as advanced indexing does.
+struct RetinaNetCls {
+  using Image = vb200_retinanet_loss_image;
+  static constexpr Norm kNorm = Norm::kImageDiv;
+  __device__ static __forceinline__ int code(const Image& d, int64_t a, int C, bool& fg) {
+    const int64_t m = d.matched[a * d.matched_stride];
+    fg = m >= 0;                                        // num_foreground counts matched >= 0, bad indices included
+    if (m == -2) return kIgnored;
+    if (m < 0) return kBackground;
+    if (m >= d.num_gt) return kBad;
+    const int64_t l = d.labels[m * d.label_stride];
+    if (l < -C || l >= C) return kBad;
+    return (int)(l < 0 ? l + C : l);
+  }
+};
+
+// FCOS (fcos.py:64-90): every negative match is background; an image without gt gives a match the class 0 of new_zeros; a
+// negative label is background (the mask is >= 0, nothing wraps).  `C` bounds the class: the box call passes INT64_MAX, as
+// its reference reads no class.  m is the match, for the box call's gt row.
+__device__ __forceinline__ int fcos_code(const vb200_fcos_loss_image& d, int64_t a, int64_t C, int64_t& m) {
+  m = d.matched[a * d.matched_stride];
   if (m < 0) return kBackground;
+  if (d.num_gt == 0) return 0;
   if (m >= d.num_gt) return kBad;
   const int64_t l = d.labels[m * d.label_stride];
-  if (l < -C || l >= C) return kBad;
-  return (int)(l < 0 ? l + C : l);                      // advanced indexing wraps negative labels
+  if (l < 0) return kBackground;
+  return l >= C ? kBad : (int)l;
 }
+
+struct FcosCls {
+  using Image = vb200_fcos_loss_image;
+  static constexpr Norm kNorm = Norm::kBatchRecip;
+  __device__ static __forceinline__ int code(const Image& d, int64_t a, int C, bool& fg) {
+    int64_t m;
+    const int c = fcos_code(d, a, C, m);
+    fg = c >= 0 || c == kBad;                           // the reference's mask is label >= 0, bad indices included
+    return c;
+  }
+};
 
 // Stable forms of one element's sigmoid focal loss (alpha 0.25, gamma 2) and its derivative.  With p = σ(x), q = σ(-x):
 // -log p = softplus(-x), -log(1 - p) = softplus(x), both max(±x, 0) + log1p(exp(-|x|)).  The two transcendentals are fp32
@@ -73,7 +111,7 @@ __device__ __forceinline__ double focal_loss(float x, bool pos) {
   return pos ? 0.25 * (s.q * s.q) * s.sp_neg : 0.75 * (s.p * s.p) * s.sp_pos;
 }
 
-// t = 1: α(1-p)²(2p·log p - (1-p));  t = 0: (1-α)p²(p - 2(1-p)·log(1-p)); times the image's scale, rounded once.  NaN for a
+// t = 1: α(1-p)²(2p·log p - (1-p));  t = 0: (1-α)p²(p - 2(1-p)·log(1-p)); times the head's scale, rounded once.  NaN for a
 // non-finite logit, as the reference's.
 __device__ __forceinline__ float focal_grad(float x, bool pos, float scale) {
   if (!isfinite(x)) return NAN;
@@ -98,23 +136,25 @@ __device__ __forceinline__ double block_sum(double v, double* scratch) {
 // ATen's division by a Python number on CUDA: a product with the number's fp32 reciprocal.
 __device__ __forceinline__ float reciprocal(float d) { return __fdiv_rn(1.f, d); }
 
-// The per-image scale of the backward, in the order autograd applies the two divisions: grad / len(targets) (a Python int),
-// then / max(1, num_foreground) -- a CUDA int64 tensor in the classification head (a true division), a Python int in the
-// regression head.
-template <bool kBox> __device__ __forceinline__ float image_scale(const LossPlan& plan, int image) {
-  const float g = __fmul_rn(*plan.grad_loss, reciprocal((float)plan.num_images));
-  const int64_t n = plan.num_fg[image];
-  const float d = (float)(n > 1 ? n : 1);
-  return kBox ? __fmul_rn(g, reciprocal(d)) : __fdiv_rn(g, d);
+__device__ __forceinline__ float max1(int64_t n) { return (float)(n > 1 ? n : 1); }
+
+// The backward's scale of an image's elements, in the order autograd applies the head's divisions to the incoming g: for
+// RetinaNet g / len(targets) (a Python int), then / max(1, num_foreground) -- a CUDA int64 tensor in the classification head
+// (a true division), a Python int in the regression head; for FCOS g / max(1, n), a Python int.
+template <Norm kNorm> __device__ __forceinline__ float loss_scale(const float* grad, const int64_t* num_fg, int num_images, int image) {
+  if (kNorm == Norm::kBatchRecip) return __fmul_rn(*grad, reciprocal(max1(num_fg[0])));
+  const float g = __fmul_rn(*grad, reciprocal((float)num_images));
+  const float d = max1(num_fg[image]);
+  return kNorm == Norm::kImageRecip ? __fmul_rn(g, reciprocal(d)) : __fdiv_rn(g, d);
 }
 
 // One CTA: kLossTile anchors of image blockIdx.y, all C classes.  The tile's elements [e0, e1) of the image's [A, C] block are
 // taken in 16-byte groups aligned on the streamed array (the logits forward, the gradient backward); the first and last groups
-// may be partial, since C need not be a multiple of 4.
-template <bool kBackward>
+// may be partial, since C need not be a multiple of 4.  Rule gives each anchor its code and the head's division.
+template <class Rule, bool kBackward>
 __global__ void __launch_bounds__(kLossThreads)
-focal_loss_kernel(const __grid_constant__ LossPlan plan) {
-  const vb200_retinanet_loss_image& d = plan.img[blockIdx.y];
+focal_loss_kernel(const __grid_constant__ LossPlan<typename Rule::Image> plan) {
+  const typename Rule::Image& d = plan.img[blockIdx.y];
   const int image = plan.first_image + (int)blockIdx.y;
   const int C = plan.num_classes;
   const int64_t a0 = (int64_t)blockIdx.x * kLossTile;
@@ -123,7 +163,7 @@ focal_loss_kernel(const __grid_constant__ LossPlan plan) {
   __shared__ double scratch[kLossThreads / 32];
 
   bool fg = false;
-  s_code[threadIdx.x] = threadIdx.x < na ? anchor_code(d, a0 + threadIdx.x, C, fg) : kIgnored;
+  s_code[threadIdx.x] = threadIdx.x < na ? Rule::code(d, a0 + threadIdx.x, C, fg) : kIgnored;
   const int tile_fg = __syncthreads_count(fg);          // also the barrier after the staging
 
   const int64_t e0 = a0 * C, e1 = (a0 + na) * C;
@@ -134,7 +174,7 @@ focal_loss_kernel(const __grid_constant__ LossPlan plan) {
   const bool vec_load = !kBackward || ((reinterpret_cast<uintptr_t>(x) ^ reinterpret_cast<uintptr_t>(out)) & 15) == 0;
   const int64_t g0 = e0 - pad;                          // first element of the first group
   const int groups = (int)((e1 - g0 + 3) >> 2);
-  const float scale = kBackward ? image_scale<false>(plan, image) : 0.f;
+  const float scale = kBackward ? loss_scale<Rule::kNorm>(plan.grad_loss, plan.num_fg, plan.num_images, image) : 0.f;
   double acc = 0.0;
 
   for (int gi = threadIdx.x; gi < groups; gi += kLossThreads) {
@@ -197,6 +237,105 @@ __device__ __forceinline__ void encode_box(const float* w, const float a[4], con
   t[3] = __fmul_rn(w[3], logf(__fdiv_rn(gh, eh)));
 }
 
+// BoxLinearCoder (models/detection/_utils.py:227-310), op by op in fp32 with nothing contracted.  decode: p = (cx - r0,
+// cy - r1, cx + r2, cy + r3) with r = rel · (w, h, w, h) when normalising, else rel; the same decode in fp64 (for the
+// gradient's values) and d p_j / d rel_j.  encode: the anchor centre's distances to the gt box's edges, / (w, h, w, h) when
+// normalising.
+__device__ __forceinline__ void linear_decode(const float rel[4], const float a[4], bool normalize, float p[4], double pd[4],
+                                              double dp_drel[4]) {
+  const float cx = __fmul_rn(0.5f, __fadd_rn(a[0], a[2])), cy = __fmul_rn(0.5f, __fadd_rn(a[1], a[3]));
+  const float w = __fsub_rn(a[2], a[0]), h = __fsub_rn(a[3], a[1]);
+  const double cxd = 0.5 * ((double)a[0] + a[2]), cyd = 0.5 * ((double)a[1] + a[3]);
+  const double wd = normalize ? (double)a[2] - a[0] : 1.0, hd = normalize ? (double)a[3] - a[1] : 1.0;
+  float r[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) r[j] = normalize ? __fmul_rn(rel[j], j & 1 ? h : w) : rel[j];
+  p[0] = __fsub_rn(cx, r[0]);
+  p[1] = __fsub_rn(cy, r[1]);
+  p[2] = __fadd_rn(cx, r[2]);
+  p[3] = __fadd_rn(cy, r[3]);
+  pd[0] = cxd - rel[0] * wd;
+  pd[1] = cyd - rel[1] * hd;
+  pd[2] = cxd + rel[2] * wd;
+  pd[3] = cyd + rel[3] * hd;
+  dp_drel[0] = -wd;
+  dp_drel[1] = -hd;
+  dp_drel[2] = wd;
+  dp_drel[3] = hd;
+}
+
+__device__ __forceinline__ void linear_encode(const float a[4], const float g[4], bool normalize, float t[4]) {
+  const float cx = __fmul_rn(0.5f, __fadd_rn(a[0], a[2])), cy = __fmul_rn(0.5f, __fadd_rn(a[1], a[3]));
+  t[0] = __fsub_rn(cx, g[0]);
+  t[1] = __fsub_rn(cy, g[1]);
+  t[2] = __fsub_rn(g[2], cx);
+  t[3] = __fsub_rn(g[3], cy);
+  if (normalize) {
+    const float w = __fsub_rn(a[2], a[0]), h = __fsub_rn(a[3], a[1]);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) t[j] = __fdiv_rn(t[j], j & 1 ? h : w);
+  }
+}
+
+constexpr float kGiouEps = 1e-7f;                       // generalized_box_iou_loss's eps, as a fp32 tensor op rounds it
+
+// generalized_box_iou_loss (ops/giou_loss.py) with _loss_inter_union (ops/_utils.py:87-105) for one box p against its gt g,
+// op by op in fp32: the intersection only where (yk2 > yk1) & (xk2 > xk1) (strict, so NaN fails), else exactly 0;
+// union = (a1 + a2) - inter; loss = 1 - (iou - (area_c - union) / (area_c + eps)).
+__device__ __forceinline__ float giou_loss(const float p[4], const float g[4]) {
+  const float xk1 = nan_max(p[0], g[0]), yk1 = nan_max(p[1], g[1]), xk2 = nan_min(p[2], g[2]), yk2 = nan_min(p[3], g[3]);
+  const float inter = yk2 > yk1 && xk2 > xk1 ? __fmul_rn(__fsub_rn(xk2, xk1), __fsub_rn(yk2, yk1)) : 0.f;
+  const float a1 = __fmul_rn(__fsub_rn(p[2], p[0]), __fsub_rn(p[3], p[1]));
+  const float a2 = __fmul_rn(__fsub_rn(g[2], g[0]), __fsub_rn(g[3], g[1]));
+  const float uni = __fsub_rn(__fadd_rn(a1, a2), inter);
+  const float iou = __fdiv_rn(inter, __fadd_rn(uni, kGiouEps));
+  const float xc1 = nan_min(p[0], g[0]), yc1 = nan_min(p[1], g[1]), xc2 = nan_max(p[2], g[2]), yc2 = nan_max(p[3], g[3]);
+  const float area_c = __fmul_rn(__fsub_rn(xc2, xc1), __fsub_rn(yc2, yc1));
+  return __fsub_rn(1.f, __fsub_rn(iou, __fdiv_rn(__fsub_rn(area_c, uni), __fadd_rn(area_c, kGiouEps))));
+}
+
+// autograd's share of torch.max(p, g) / torch.min(p, g) for p: half where they are equal, none where the other side wins
+__device__ __forceinline__ double max_share(float p, float g) { return p == g ? 0.5 : p < g ? 0.0 : 1.0; }
+__device__ __forceinline__ double min_share(float p, float g) { return p == g ? 0.5 : p > g ? 0.0 : 1.0; }
+
+// d giou_loss / d p.  Every branch -- the overlap mask and which side of each min / max wins -- is the fp32 forward's
+// decision on p; the values are fp64, from pd (p's fp64 decode).  With U = union + eps, C = area_c + eps, I = inter:
+// dL/dI = -1/U - I/U² + 1/C, dL/d a1 = I/U² - 1/C, dL/d area_c = U/C².
+__device__ __forceinline__ void giou_grad(const float p[4], const double pd[4], const float g[4], double dl[4]) {
+  const bool overlap = nan_min(p[3], g[3]) > nan_max(p[1], g[1]) && nan_min(p[2], g[2]) > nan_max(p[0], g[0]);
+  double gd[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) gd[j] = g[j];
+  const double iw = nan_min(pd[2], gd[2]) - nan_max(pd[0], gd[0]), ih = nan_min(pd[3], gd[3]) - nan_max(pd[1], gd[1]);
+  const double I = overlap ? iw * ih : 0.0;
+  const double pw = pd[2] - pd[0], ph = pd[3] - pd[1];
+  const double U = pw * ph + (gd[2] - gd[0]) * (gd[3] - gd[1]) - I + (double)kGiouEps;
+  const double cw = nan_max(pd[2], gd[2]) - nan_min(pd[0], gd[0]), ch = nan_max(pd[3], gd[3]) - nan_min(pd[1], gd[1]);
+  const double C = cw * ch + (double)kGiouEps;
+  const double d_a1 = I / (U * U) - 1.0 / C, d_c = U / (C * C);
+  dl[0] = -d_a1 * ph - d_c * ch * min_share(p[0], g[0]);
+  dl[1] = -d_a1 * pw - d_c * cw * min_share(p[1], g[1]);
+  dl[2] = d_a1 * ph + d_c * ch * max_share(p[2], g[2]);
+  dl[3] = d_a1 * pw + d_c * cw * max_share(p[3], g[3]);
+  if (overlap) {
+    const double d_i = -1.0 / U - I / (U * U) + 1.0 / C;
+    dl[0] -= d_i * ih * max_share(p[0], g[0]);
+    dl[1] -= d_i * iw * max_share(p[1], g[1]);
+    dl[2] += d_i * ih * min_share(p[2], g[2]);
+    dl[3] += d_i * iw * min_share(p[3], g[3]);
+  }
+}
+
+// The centre-ness target (fcos.py:105-115): sqrt(min(l, r) / max(l, r) · min(t, b) / max(t, b)) of encode(anchor, gt), with
+// the NaN-propagating min and max of Tensor.min / .max(dim).
+__device__ __forceinline__ float ctrness_target(const float a[4], const float g[4], bool normalize) {
+  float t[4];
+  linear_encode(a, g, normalize, t);
+  const float lr = __fdiv_rn(nan_min(t[0], t[2]), nan_max(t[0], t[2]));
+  const float tb = __fdiv_rn(nan_min(t[1], t[3]), nan_max(t[1], t[3]));
+  return __fsqrt_rn(__fmul_rn(lr, tb));
+}
+
 __device__ __forceinline__ void load_row(const float* base, int64_t row, const int64_t* stride, float v[4]) {
 #pragma unroll
   for (int j = 0; j < 4; ++j) v[j] = base[row * stride[0] + j * stride[1]];
@@ -208,7 +347,7 @@ __device__ __forceinline__ float sign_of(float v) { return (float)((0.f < v) - (
 // One CTA: kLossTile anchors of image blockIdx.y, one per thread.  Only foreground anchors read their regression row.
 template <bool kBackward>
 __global__ void __launch_bounds__(kLossThreads)
-box_loss_kernel(const __grid_constant__ LossPlan plan) {
+box_loss_kernel(const __grid_constant__ LossPlan<vb200_retinanet_loss_image> plan) {
   const vb200_retinanet_loss_image& d = plan.img[blockIdx.y];
   const int image = plan.first_image + (int)blockIdx.y;
   const int64_t a = (int64_t)blockIdx.x * kLossTile + threadIdx.x;
@@ -231,7 +370,7 @@ box_loss_kernel(const __grid_constant__ LossPlan plan) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) pv[j] = d.pred[a * 4 + j];
       if (kBackward) {
-        const float scale = image_scale<true>(plan, image);
+        const float scale = loss_scale<Norm::kImageRecip>(plan.grad_loss, plan.num_fg, plan.num_images, image);
 #pragma unroll
         for (int j = 0; j < 4; ++j) gout[j] = scale * sign_of(__fsub_rn(pv[j], t[j]));
       } else {
@@ -252,39 +391,120 @@ box_loss_kernel(const __grid_constant__ LossPlan plan) {
   }
 }
 
-// Per image: the partials in a fixed order, / max(1, n_fg) as the head divides (true division in the classification head,
-// the reciprocal product in the regression head); then ((L0 + L1) + L2) ... as _sum adds them, times the fp32 reciprocal of
-// len(targets).
-template <bool kBox>
+// FCOS's GIoU and centre-ness losses.  One CTA: kLossTile anchors of image blockIdx.y, one per thread; only foreground
+// anchors read their regression row, centre-ness logit, anchor and gt box (the zero box for an image without gt).  The
+// centre-ness term is binary_cross_entropy_with_logits, (1 - t) x - log σ(x) with -log σ(x) = softplus(-x) in the focal
+// loss's stable form; its derivative σ(x) - t.
+template <bool kBackward>
+__global__ void __launch_bounds__(kLossThreads)
+fcos_box_loss_kernel(const __grid_constant__ LossPlan<vb200_fcos_loss_image> plan) {
+  const vb200_fcos_loss_image& d = plan.img[blockIdx.y];
+  const int image = plan.first_image + (int)blockIdx.y;
+  const int64_t a = (int64_t)blockIdx.x * kLossTile + threadIdx.x;
+  const bool valid = a < plan.num_anchors;
+  int64_t m = -1;
+  const int code = valid ? fcos_code(d, a, INT64_MAX, m) : kBackground;
+  const bool fg = code >= 0 || code == kBad;
+  __shared__ double scratch[kLossThreads / 32];
+  double giou = 0.0, bce = 0.0;
+  float gbox[4] = {0.f, 0.f, 0.f, 0.f}, gctr = 0.f;
+  if (code == kBad) {
+    giou = bce = (double)NAN;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) gbox[j] = NAN;
+    gctr = NAN;
+  } else if (fg) {
+    float an[4], gt[4] = {0.f, 0.f, 0.f, 0.f}, rel[4], p[4];
+    double pd[4], dp_drel[4];
+    load_row(d.anchors, a, d.anchor_stride, an);
+    if (d.num_gt > 0) load_row(d.gt, m, d.gt_stride, gt);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) rel[j] = d.pred[a * 4 + j];
+    const float x = d.ctrness[a * d.ctrness_stride];
+    const float t = ctrness_target(an, gt, plan.normalize);
+    linear_decode(rel, an, plan.normalize, p, pd, dp_drel);
+    if (kBackward) {
+      if (plan.grad_loss) {
+        const double s = loss_scale<Norm::kBatchRecip>(plan.grad_loss, plan.num_fg, plan.num_images, image);
+        double dl[4];
+        giou_grad(p, pd, gt, dl);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) gbox[j] = (float)(s * dl[j] * dp_drel[j]);
+      }
+      if (plan.grad_loss2) {
+        const double s = loss_scale<Norm::kBatchRecip>(plan.grad_loss2, plan.num_fg, plan.num_images, image);
+        gctr = (float)(s * (sig(x).p - (double)t));
+      }
+    } else {
+      giou = (double)giou_loss(p, gt);
+      bce = (1.0 - (double)t) * (double)x + sig(x).sp_neg;
+    }
+  }
+  if (kBackward) {
+    if (valid) {
+      *reinterpret_cast<float4*>(d.grad + a * 4) = make_float4(gbox[0], gbox[1], gbox[2], gbox[3]);
+      d.grad_ctrness[a] = gctr;
+    }
+  } else {
+    const int tile_fg = __syncthreads_count(fg);
+    const double sum = block_sum(giou, scratch);
+    const double sum2 = block_sum(bce, scratch);
+    if (threadIdx.x == 0) {
+      plan.partial[(int64_t)image * plan.tiles + blockIdx.x] = sum;
+      plan.partial2[(int64_t)image * plan.tiles + blockIdx.x] = sum2;
+      plan.tile_fg[(int64_t)image * plan.tiles + blockIdx.x] = tile_fg;
+    }
+  }
+}
+
+// Each image's partials and counts in a fixed order.  Per image (RetinaNet): / max(1, n_i) as the head divides, then
+// ((L0 + L1) + L2) ... as _sum adds them, times the fp32 reciprocal of len(targets); each image's count kept.  For the batch
+// (FCOS, launched as one image of all the batch's slots): the sum rounded to fp32 once, times fl(1 / max(1, n)); the batch's
+// count kept.  partial2 (may be null) gives loss2 the same way.
+template <Norm kNorm>
 __global__ void __launch_bounds__(kFinalizeThreads)
-loss_finalize_kernel(const double* __restrict__ partial, const int* __restrict__ tile_fg, int tiles, int num_images, float* loss,
-                     int64_t* num_fg) {
+loss_finalize_kernel(const double* __restrict__ partial, const double* __restrict__ partial2, const int* __restrict__ tile_fg,
+                     int tiles, int num_images, float* loss, float* loss2, int64_t* num_fg) {
   __shared__ double scratch[kFinalizeThreads / 32];
   float total = 0.f;
   for (int i = 0; i < num_images; ++i) {
-    double s = 0.0, n = 0.0;                           // counts below 2^53 are exact in a double
+    double s = 0.0, s2 = 0.0, n = 0.0;                 // counts below 2^53 are exact in a double
     for (int j = threadIdx.x; j < tiles; j += kFinalizeThreads) {
       s += partial[(int64_t)i * tiles + j];
+      if (partial2) s2 += partial2[(int64_t)i * tiles + j];
       n += (double)tile_fg[(int64_t)i * tiles + j];
     }
     s = block_sum(s, scratch);
+    if (partial2) s2 = block_sum(s2, scratch);
     n = block_sum(n, scratch);
     if (threadIdx.x == 0) {
       const int64_t count = (int64_t)n;
       num_fg[i] = count;
-      const float dv = (float)(count > 1 ? count : 1);
-      const float li = kBox ? __fmul_rn((float)s, reciprocal(dv)) : __fdiv_rn((float)s, dv);
-      total = i == 0 ? li : __fadd_rn(total, li);
+      if (kNorm == Norm::kBatchRecip) {
+        const float r = reciprocal(max1(count));
+        *loss = __fmul_rn((float)s, r);
+        if (loss2) *loss2 = __fmul_rn((float)s2, r);
+      } else {
+        const float dv = max1(count);
+        const float li = kNorm == Norm::kImageRecip ? __fmul_rn((float)s, reciprocal(dv)) : __fdiv_rn((float)s, dv);
+        total = i == 0 ? li : __fadd_rn(total, li);
+      }
     }
   }
-  if (threadIdx.x == 0) *loss = __fmul_rn(total, reciprocal((float)num_images));
+  if (kNorm != Norm::kBatchRecip && threadIdx.x == 0) *loss = __fmul_rn(total, reciprocal((float)num_images));
+}
+
+int check_sizes(const void* images, int num_images, int64_t num_anchors, int width, const char* op) {
+  VB200_REQUIRE(num_images >= 1 && images, "%s: at least one image", op);
+  VB200_REQUIRE(num_anchors >= 0 && width >= 1 && num_anchors * width < ((int64_t)1 << 31), "%s: bad sizes (%lld anchors, width %d)", op,
+                (long long)num_anchors, width);
+  return 0;
 }
 
 int check_call(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors, int width, bool box, bool backward,
                const char* op) {
-  VB200_REQUIRE(num_images >= 1 && images, "%s: at least one image", op);
-  VB200_REQUIRE(num_anchors >= 0 && width >= 1 && num_anchors * width < ((int64_t)1 << 31), "%s: bad sizes (%lld anchors, width %d)", op,
-                (long long)num_anchors, width);
+  const int rc = check_sizes(images, num_images, num_anchors, width, op);
+  if (rc) return rc;
   for (int i = 0; i < num_images; ++i) {
     const vb200_retinanet_loss_image& d = images[i];
     VB200_REQUIRE(d.num_gt >= 0, "%s: image %d: bad gt count", op, i);
@@ -297,17 +517,35 @@ int check_call(const vb200_retinanet_loss_image* images, int num_images, int64_t
   return 0;
 }
 
-template <bool kBox, bool kBackward>
-int launch_loss(LossPlan& plan, const vb200_retinanet_loss_image* images, int num_images, cudaStream_t st) {
+int check_call(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int width, bool box, bool backward,
+               const char* op) {
+  const int rc = check_sizes(images, num_images, num_anchors, width, op);
+  if (rc) return rc;
+  for (int i = 0; i < num_images; ++i) {
+    const vb200_fcos_loss_image& d = images[i];
+    VB200_REQUIRE(d.num_gt >= 0, "%s: image %d: bad gt count", op, i);
+    if (num_anchors == 0) continue;
+    VB200_REQUIRE(d.pred && d.matched && (!backward || d.grad) && (!box || (d.anchors && d.ctrness && (!backward || d.grad_ctrness))),
+                  "%s: image %d: null pointer", op, i);
+    VB200_REQUIRE(d.num_gt == 0 || (d.labels && (!box || d.gt)), "%s: image %d: null gt pointer", op, i);
+    VB200_REQUIRE(!box || !backward || (reinterpret_cast<uintptr_t>(d.grad) & 15) == 0, "%s: image %d: gradient rows must be 16-byte aligned",
+                  op, i);
+  }
+  return 0;
+}
+
+// One launch of `kernel` per VB200_LOSS_MAX_IMAGES images, each with its images' descriptors in the plan.
+template <class Image>
+int launch_loss(void (*kernel)(const LossPlan<Image>), const char* name, LossPlan<Image>& plan, const Image* images, int num_images,
+                cudaStream_t st) {
   if (plan.tiles == 0) return 0;
   for (int done = 0; done < num_images; done += VB200_LOSS_MAX_IMAGES) {
     const int chunk = num_images - done < VB200_LOSS_MAX_IMAGES ? num_images - done : VB200_LOSS_MAX_IMAGES;
     for (int i = 0; i < chunk; ++i) plan.img[i] = images[done + i];
     plan.first_image = done;
     const dim3 grid((unsigned)plan.tiles, (unsigned)chunk);
-    if (kBox) box_loss_kernel<kBackward><<<grid, kLossThreads, 0, st>>>(plan);
-    else focal_loss_kernel<kBackward><<<grid, kLossThreads, 0, st>>>(plan);
-    const int rc = check_launch(kBox ? "box_loss_kernel" : "focal_loss_kernel");
+    kernel<<<grid, kLossThreads, 0, st>>>(plan);
+    const int rc = check_launch(name);
     if (rc) return rc;
   }
   return 0;
@@ -315,58 +553,69 @@ int launch_loss(LossPlan& plan, const vb200_retinanet_loss_image* images, int nu
 
 int tiles_of(int64_t num_anchors) { return (int)ceil_div64(num_anchors, kLossTile); }
 
-size_t loss_workspace_bytes(int num_images, int64_t num_anchors) {
+// the per-(image, tile) partials of `terms` losses and the foreground counts
+size_t loss_workspace_bytes(int num_images, int64_t num_anchors, int terms) {
   if (num_images < 1 || num_anchors < 0) return 0;
   const size_t slots = (size_t)num_images * (size_t)tiles_of(num_anchors);
-  return align256(slots * sizeof(double)) + align256(slots * sizeof(int));
+  return terms * align256(slots * sizeof(double)) + align256(slots * sizeof(int));
 }
 
-template <bool kBox>
-int loss_forward(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors, int width, const float* weights,
-                 float* loss, int64_t* num_fg, void* workspace, size_t workspace_bytes, cudaStream_t st, const char* op) {
-  const int rc = check_call(images, num_images, num_anchors, width, kBox, false, op);
+template <class Image>
+LossPlan<Image> make_plan(int num_images, int64_t num_anchors, int width, const float* weights, bool normalize) {
+  LossPlan<Image> plan;
+  plan.num_anchors = num_anchors;
+  plan.num_classes = width;
+  plan.tiles = tiles_of(num_anchors);
+  plan.first_image = 0;
+  plan.num_images = num_images;
+  plan.partial = plan.partial2 = nullptr;
+  plan.tile_fg = nullptr;
+  plan.grad_loss = plan.grad_loss2 = nullptr;
+  plan.num_fg = nullptr;
+  for (int j = 0; j < 4; ++j) plan.weights[j] = weights ? weights[j] : 0.f;
+  plan.normalize = normalize;
+  return plan;
+}
+
+// The forward of one loss call: the partials of one loss (loss2 null) or two, then the finalize.
+template <Norm kNorm, class Image>
+int loss_forward(void (*kernel)(const LossPlan<Image>), const char* name, LossPlan<Image>& plan, const Image* images, int num_images,
+                 bool box, float* loss, float* loss2, int64_t* num_fg, void* workspace, size_t workspace_bytes, cudaStream_t st,
+                 const char* op) {
+  const int rc = check_call(images, num_images, plan.num_anchors, plan.num_classes, box, false, op);
   if (rc) return rc;
   VB200_REQUIRE(loss && num_fg, "%s: null outputs", op);
-  const size_t need = loss_workspace_bytes(num_images, num_anchors);
+  const int terms = loss2 ? 2 : 1;
+  const size_t need = loss_workspace_bytes(num_images, plan.num_anchors, terms);
   if (need && (!workspace || workspace_bytes < need)) {
     set_error("%s: workspace of %zu bytes, %zu needed", op, workspace_bytes, need);
     return VB200_EWORKSPACE;
   }
-  LossPlan plan;
-  plan.num_anchors = num_anchors;
-  plan.num_classes = width;
-  plan.tiles = tiles_of(num_anchors);
-  plan.num_images = num_images;
   Carver ws(workspace);
   plan.partial = ws.take<double>((size_t)num_images * plan.tiles);
+  if (loss2) plan.partial2 = ws.take<double>((size_t)num_images * plan.tiles);
   plan.tile_fg = ws.take<int>((size_t)num_images * plan.tiles);
-  plan.grad_loss = nullptr;
-  plan.num_fg = nullptr;
-  for (int j = 0; j < 4; ++j) plan.weights[j] = weights ? weights[j] : 0.f;
-  const int lrc = launch_loss<kBox, false>(plan, images, num_images, st);
+  const int lrc = launch_loss<Image>(kernel, name, plan, images, num_images, st);
   if (lrc) return lrc;
-  loss_finalize_kernel<kBox><<<1, kFinalizeThreads, 0, st>>>(plan.partial, plan.tile_fg, plan.tiles, num_images, loss, num_fg);
+  const bool batch = kNorm == Norm::kBatchRecip;      // the [num_images, tiles] slots as one image's
+  loss_finalize_kernel<kNorm><<<1, kFinalizeThreads, 0, st>>>(plan.partial, plan.partial2, plan.tile_fg,
+                                                              batch ? num_images * plan.tiles : plan.tiles, batch ? 1 : num_images,
+                                                              loss, loss2, num_fg);
   return check_launch("loss_finalize_kernel");
 }
 
-template <bool kBox>
-int loss_backward(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors, int width, const float* weights,
-                  const float* grad_loss, const int64_t* num_fg, cudaStream_t st, const char* op) {
-  const int rc = check_call(images, num_images, num_anchors, width, kBox, true, op);
+template <class Image>
+int loss_backward(void (*kernel)(const LossPlan<Image>), const char* name, LossPlan<Image>& plan, const Image* images, int num_images,
+                  bool box, const int64_t* num_fg, cudaStream_t st, const char* op) {
+  const int rc = check_call(images, num_images, plan.num_anchors, plan.num_classes, box, true, op);
   if (rc) return rc;
-  VB200_REQUIRE(grad_loss && num_fg, "%s: null gradient or counts", op);
-  LossPlan plan;
-  plan.num_anchors = num_anchors;
-  plan.num_classes = width;
-  plan.tiles = tiles_of(num_anchors);
-  plan.num_images = num_images;
-  plan.partial = nullptr;
-  plan.tile_fg = nullptr;
-  plan.grad_loss = grad_loss;
+  VB200_REQUIRE(num_fg && (plan.grad_loss || plan.grad_loss2), "%s: null gradient or counts", op);
   plan.num_fg = num_fg;
-  for (int j = 0; j < 4; ++j) plan.weights[j] = weights ? weights[j] : 0.f;
-  return launch_loss<kBox, true>(plan, images, num_images, st);
+  return launch_loss<Image>(kernel, name, plan, images, num_images, st);
 }
+
+using RetinaPlan = LossPlan<vb200_retinanet_loss_image>;
+using FcosPlan = LossPlan<vb200_fcos_loss_image>;
 
 }  // namespace
 }  // namespace vb200
@@ -374,39 +623,87 @@ int loss_backward(const vb200_retinanet_loss_image* images, int num_images, int6
 using namespace vb200;
 
 extern "C" size_t vb200_retinanet_cls_loss_workspace_bytes(int num_images, int64_t num_anchors) {
-  return loss_workspace_bytes(num_images, num_anchors);
+  return loss_workspace_bytes(num_images, num_anchors, 1);
 }
 
 extern "C" int vb200_retinanet_cls_loss(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors, int num_classes,
                                         float* loss, int64_t* num_foreground, void* workspace, size_t workspace_bytes,
                                         vb200_stream stream) {
-  return loss_forward<false>(images, num_images, num_anchors, num_classes, nullptr, loss, num_foreground, workspace, workspace_bytes,
-                             (cudaStream_t)stream, "retinanet_cls_loss");
+  RetinaPlan plan = make_plan<vb200_retinanet_loss_image>(num_images, num_anchors, num_classes, nullptr, false);
+  return loss_forward<Norm::kImageDiv>(focal_loss_kernel<RetinaNetCls, false>, "focal_loss_kernel", plan, images, num_images, false, loss,
+                                       nullptr, num_foreground, workspace, workspace_bytes, (cudaStream_t)stream, "retinanet_cls_loss");
 }
 
 extern "C" int vb200_retinanet_cls_loss_backward(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
                                                  int num_classes, const float* grad_loss, const int64_t* num_foreground,
                                                  vb200_stream stream) {
-  return loss_backward<false>(images, num_images, num_anchors, num_classes, nullptr, grad_loss, num_foreground, (cudaStream_t)stream,
-                              "retinanet_cls_loss_backward");
+  RetinaPlan plan = make_plan<vb200_retinanet_loss_image>(num_images, num_anchors, num_classes, nullptr, false);
+  plan.grad_loss = grad_loss;
+  return loss_backward(focal_loss_kernel<RetinaNetCls, true>, "focal_loss_kernel", plan, images, num_images, false, num_foreground,
+                       (cudaStream_t)stream, "retinanet_cls_loss_backward");
 }
 
 extern "C" size_t vb200_retinanet_box_loss_workspace_bytes(int num_images, int64_t num_anchors) {
-  return loss_workspace_bytes(num_images, num_anchors);
+  return loss_workspace_bytes(num_images, num_anchors, 1);
 }
 
 extern "C" int vb200_retinanet_box_loss(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
                                         const float* weights_host, float* loss, int64_t* num_foreground, void* workspace,
                                         size_t workspace_bytes, vb200_stream stream) {
   VB200_REQUIRE(weights_host, "retinanet_box_loss: null weights");
-  return loss_forward<true>(images, num_images, num_anchors, 4, weights_host, loss, num_foreground, workspace, workspace_bytes,
-                            (cudaStream_t)stream, "retinanet_box_loss");
+  RetinaPlan plan = make_plan<vb200_retinanet_loss_image>(num_images, num_anchors, 4, weights_host, false);
+  return loss_forward<Norm::kImageRecip>(box_loss_kernel<false>, "box_loss_kernel", plan, images, num_images, true, loss, nullptr,
+                                         num_foreground, workspace, workspace_bytes, (cudaStream_t)stream, "retinanet_box_loss");
 }
 
 extern "C" int vb200_retinanet_box_loss_backward(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
                                                  const float* weights_host, const float* grad_loss, const int64_t* num_foreground,
                                                  vb200_stream stream) {
   VB200_REQUIRE(weights_host, "retinanet_box_loss_backward: null weights");
-  return loss_backward<true>(images, num_images, num_anchors, 4, weights_host, grad_loss, num_foreground, (cudaStream_t)stream,
-                             "retinanet_box_loss_backward");
+  RetinaPlan plan = make_plan<vb200_retinanet_loss_image>(num_images, num_anchors, 4, weights_host, false);
+  plan.grad_loss = grad_loss;
+  return loss_backward(box_loss_kernel<true>, "box_loss_kernel", plan, images, num_images, true, num_foreground, (cudaStream_t)stream,
+                       "retinanet_box_loss_backward");
+}
+
+extern "C" size_t vb200_fcos_cls_loss_workspace_bytes(int num_images, int64_t num_anchors) {
+  return loss_workspace_bytes(num_images, num_anchors, 1);
+}
+
+extern "C" int vb200_fcos_cls_loss(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int num_classes, float* loss,
+                                   int64_t* num_foreground, void* workspace, size_t workspace_bytes, vb200_stream stream) {
+  FcosPlan plan = make_plan<vb200_fcos_loss_image>(num_images, num_anchors, num_classes, nullptr, false);
+  return loss_forward<Norm::kBatchRecip>(focal_loss_kernel<FcosCls, false>, "focal_loss_kernel", plan, images, num_images, false, loss,
+                                         nullptr, num_foreground, workspace, workspace_bytes, (cudaStream_t)stream, "fcos_cls_loss");
+}
+
+extern "C" int vb200_fcos_cls_loss_backward(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int num_classes,
+                                            const float* grad_loss, const int64_t* num_foreground, vb200_stream stream) {
+  FcosPlan plan = make_plan<vb200_fcos_loss_image>(num_images, num_anchors, num_classes, nullptr, false);
+  plan.grad_loss = grad_loss;
+  return loss_backward(focal_loss_kernel<FcosCls, true>, "focal_loss_kernel", plan, images, num_images, false, num_foreground,
+                       (cudaStream_t)stream, "fcos_cls_loss_backward");
+}
+
+extern "C" size_t vb200_fcos_box_loss_workspace_bytes(int num_images, int64_t num_anchors) {
+  return loss_workspace_bytes(num_images, num_anchors, 2);
+}
+
+extern "C" int vb200_fcos_box_loss(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int normalize_by_size,
+                                   float* loss_box, float* loss_ctrness, int64_t* num_foreground, void* workspace, size_t workspace_bytes,
+                                   vb200_stream stream) {
+  VB200_REQUIRE(loss_ctrness, "fcos_box_loss: null outputs");
+  FcosPlan plan = make_plan<vb200_fcos_loss_image>(num_images, num_anchors, 4, nullptr, normalize_by_size != 0);
+  return loss_forward<Norm::kBatchRecip>(fcos_box_loss_kernel<false>, "fcos_box_loss_kernel", plan, images, num_images, true, loss_box,
+                                         loss_ctrness, num_foreground, workspace, workspace_bytes, (cudaStream_t)stream, "fcos_box_loss");
+}
+
+extern "C" int vb200_fcos_box_loss_backward(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors,
+                                            int normalize_by_size, const float* grad_box, const float* grad_ctrness,
+                                            const int64_t* num_foreground, vb200_stream stream) {
+  FcosPlan plan = make_plan<vb200_fcos_loss_image>(num_images, num_anchors, 4, nullptr, normalize_by_size != 0);
+  plan.grad_loss = grad_box;
+  plan.grad_loss2 = grad_ctrness;
+  return loss_backward(fcos_box_loss_kernel<true>, "fcos_box_loss_kernel", plan, images, num_images, true, num_foreground,
+                       (cudaStream_t)stream, "fcos_box_loss_backward");
 }

@@ -65,9 +65,6 @@ __device__ __forceinline__ unsigned long long warp_max(unsigned long long k) {
   return k;
 }
 
-// torch.maximum / torch.minimum: a NaN in either operand is the result
-template <typename A> __device__ __forceinline__ A nan_max(A a, A b) { return a != a ? a : b != b ? b : (a > b ? a : b); }
-template <typename A> __device__ __forceinline__ A nan_min(A a, A b) { return a != a ? a : b != b ? b : (a < b ? a : b); }
 // clamp(min=0), which keeps a NaN
 template <typename A> __device__ __forceinline__ A clamp0(A v) { return v < A(0) ? A(0) : v; }
 

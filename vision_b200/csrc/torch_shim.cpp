@@ -1131,6 +1131,138 @@ at::Tensor retinanet_box_loss_backward(const at::Tensor& grad, const at::Tensor&
   return out;
 }
 
+// ---- FCOS head losses (fcos.py:52-125) ----------------------------------------------------------------------------------
+// cls_logits [B, A, C] / bbox_regression [B, A, 4] as loss_images takes them; bbox_ctrness (box call) fp32 [B, A, 1] on the
+// same GPU, any strides; labels one int64 [M_i] per image on that GPU (as many rows as the image's gt boxes in the box call).
+// Each forward returns its 0-dim losses and the batch's foreground count (int64, 0-dim) that its backward takes.
+std::vector<vb200_fcos_loss_image> fcos_loss_images(const at::Tensor& pred, int64_t width, const at::Tensor* ctrness, at::TensorList matched_idxs,
+                                                    at::TensorList labels, at::TensorList anchors, at::TensorList gt_boxes, const char* op) {
+  const bool box = ctrness != nullptr;
+  TORCH_CHECK(labels.size() == matched_idxs.size(), op, ": one labels tensor per image");
+  const auto base = loss_images(pred, width, matched_idxs, labels, anchors, gt_boxes, box, op);
+  const int64_t A = pred.size(1);
+  if (box)
+    TORCH_CHECK(ctrness->is_cuda() && ctrness->get_device() == pred.get_device() && ctrness->scalar_type() == at::kFloat && ctrness->dim() == 3 &&
+                    ctrness->size(0) == pred.size(0) && ctrness->size(1) == A && ctrness->size(2) == 1,
+                op, ": bbox_ctrness must be a float32 [B, A, 1] tensor on the predictions' GPU");
+  std::vector<vb200_fcos_loss_image> desc(base.size());
+  for (size_t i = 0; i < base.size(); ++i) {
+    const vb200_retinanet_loss_image& r = base[i];
+    vb200_fcos_loss_image& d = desc[i];
+    d = {};
+    d.pred = r.pred;
+    d.matched = r.matched;
+    d.matched_stride = r.matched_stride;
+    const at::Tensor& l = labels[i];
+    TORCH_CHECK(l.is_cuda() && l.get_device() == pred.get_device() && l.scalar_type() == at::kLong && l.dim() == 1 && (!box || l.size(0) == r.num_gt),
+                op, ": labels must be int64 [M] tensors on the predictions' GPU, one per gt box");
+    d.labels = l.data_ptr<int64_t>();
+    d.label_stride = l.stride(0);
+    d.num_gt = l.size(0);
+    if (box) {
+      d.ctrness = ctrness->data_ptr<float>() + (int64_t)i * ctrness->stride(0);
+      d.ctrness_stride = ctrness->stride(1);
+      d.gt = r.gt;
+      d.anchors = r.anchors;
+      for (int k = 0; k < 2; ++k) {
+        d.gt_stride[k] = r.gt_stride[k];
+        d.anchor_stride[k] = r.anchor_stride[k];
+      }
+    }
+  }
+  return desc;
+}
+
+void check_fcos_backward(const at::Tensor& grad, const at::Tensor& pred, const at::Tensor& num_foreground, const char* op) {
+  TORCH_CHECK(grad.is_cuda() && grad.get_device() == pred.get_device() && grad.scalar_type() == at::kFloat && grad.numel() == 1, op,
+              ": each incoming gradient must be one float32 value on the predictions' GPU");
+  TORCH_CHECK(num_foreground.is_cuda() && num_foreground.get_device() == pred.get_device() && num_foreground.scalar_type() == at::kLong &&
+                  num_foreground.numel() == 1,
+              op, ": num_foreground must be the forward's int64 count");
+}
+
+std::tuple<at::Tensor, at::Tensor> fcos_cls_loss(const at::Tensor& cls_logits, at::TensorList matched_idxs, at::TensorList labels) {
+  TORCH_CHECK(cls_logits.dim() == 3, "fcos_cls_loss: cls_logits must be [B, A, C]");
+  auto desc = fcos_loss_images(cls_logits, cls_logits.size(2), nullptr, matched_idxs, labels, {}, {}, "fcos_cls_loss");
+  at::cuda::CUDAGuard guard(cls_logits.device());
+  const int B = (int)desc.size();
+  const int64_t A = cls_logits.size(1);
+  at::Tensor loss = at::empty({}, cls_logits.options());
+  at::Tensor count = at::empty({}, cls_logits.options().dtype(at::kLong));
+  const size_t wsb = vb200_fcos_cls_loss_workspace_bytes(B, A);
+  at::Tensor ws = workspace(wsb, cls_logits);
+  check_rc(vb200_fcos_cls_loss(desc.data(), B, A, (int)cls_logits.size(2), loss.data_ptr<float>(), count.data_ptr<int64_t>(), ws.data_ptr(),
+                               wsb, cur_stream()),
+           "fcos_cls_loss");
+  return std::make_tuple(loss, count);
+}
+
+at::Tensor fcos_cls_loss_backward(const at::Tensor& grad, const at::Tensor& cls_logits, at::TensorList matched_idxs, at::TensorList labels,
+                                  const at::Tensor& num_foreground) {
+  TORCH_CHECK(cls_logits.dim() == 3, "fcos_cls_loss_backward: cls_logits must be [B, A, C]");
+  auto desc = fcos_loss_images(cls_logits, cls_logits.size(2), nullptr, matched_idxs, labels, {}, {}, "fcos_cls_loss_backward");
+  check_fcos_backward(grad, cls_logits, num_foreground, "fcos_cls_loss_backward");
+  at::cuda::CUDAGuard guard(cls_logits.device());
+  const int B = (int)desc.size();
+  at::Tensor g = grad.contiguous(), n = num_foreground.contiguous();
+  at::Tensor out = at::empty(cls_logits.sizes(), cls_logits.options());
+  for (int i = 0; i < B; ++i) desc[(size_t)i].grad = out.data_ptr<float>() + (int64_t)i * out.stride(0);
+  check_rc(vb200_fcos_cls_loss_backward(desc.data(), B, cls_logits.size(1), (int)cls_logits.size(2), g.data_ptr<float>(), n.data_ptr<int64_t>(),
+                                        cur_stream()),
+           "fcos_cls_loss_backward");
+  return out;
+}
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor> fcos_box_loss(const at::Tensor& bbox_regression, const at::Tensor& bbox_ctrness, at::TensorList anchors,
+                                                             at::TensorList gt_boxes, at::TensorList labels, at::TensorList matched_idxs,
+                                                             bool normalize_by_size) {
+  auto desc = fcos_loss_images(bbox_regression, 4, &bbox_ctrness, matched_idxs, labels, anchors, gt_boxes, "fcos_box_loss");
+  at::cuda::CUDAGuard guard(bbox_regression.device());
+  const int B = (int)desc.size();
+  const int64_t A = bbox_regression.size(1);
+  at::Tensor loss_box = at::empty({}, bbox_regression.options()), loss_ctr = at::empty({}, bbox_regression.options());
+  at::Tensor count = at::empty({}, bbox_regression.options().dtype(at::kLong));
+  const size_t wsb = vb200_fcos_box_loss_workspace_bytes(B, A);
+  at::Tensor ws = workspace(wsb, bbox_regression);
+  check_rc(vb200_fcos_box_loss(desc.data(), B, A, normalize_by_size ? 1 : 0, loss_box.data_ptr<float>(), loss_ctr.data_ptr<float>(),
+                               count.data_ptr<int64_t>(), ws.data_ptr(), wsb, cur_stream()),
+           "fcos_box_loss");
+  return std::make_tuple(loss_box, loss_ctr, count);
+}
+
+// An undefined incoming gradient counts as zero: its rows are 0 (both undefined: no launch).
+std::tuple<at::Tensor, at::Tensor> fcos_box_loss_backward(const std::optional<at::Tensor>& grad_box, const std::optional<at::Tensor>& grad_ctrness,
+                                                          const at::Tensor& bbox_regression, const at::Tensor& bbox_ctrness, at::TensorList anchors,
+                                                          at::TensorList gt_boxes, at::TensorList labels, at::TensorList matched_idxs,
+                                                          bool normalize_by_size, const at::Tensor& num_foreground) {
+  auto desc = fcos_loss_images(bbox_regression, 4, &bbox_ctrness, matched_idxs, labels, anchors, gt_boxes, "fcos_box_loss_backward");
+  const bool has_box = grad_box.has_value() && grad_box->defined(), has_ctr = grad_ctrness.has_value() && grad_ctrness->defined();
+  at::cuda::CUDAGuard guard(bbox_regression.device());
+  if (!has_box && !has_ctr)
+    return std::make_tuple(at::zeros(bbox_regression.sizes(), bbox_regression.options()), at::zeros(bbox_ctrness.sizes(), bbox_ctrness.options()));
+  at::Tensor gb, gc;
+  if (has_box) {
+    check_fcos_backward(*grad_box, bbox_regression, num_foreground, "fcos_box_loss_backward");
+    gb = grad_box->contiguous();
+  }
+  if (has_ctr) {
+    check_fcos_backward(*grad_ctrness, bbox_regression, num_foreground, "fcos_box_loss_backward");
+    gc = grad_ctrness->contiguous();
+  }
+  const int B = (int)desc.size();
+  at::Tensor n = num_foreground.contiguous();
+  at::Tensor out = at::empty(bbox_regression.sizes(), bbox_regression.options());
+  at::Tensor out_ctr = at::empty(bbox_ctrness.sizes(), bbox_ctrness.options());
+  for (int i = 0; i < B; ++i) {
+    desc[(size_t)i].grad = out.data_ptr<float>() + (int64_t)i * out.stride(0);
+    desc[(size_t)i].grad_ctrness = out_ctr.data_ptr<float>() + (int64_t)i * out_ctr.stride(0);
+  }
+  check_rc(vb200_fcos_box_loss_backward(desc.data(), B, bbox_regression.size(1), normalize_by_size ? 1 : 0, has_box ? gb.data_ptr<float>() : nullptr,
+                                        has_ctr ? gc.data_ptr<float>() : nullptr, n.data_ptr<int64_t>(), cur_stream()),
+           "fcos_box_loss_backward");
+  return std::make_tuple(out, out_ctr);
+}
+
 // ---- box_iou_rotated (csrc/ops/box_iou_rotated.cpp; checks as cuda/box_iou_rotated_kernel.cu:92-118) ----------------
 at::Tensor box_iou_rotated(const at::Tensor& boxes1, const at::Tensor& boxes2) {
   TORCH_CHECK(boxes1.is_cuda() && boxes2.is_cuda(), "boxes1 and boxes2 must be CUDA tensors");
@@ -1205,6 +1337,10 @@ TORCH_LIBRARY(vision_b200, m) {
   m.def("retinanet_cls_loss_backward(Tensor grad, Tensor cls_logits, Tensor[] matched_idxs, Tensor[] labels, Tensor num_foreground) -> Tensor");
   m.def("retinanet_box_loss(Tensor bbox_regression, Tensor[] anchors, Tensor[] gt_boxes, Tensor[] matched_idxs, float[] weights) -> (Tensor, Tensor)");
   m.def("retinanet_box_loss_backward(Tensor grad, Tensor bbox_regression, Tensor[] anchors, Tensor[] gt_boxes, Tensor[] matched_idxs, float[] weights, Tensor num_foreground) -> Tensor");
+  m.def("fcos_cls_loss(Tensor cls_logits, Tensor[] matched_idxs, Tensor[] labels) -> (Tensor, Tensor)");
+  m.def("fcos_cls_loss_backward(Tensor grad, Tensor cls_logits, Tensor[] matched_idxs, Tensor[] labels, Tensor num_foreground) -> Tensor");
+  m.def("fcos_box_loss(Tensor bbox_regression, Tensor bbox_ctrness, Tensor[] anchors, Tensor[] gt_boxes, Tensor[] labels, Tensor[] matched_idxs, bool normalize_by_size) -> (Tensor, Tensor, Tensor)");
+  m.def("fcos_box_loss_backward(Tensor? grad_box, Tensor? grad_ctrness, Tensor bbox_regression, Tensor bbox_ctrness, Tensor[] anchors, Tensor[] gt_boxes, Tensor[] labels, Tensor[] matched_idxs, bool normalize_by_size, Tensor num_foreground) -> (Tensor, Tensor)");
   m.def("multiscale_roi_align(Tensor[] features, Tensor rois, float[] scales, int pooled_height, int pooled_width, int sampling_ratio, int k_min, int k_max, float canonical_scale, float canonical_level, float eps) -> (Tensor, Tensor)");
   m.def("_roi_align_backward(Tensor grad, Tensor rois, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width, int sampling_ratio, bool aligned) -> Tensor");
   m.def("_roi_pool_backward(Tensor grad, Tensor rois, Tensor argmax, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width) -> Tensor");
@@ -1246,6 +1382,10 @@ TORCH_LIBRARY_IMPL(vision_b200, CUDA, m) {
   m.impl("retinanet_cls_loss_backward", TORCH_FN(retinanet_cls_loss_backward));
   m.impl("retinanet_box_loss", TORCH_FN(retinanet_box_loss));
   m.impl("retinanet_box_loss_backward", TORCH_FN(retinanet_box_loss_backward));
+  m.impl("fcos_cls_loss", TORCH_FN(fcos_cls_loss));
+  m.impl("fcos_cls_loss_backward", TORCH_FN(fcos_cls_loss_backward));
+  m.impl("fcos_box_loss", TORCH_FN(fcos_box_loss));
+  m.impl("fcos_box_loss_backward", TORCH_FN(fcos_box_loss_backward));
   m.impl("resize_crop_normalize", TORCH_FN(resize_crop_normalize));
   m.impl("box_iou_rotated", TORCH_FN(box_iou_rotated));
   m.impl("_deform_conv2d_backward", TORCH_FN(deform_conv2d_backward));

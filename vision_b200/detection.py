@@ -23,7 +23,9 @@ centre-sampling matching loop of ``FCOS.compute_loss`` (fcos.py:440-487) is ONE 
 RetinaNet's head losses, ``RetinaNetClassificationHead.compute_loss`` (retinanet.py:158-189, the sigmoid focal loss) and
 ``RetinaNetRegressionHead.compute_loss`` (:272-302, the "l1" box loss), per-image loops of full-size masks, gathers and
 elementwise chains, are ONE call each of ``vision_b200::retinanet_cls_loss`` / ``retinanet_box_loss`` for all images, with
-a fused backward (_autograd.py)."""
+a fused backward (_autograd.py).  FCOS's, ``FCOSHead.compute_loss`` (fcos.py:52-125: the focal, GIoU and centre-ness
+losses after a per-image gather loop and a ``.item()``), is ONE call of ``vision_b200::fcos_cls_loss`` and one of
+``fcos_box_loss``, each with a fused backward."""
 from __future__ import annotations
 
 import math
@@ -549,3 +551,54 @@ def fcos_compute_loss(self, targets, head_outputs, anchors, num_anchors_per_leve
         return _orig(self, targets, head_outputs, anchors, num_anchors_per_level)
     matched_idxs = fcos_match_op(gt_boxes, anchors, self.center_sampling_radius, num_anchors_per_level)
     return self.head.compute_loss(targets, head_outputs, anchors, matched_idxs)
+
+
+def fcos_head_loss_supported(head, targets, head_outputs, anchors, matched_idxs) -> bool:
+    """Inputs the FCOS loss kernels reproduce FCOSHead.compute_loss on: a plain ``det_utils.BoxLinearCoder``; the three head
+    outputs as _loss_inputs_ok takes them (fp32, so autocast's fp16 / bf16 outputs keep the reference) with widths C, 4
+    and 1 and one A; per image an int64 [M] labels tensor and fp32 [M, 4] gt boxes, and one fp32 [A, 4] anchor tensor, all
+    on the outputs' GPU."""
+    from torchvision.models.detection import _utils as det_utils
+
+    coder = getattr(head, "box_coder", None)
+    if type(coder) is not det_utils.BoxLinearCoder or not isinstance(coder.normalize_by_size, bool) or not isinstance(head_outputs, dict):
+        return False
+    logits, regression, ctrness = (head_outputs.get(k) for k in ("cls_logits", "bbox_regression", "bbox_ctrness"))
+    if not isinstance(logits, Tensor) or logits.dim() != 3 or not _loss_inputs_ok(targets, logits, matched_idxs, logits.shape[2]):
+        return False
+    if not (_loss_inputs_ok(targets, regression, matched_idxs, 4) and _loss_inputs_ok(targets, ctrness, matched_idxs, 1)):
+        return False
+    if not isinstance(anchors, (list, tuple)) or len(anchors) != len(targets):
+        return False
+    A, device = logits.shape[1], logits.device
+    for t, a in zip(targets, anchors):
+        g, l = t.get("boxes"), t.get("labels")
+        if not (_same_gpu(l, device, torch.int64, 1) and _same_gpu(g, device, torch.float32, 2) and tuple(g.shape) == (l.shape[0], 4)
+                and _same_gpu(a, device, torch.float32, 2) and tuple(a.shape) == (A, 4)):
+            return False
+    return True
+
+
+def fcos_cls_loss_op(cls_logits, matched_idxs, labels):
+    _lib.load_ops()
+    loss, _ = torch.ops.vision_b200.fcos_cls_loss(cls_logits, list(matched_idxs), list(labels))
+    return loss
+
+
+def fcos_box_loss_op(bbox_regression, bbox_ctrness, anchors, gt_boxes, labels, matched_idxs, normalize_by_size: bool):
+    _lib.load_ops()
+    loss_box, loss_ctrness, _ = torch.ops.vision_b200.fcos_box_loss(bbox_regression, bbox_ctrness, list(anchors), list(gt_boxes),
+                                                                    list(labels), list(matched_idxs), bool(normalize_by_size))
+    return loss_box, loss_ctrness
+
+
+def fcos_head_compute_loss(self, targets, head_outputs, anchors, matched_idxs, _orig=None):
+    """FCOSHead.compute_loss as two fused calls for all images (the focal loss; the GIoU and centre-ness losses): the same
+    three losses with no host sync, and dense gradients of the three head outputs written in one pass each."""
+    if not fcos_head_loss_supported(self, targets, head_outputs, anchors, matched_idxs):
+        return _orig(self, targets, head_outputs, anchors, matched_idxs)
+    labels = [t["labels"] for t in targets]
+    loss_box, loss_ctrness = fcos_box_loss_op(head_outputs["bbox_regression"], head_outputs["bbox_ctrness"], anchors,
+                                              [t["boxes"] for t in targets], labels, matched_idxs, self.box_coder.normalize_by_size)
+    return {"classification": fcos_cls_loss_op(head_outputs["cls_logits"], matched_idxs, labels), "bbox_regression": loss_box,
+            "bbox_ctrness": loss_ctrness}
