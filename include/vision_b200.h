@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define VB200_ABI_VERSION 1
+#define VB200_ABI_VERSION 2
 
 #if defined(__GNUC__)
 #define VB200_API __attribute__((visibility("default")))
@@ -74,9 +74,6 @@ VB200_API uint64_t vb200_launch_count(void);
 /* The VB200_* path overrides (DESIGN.md, testing / profiling only) are read from the environment once, the first
  * time a launcher needs them; this re-reads them (tests switch paths inside one process). */
 VB200_API void vb200_reload_env(void);
-/* Generation counter of those overrides (bumped by every (re)load): callers that cache work recorded under one setting
- * of them, e.g. captured CUDA graphs (as the library's own batched_nms graph cache does), key the cache on it. */
-VB200_API int vb200_env_generation(void);
 
 /* ---- roi_align ---------------------------------------------------------
  * Replaces roi_align_forward_kernel, csrc/ops/cuda/roi_align_kernel.cu:334-394
@@ -146,18 +143,15 @@ VB200_API int vb200_ps_roi_align_forward(const void* input, const void* rois, vo
 /* ---- ps_roi_pool (API completeness, SURVEY.md §8f4) --------------------
  * Replaces ps_roi_pool_forward_kernel / ps_roi_pool_backward_kernel, csrc/ops/cuda/ps_roi_pool_kernel.cu:15-142
  * (schemas csrc/ops/ps_roi_pool.cpp:71-73).  Shapes as ps_roi_align; the backward writes grad_input in full itself.
- * vb200_ps_roi_pool_backward is vb200_ps_roi_pool_backward_ex with deterministic = 0 and no workspace (an atomic scatter);
- * _ex with deterministic != 0 and vb200_roi_backward_workspace_bytes(num_rois, pooled_h, pooled_w, 1) bytes of workspace
- * is bit-reproducible (see the backward section below). */
+ * With deterministic == 0 (workspace unused) the backward is an atomic scatter; with deterministic != 0 and
+ * vb200_roi_backward_workspace_bytes(num_rois, pooled_h, pooled_w, 1) bytes of workspace it is bit-reproducible (see the
+ * backward section below). */
 VB200_API int vb200_ps_roi_pool_forward(const void* input, const void* rois, void* output, int32_t* channel_mapping, int dtype,
                               int batch, int channels, int height, int width, int num_rois, int pooled_h, int pooled_w,
                               double spatial_scale, vb200_stream stream);
 VB200_API int vb200_ps_roi_pool_backward(const void* grad, const void* rois, void* grad_input, int dtype, int batch, int channels,
                                int height, int width, int num_rois, int pooled_h, int pooled_w, double spatial_scale,
-                               vb200_stream stream);
-VB200_API int vb200_ps_roi_pool_backward_ex(const void* grad, const void* rois, void* grad_input, int dtype, int batch, int channels,
-                                  int height, int width, int num_rois, int pooled_h, int pooled_w, double spatial_scale,
-                                  int deterministic, void* workspace, size_t workspace_bytes, vb200_stream stream);
+                               int deterministic, void* workspace, size_t workspace_bytes, vb200_stream stream);
 
 /* ---- backward of the RoI ops --------------------------------------------
  * Replace roi_align_backward_kernel (csrc/ops/cuda/roi_align_kernel.cu:396-468, schema roi_align.cpp:76-77),
@@ -393,106 +387,78 @@ VB200_API void vb200_fcos_level_bounds(int64_t num_anchors, int64_t first_level,
 VB200_API int vb200_fcos_match(const vb200_fcos_image* images, int num_images, int gt_dtype, int anchor_dtype, double radius,
                                int64_t first_level, int64_t last_level, vb200_stream stream);
 
-/* ---- RetinaNet head losses ---------------------------------------------------------------------------------------------
- * Replace the per-image loops of RetinaNetClassificationHead.compute_loss (torchvision/models/detection/retinanet.py:158-189,
- * with sigmoid_focal_loss, ops/focal_loss.py:41-56, alpha 0.25, gamma 2) and of RetinaNetRegressionHead.compute_loss
- * (retinanet.py:272-302 with _box_loss "l1", models/detection/_utils.py:524-526, and encode_boxes, :103-118), forward and
- * backward, for all images of a call, with no host sync and no full-size intermediate.
- * Image i, all fp32: pred is the image's dense rows of cls_logits [A, C] or bbox_regression [A, 4] (unit stride, rows of C
- * or 4); matched int64 [A] (element stride matched_stride), the Matcher's indices: >= 0 foreground, -2 ignored, other
- * negatives background; classification: labels int64 [num_gt] (stride label_stride), the target class of a foreground
- * anchor is labels[matched], a label in [-C, 0) wrapping as indexing does; regression: gt [num_gt, 4] and anchors [A, 4]
- * (element strides (row, column)); grad (backward only) the image's dense rows of the gradient, written exactly once.
- * A matched index >= num_gt or a label outside [-C, C) (the reference raises a device-side assert) makes the image's loss
- * NaN and its gradient rows NaN; nothing outside labels, gt or the pred rows is read.
- * Forward: *loss (device fp32) = (sum_i L_i) * fl(1 / B) with the images added in order, L_i = S_i / max(1, n_i) as the
- * heads divide (a true division in the classification head, the product with fl(1 / n_i) in the regression head), S_i the
- * image's sum, n_i its foreground count (written to num_foreground[i], device int64).  Classification elements follow the
- * focal loss in stable fp32 forms, the regression targets are encode_single's bits.  Backward: grad_loss (device fp32, 0-dim)
- * times the per-image scale fl(fl(g * fl(1 / B)) / max(1, n_i)) (the product with fl(1 / n_i) for regression) times the
- * element's derivative; 0 for ignored and background-regression rows, sign(pred - target) as torch.sign (0 for ±0 and NaN).
+/* ---- single-stage detector head losses ----------------------------------------------------------------------------------
+ * Replace, forward and backward, for all images of a call with no host sync and no full-size intermediate:
+ *   VB200_LOSS_RETINANET_CLS  the per-image loop of RetinaNetClassificationHead.compute_loss
+ *                             (torchvision/models/detection/retinanet.py:158-189, with sigmoid_focal_loss, ops/focal_loss.py:41-56,
+ *                             alpha 0.25, gamma 2);
+ *   VB200_LOSS_RETINANET_BOX  that of RetinaNetRegressionHead.compute_loss (retinanet.py:272-302 with _box_loss "l1",
+ *                             models/detection/_utils.py:524-526, and encode_boxes, :103-118);
+ *   VB200_LOSS_FCOS_CLS, _BOX FCOSHead.compute_loss (fcos.py:52-125): its per-image gather loop, the .item() host sync,
+ *                             sigmoid_focal_loss (alpha 0.25, gamma 2), BoxLinearCoder.decode / .encode (_utils.py:240-310),
+ *                             generalized_box_iou_loss (ops/giou_loss.py with _loss_inter_union, ops/_utils.py:87-105) and
+ *                             binary_cross_entropy_with_logits on the centre-ness; the classification loss in one call, the GIoU
+ *                             and centre-ness losses together in the other.
+ * Image i, all fp32: pred is the image's dense rows of cls_logits [A, C] or bbox_regression [A, 4] (unit stride, rows of
+ * `width` = C for the classification kinds, 4 for the box kinds); matched int64 [A] (element stride matched_stride); labels
+ * int64 [num_gt] (stride label_stride; not RETINANET_BOX); gt [num_gt, 4] and anchors [A, 4] (element strides (row, column);
+ * box kinds only); ctrness the image's bbox_ctrness [A] (element stride ctrness_stride, FCOS_BOX only); grad / grad_ctrness
+ * (backward only; grad_ctrness FCOS_BOX only) the image's dense rows of the gradients, written exactly once.  A call ignores
+ * the fields its kind does not use.  A bad index (per kind below) makes the loss NaN and the anchor's gradient rows NaN
+ * where the reference raises a device-side assert; nothing outside labels, gt or the pred rows is read.
+ * Arguments: weights_host (RETINANET_BOX only, required) the box coder's weights as torch.as_tensor(weights, dtype=float32)
+ * rounds them; normalize_by_size (read for FCOS_BOX only) the BoxLinearCoder's flag (nonzero: the codes are relative to the
+ * anchor's width and height); loss / loss2 (device fp32, 0-dim) the losses, loss2 required for FCOS_BOX and null otherwise;
+ * grad_loss / grad_loss2 (device fp32, 0-dim) their incoming gradients, grad_loss2 for FCOS_BOX only, not both null.
  * Every sum is in a fixed order, no floating-point atomics: results are bit-reproducible.  workspace: the query's bytes, a
- * function of (B, A) only.  Per VB200_LOSS_MAX_IMAGES images one kernel launch, plus one finalize launch per forward.
- * A * C (A * 4) must be below 2^31.  Asynchronous. */
+ * function of (kind, B, A) only.  Per VB200_LOSS_MAX_IMAGES images one kernel launch, plus one finalize launch per forward.
+ * A * width must be below 2^31.  An unknown kind is VB200_EINVAL.  Asynchronous.
+ *
+ * RetinaNet.  matched holds the Matcher's indices: >= 0 foreground, -2 ignored, other negatives background; the target class
+ * of a foreground anchor is labels[matched], a label in [-C, 0) wrapping as indexing does.  A matched index >= num_gt or a
+ * label outside [-C, C) is bad: the image's loss is NaN and its gradient rows NaN.  Forward: *loss = (sum_i L_i) * fl(1 / B)
+ * with the images added in order, L_i = S_i / max(1, n_i) as the heads divide (a true division in the classification head,
+ * the product with fl(1 / n_i) in the regression head), S_i the image's sum, n_i its foreground count (written to
+ * num_foreground[i], device int64).  Classification elements follow the focal loss in stable fp32 forms, the regression
+ * targets are encode_single's bits.  Backward: grad_loss times the per-image scale fl(fl(g * fl(1 / B)) / max(1, n_i)) (the
+ * product with fl(1 / n_i) for regression) times the element's derivative; 0 for ignored and background-regression rows,
+ * sign(pred - target) as torch.sign (0 for ±0 and NaN).
+ *
+ * FCOS.  Foreground, as the reference derives it with m = matched[a]: m < 0 (-2 included) is background; an image with no gt
+ * and m >= 0 has target class 0 and the zero gt box; otherwise l = labels[m] is the target class if l >= 0 and background if
+ * l < 0 (not wrapped).  m >= num_gt > 0, or (classification) l >= C, is bad: the loss is NaN and the anchor's gradient rows
+ * NaN.  n = the number of foreground anchors of the whole batch (bad ones included), written to *num_foreground (device
+ * int64).  Forward: each of *loss, *loss2 = fl(S) * fl(1 / max(1, n)), S the sum over the whole batch (the head divides by
+ * the Python int from .item(), which ATen's CUDA division turns into the product with its fp32 reciprocal; no 1 / B).
+ * Classification: the focal loss of every element, in the stable forms of the RetinaNet kind.  Box: per foreground anchor
+ * the GIoU loss of decode(bbox_regression, anchor) against the gt box (*loss), and BCE-with-logits (1 - t) x - log sigmoid(x)
+ * of the centre-ness logit x against t = sqrt(min(l, r) / max(l, r) * min(t, b) / max(t, b)) of encode(anchor, gt) (*loss2);
+ * decode, encode and the GIoU restated op by op in fp32, so every branch (overlap, min / max) is the reference's fp32
+ * decision.  Backward: s = fl(g * fl(1 / max(1, n))), g read from device memory, times each element's derivative; the GIoU
+ * gradient is analytic through the decode, with torch.max / torch.min's tie rule (equal operands get half the gradient
+ * each), and the centre-ness gradient s (sigmoid(x) - t).  Non-foreground rows are exactly 0; a null grad_loss or grad_loss2
+ * counts as a zero gradient: its rows are 0. */
 #define VB200_LOSS_MAX_IMAGES 64
-typedef struct vb200_retinanet_loss_image {
+enum { VB200_LOSS_RETINANET_CLS, VB200_LOSS_RETINANET_BOX, VB200_LOSS_FCOS_CLS, VB200_LOSS_FCOS_BOX };
+typedef struct vb200_loss_image {
   const float* pred;
+  const float* ctrness;        /* FCOS box only */
   const int64_t* matched;
-  const int64_t* labels;       /* classification only */
-  const float* gt;             /* regression only */
-  const float* anchors;        /* regression only */
+  const int64_t* labels;       /* not RetinaNet box */
+  const float* gt;             /* box kinds only */
+  const float* anchors;        /* box kinds only */
   float* grad;                 /* backward only */
-  int64_t matched_stride, label_stride, gt_stride[2], anchor_stride[2];
-  int64_t num_gt;
-} vb200_retinanet_loss_image;
-VB200_API size_t vb200_retinanet_cls_loss_workspace_bytes(int num_images, int64_t num_anchors);
-VB200_API int vb200_retinanet_cls_loss(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors, int num_classes,
-                                       float* loss, int64_t* num_foreground, void* workspace, size_t workspace_bytes,
-                                       vb200_stream stream);
-VB200_API int vb200_retinanet_cls_loss_backward(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
-                                                int num_classes, const float* grad_loss, const int64_t* num_foreground,
-                                                vb200_stream stream);
-/* weights_host: the box coder's weights as torch.as_tensor(weights, dtype=float32) rounds them */
-VB200_API size_t vb200_retinanet_box_loss_workspace_bytes(int num_images, int64_t num_anchors);
-VB200_API int vb200_retinanet_box_loss(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
-                                       const float* weights_host, float* loss, int64_t* num_foreground, void* workspace,
-                                       size_t workspace_bytes, vb200_stream stream);
-VB200_API int vb200_retinanet_box_loss_backward(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
-                                                const float* weights_host, const float* grad_loss, const int64_t* num_foreground,
-                                                vb200_stream stream);
-
-/* ---- FCOS head losses --------------------------------------------------------------------------------------------------
- * Replace FCOSHead.compute_loss (torchvision/models/detection/fcos.py:52-125): its per-image gather loop, the .item() host
- * sync, sigmoid_focal_loss (ops/focal_loss.py:41-56, alpha 0.25, gamma 2), BoxLinearCoder.decode / .encode
- * (models/detection/_utils.py:240-310), generalized_box_iou_loss (ops/giou_loss.py with _loss_inter_union, ops/_utils.py:87-105)
- * and binary_cross_entropy_with_logits on the centre-ness, forward and backward, for all images of a call, with no host sync
- * and no full-size intermediate.  Two calls: the classification loss, and the GIoU and centre-ness losses together.
- * Image i, all fp32: pred is the image's dense rows of cls_logits [A, C] or bbox_regression [A, 4] (unit stride, rows of C
- * or 4); ctrness the image's bbox_ctrness [A] (element stride ctrness_stride, box call only); matched int64 [A] (stride
- * matched_stride); labels int64 [num_gt] (stride label_stride); gt [num_gt, 4] and anchors [A, 4] (element strides (row,
- * column), box call only); grad / grad_ctrness (backward only) the image's dense rows of the gradients, written exactly once.
- * Foreground, as the reference derives it with m = matched[a]: m < 0 (-2 included) is background; an image with no gt and
- * m >= 0 has target class 0 and the zero gt box; otherwise l = labels[m] is the target class if l >= 0 and background if
- * l < 0 (not wrapped).  m >= num_gt > 0, or (classification) l >= C, is bad: the reference raises a device-side assert, here
- * the loss is NaN and the anchor's gradient rows NaN; nothing outside labels, gt or the pred rows is read.
- * n = the number of foreground anchors of the whole batch (bad ones included), written to *num_foreground (device int64).
- * Forward: each *loss (device fp32) = fl(S) * fl(1 / max(1, n)), S the sum over the whole batch (the head divides by the
- * Python int from .item(), which ATen's CUDA division turns into the product with its fp32 reciprocal; no 1 / B).
- * Classification: the focal loss of every element, in the stable forms of the RetinaNet call.  Box: per foreground anchor
- * the GIoU loss of decode(bbox_regression, anchor) against the gt box, and BCE-with-logits (1 - t) x - log sigmoid(x) of the
- * centre-ness logit x against t = sqrt(min(l, r) / max(l, r) * min(t, b) / max(t, b)) of encode(anchor, gt); decode, encode
- * and the GIoU restated op by op in fp32, so every branch (overlap, min / max) is the reference's fp32 decision.
- * Backward: s = fl(g * fl(1 / max(1, n))), g read from device memory, times each element's derivative; the GIoU gradient is
- * analytic through the decode, with torch.max / torch.min's tie rule (equal operands get half the gradient each), and the
- * centre-ness gradient s (sigmoid(x) - t).  Non-foreground rows are exactly 0; a null grad_box or grad_ctrness (not both)
- * counts as a zero gradient: its rows are 0.  Every sum is in a fixed order, no floating-point atomics: results are bit-reproducible.
- * workspace: the query's bytes, a function of (B, A) only.  Per VB200_LOSS_MAX_IMAGES images one kernel launch, plus one
- * finalize launch per forward.  A * C (A * 4) must be below 2^31.  Asynchronous. */
-typedef struct vb200_fcos_loss_image {
-  const float* pred;
-  const float* ctrness;        /* box call only */
-  const int64_t* matched;
-  const int64_t* labels;
-  const float* gt;             /* box call only */
-  const float* anchors;        /* box call only */
-  float* grad;                 /* backward only */
-  float* grad_ctrness;         /* box backward only */
+  float* grad_ctrness;         /* FCOS box backward only */
   int64_t ctrness_stride, matched_stride, label_stride, gt_stride[2], anchor_stride[2];
   int64_t num_gt;
-} vb200_fcos_loss_image;
-VB200_API size_t vb200_fcos_cls_loss_workspace_bytes(int num_images, int64_t num_anchors);
-VB200_API int vb200_fcos_cls_loss(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int num_classes, float* loss,
-                                  int64_t* num_foreground, void* workspace, size_t workspace_bytes, vb200_stream stream);
-VB200_API int vb200_fcos_cls_loss_backward(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int num_classes,
-                                           const float* grad_loss, const int64_t* num_foreground, vb200_stream stream);
-/* normalize_by_size: the BoxLinearCoder's flag (nonzero: the codes are relative to the anchor's width and height) */
-VB200_API size_t vb200_fcos_box_loss_workspace_bytes(int num_images, int64_t num_anchors);
-VB200_API int vb200_fcos_box_loss(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int normalize_by_size,
-                                  float* loss_box, float* loss_ctrness, int64_t* num_foreground, void* workspace,
-                                  size_t workspace_bytes, vb200_stream stream);
-VB200_API int vb200_fcos_box_loss_backward(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors,
-                                           int normalize_by_size, const float* grad_box, const float* grad_ctrness,
-                                           const int64_t* num_foreground, vb200_stream stream);
+} vb200_loss_image;
+VB200_API size_t vb200_head_loss_workspace_bytes(int kind, int num_images, int64_t num_anchors);
+VB200_API int vb200_head_loss(int kind, const vb200_loss_image* images, int num_images, int64_t num_anchors, int width,
+                              const float* weights_host, int normalize_by_size, float* loss, float* loss2, int64_t* num_foreground,
+                              void* workspace, size_t workspace_bytes, vb200_stream stream);
+VB200_API int vb200_head_loss_backward(int kind, const vb200_loss_image* images, int num_images, int64_t num_anchors, int width,
+                                       const float* weights_host, int normalize_by_size, const float* grad_loss,
+                                       const float* grad_loss2, const int64_t* num_foreground, vb200_stream stream);
 
 /* ---- deform_conv2d -----------------------------------------------------
  * Replaces deform_conv2d_forward_kernel, csrc/ops/cuda/deform_conv2d_kernel.cu:1035-1255
@@ -508,37 +474,26 @@ VB200_API int vb200_fcos_box_loss_backward(const vb200_fcos_loss_image* images, 
 VB200_API size_t vb200_deform_conv2d_workspace_bytes(int dtype, int batch, int c_in, int in_h, int in_w,
                                            int c_out, int kh, int kw, int out_h, int out_w,
                                            int groups, int offset_groups);
-VB200_API int vb200_deform_conv2d_forward(const void* input, const void* weight, const void* offset,
-                                const void* mask, const void* bias, void* out, int dtype,
-                                int batch, int c_in, int in_h, int in_w, int c_out, int kh,
-                                int kw, int stride_h, int stride_w, int pad_h, int pad_w,
-                                int dil_h, int dil_w, int groups, int offset_groups,
-                                int use_mask, void* workspace, size_t workspace_bytes,
-                                vb200_stream stream);
 
 /* Weights are constant across inference calls and a channels-last producer can hand the input over without the
  * NCHW -> NHWC staging pass: vb200_deform_conv2d_pack_weight() writes the swizzled K-major image the tensor-core
  * kernels read (vb200_deform_conv2d_packed_weight_bytes() bytes; 0 = this shape takes the SIMT kernel), and
- * vb200_deform_conv2d_forward_ex() takes it (packed_weight may be NULL) plus `input_is_nhwc` (input laid out
+ * vb200_deform_conv2d_forward() takes it (packed_weight may be NULL) plus `input_is_nhwc` (input laid out
  * [batch, in_h, in_w, c_in], 16-byte aligned).  The torch shim caches the packed image per weight tensor / version. */
 VB200_API size_t vb200_deform_conv2d_packed_weight_bytes(int dtype, int c_in, int c_out, int kh, int kw, int groups, int offset_groups);
 VB200_API int vb200_deform_conv2d_pack_weight(const void* weight, void* packed, int dtype, int c_in, int c_out, int kh, int kw,
                                     int groups, int offset_groups, vb200_stream stream);
-VB200_API int vb200_deform_conv2d_forward_ex(const void* input, const void* weight, const void* packed_weight, int input_is_nhwc,
-                                   const void* offset, const void* mask, const void* bias, void* out, int dtype, int batch,
-                                   int c_in, int in_h, int in_w, int c_out, int kh, int kw, int stride_h, int stride_w,
-                                   int pad_h, int pad_w, int dil_h, int dil_w, int groups, int offset_groups, int use_mask,
-                                   void* workspace, size_t workspace_bytes, vb200_stream stream);
-/* deform_conv2d fused with the all-gather of its output over the GPUs of one box (SURVEY.md 8e: the batch shards, one
- * all-gather of the per-shard outputs): outs[0] is the caller's slot of its own gathered buffer, outs[1..n_outs) the SAME slot
- * of every peer's buffer (peer-mapped device pointers); the wgmma kernel's epilogue stores each output element to all of
- * them.  Other arguments as vb200_deform_conv2d_forward_ex.  The caller synchronises the ranks before anyone reads. */
-VB200_API int vb200_deform_conv2d_forward_gather(const void* input, const void* weight, const void* packed_weight, int input_is_nhwc,
-                                       const void* offset, const void* mask, const void* bias, void* const* outs, int n_outs,
-                                       int dtype, int batch, int c_in, int in_h, int in_w, int c_out, int kh, int kw,
-                                       int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int groups,
-                                       int offset_groups, int use_mask, void* workspace, size_t workspace_bytes,
-                                       vb200_stream stream);
+/* outs[0] is the output; outs[1..n_outs) (1 <= n_outs <= 8) fuse the all-gather of the output over the GPUs of one box
+ * (SURVEY.md 8e: the batch shards, one all-gather of the per-shard outputs): outs[0] is then the caller's slot of its own
+ * gathered buffer and outs[1..n_outs) the SAME slot of every peer's buffer (peer-mapped device pointers); the wgmma kernel's
+ * epilogue stores each output element to all of them.  The caller synchronises the ranks before anyone reads.  n_outs = 1
+ * is the plain op. */
+VB200_API int vb200_deform_conv2d_forward(const void* input, const void* weight, const void* packed_weight, int input_is_nhwc,
+                                const void* offset, const void* mask, const void* bias, void* const* outs, int n_outs,
+                                int dtype, int batch, int c_in, int in_h, int in_w, int c_out, int kh, int kw,
+                                int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int groups,
+                                int offset_groups, int use_mask, void* workspace, size_t workspace_bytes,
+                                vb200_stream stream);
 
 /* ---- deform_conv2d backward ----------------------------------------------
  * Replace the kernels of deform_conv2d_backward_kernel, csrc/ops/cuda/deform_conv2d_kernel.cu:319-1033 (schema
@@ -554,29 +509,25 @@ VB200_API int vb200_deform_conv2d_sample_columns(const void* input, const void* 
                                        int n_imgs, int c_in, int in_h, int in_w, int kh, int kw, int stride_h, int stride_w,
                                        int pad_h, int pad_w, int dil_h, int dil_w, int offset_groups, int use_mask,
                                        vb200_stream stream);
-VB200_API int vb200_deform_conv2d_backward_inputs(const void* dcol, const void* input, const void* offset, const void* mask,
-                                        void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs, int c_in,
-                                        int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w,
-                                        int dil_h, int dil_w, int offset_groups, int use_mask, vb200_stream stream);
 /* Bit-reproducible grad_input (the reference instead raises under torch.use_deterministic_algorithms,
  * alertNotDeterministic("compute_grad_input"), deformable_col2im's caller :441).  With `deterministic` set,
- * vb200_deform_conv2d_backward_inputs_ex writes grad_input IN FULL (no pre-zeroing) by a gather instead of the scatter: the
+ * vb200_deform_conv2d_backward_inputs writes grad_input IN FULL (no pre-zeroing) by a gather instead of the scatter: the
  * samples are binned by the cell (floor y, floor x) they fall in and sorted stably, and each grad_input[b, c, y, x] is summed
  * over the cells (y, x), (y, x-1), (y-1, x), (y-1, x-1) in that order, inside a cell in ascending (offset group, tap, output
  * pixel) order, in fp32 (double for F64) and rounded once.  The value depends on image b's data alone.  grad_offset /
  * grad_mask are the same as without the flag.  The workspace (vb200_deform_conv2d_backward_inputs_workspace_bytes, host
  * arithmetic only, 0 for an empty shape) holds the sort keys, the cell table and one record per sample; images are processed
  * in passes whose sample count fits int32 and key range fits 32 bits, and a shape whose single image exceeds that returns
- * VB200_EUNSUPPORTED before anything is launched.  With deterministic == 0 the call is vb200_deform_conv2d_backward_inputs
- * (workspace unused, grad_input pre-zeroed and scattered with atomics). */
+ * VB200_EUNSUPPORTED before anything is launched.  With deterministic == 0 the workspace is unused and grad_input is
+ * pre-zeroed and scattered with atomics, as described above. */
 VB200_API size_t vb200_deform_conv2d_backward_inputs_workspace_bytes(int dtype, int n_imgs, int c_in, int in_h, int in_w, int kh, int kw,
                                                            int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w,
                                                            int offset_groups);
-VB200_API int vb200_deform_conv2d_backward_inputs_ex(const void* dcol, const void* input, const void* offset, const void* mask,
-                                           void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs, int c_in,
-                                           int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w,
-                                           int dil_h, int dil_w, int offset_groups, int use_mask, int deterministic,
-                                           void* workspace, size_t workspace_bytes, vb200_stream stream);
+VB200_API int vb200_deform_conv2d_backward_inputs(const void* dcol, const void* input, const void* offset, const void* mask,
+                                        void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs, int c_in,
+                                        int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w,
+                                        int dil_h, int dil_w, int offset_groups, int use_mask, int deterministic,
+                                        void* workspace, size_t workspace_bytes, vb200_stream stream);
 
 /* ---- resize ------------------------------------------------------------
  * Replaces the interpolate path of resize_image,

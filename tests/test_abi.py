@@ -14,7 +14,7 @@ def _declared():
     return sorted(set(re.findall(r"^VB200_API [\w\s\*]+?\b(vb200_\w+)\(", text, flags=re.M)))
 
 
-def test_header_symbols_exported():
+def test_header_symbols_exported_at_abi_version_2():
     from vision_b200 import _lib
 
     lib = _lib.core()
@@ -23,7 +23,7 @@ def test_header_symbols_exported():
     assert sorted(_lib.ABI_SYMBOLS) == declared
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/vision_b200.h but not exported"
-    assert lib.vb200_abi_version() == 1
+    assert lib.vb200_abi_version() == 2
 
 
 def test_header_cites_reference_for_each_entry_point():

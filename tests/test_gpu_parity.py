@@ -50,11 +50,11 @@ class force_env:
         _lib.core().vb200_reload_env()
 
 
-def test_native_library_loaded(vb):
+def test_native_library_loaded_at_abi_version_2(vb):
     """The process must have the in-tree .so mapped — no eager / library fallback."""
     maps = open("/proc/self/maps").read()
     assert "libvision_b200.so" in maps and "libvision_b200_torch.so" in maps
-    assert torch.ops.vision_b200._abi_version() == 1
+    assert torch.ops.vision_b200._abi_version() == 2
 
 
 # =============================== roi_align ===================================

@@ -190,19 +190,25 @@ def register() -> None:
     def _(gt_boxes, anchors, radius, first_level, last_level):
         return [a.new_empty((a.shape[0],), dtype=torch.int64) for a in anchors]
 
-    # ---- RetinaNet head losses: cls_logits and bbox_regression are the only differentiable inputs; the counts are not ----
+    # ---- RetinaNet and FCOS head losses: cls_logits, bbox_regression and bbox_ctrness are the only differentiable inputs; the
+    # counts are not.  The two classification losses share their formula, each with its own backward op ----
     def cls_loss_setup(ctx, inputs, output):
         logits, matched, labels = inputs
         ctx.mark_non_differentiable(output[1])
         ctx.save_for_backward(logits, output[1])
         ctx.lists = (list(matched), list(labels))
 
-    def cls_loss_backward(ctx, grad, _grad_counts):
-        logits, counts = ctx.saved_tensors
-        matched, labels = ctx.lists
-        return ops.retinanet_cls_loss_backward(grad, logits, matched, labels, counts), [None] * len(matched), [None] * len(labels)
+    def cls_loss_backward(backward_op):
+        def backward(ctx, grad, _grad_counts):
+            logits, counts = ctx.saved_tensors
+            matched, labels = ctx.lists
+            return backward_op(grad, logits, matched, labels, counts), [None] * len(matched), [None] * len(labels)
 
-    lib.register_autograd("vision_b200::retinanet_cls_loss", cls_loss_backward, setup_context=cls_loss_setup)
+        return backward
+
+    lib.register_autograd("vision_b200::retinanet_cls_loss", cls_loss_backward(ops.retinanet_cls_loss_backward),
+                          setup_context=cls_loss_setup)
+    lib.register_autograd("vision_b200::fcos_cls_loss", cls_loss_backward(ops.fcos_cls_loss_backward), setup_context=cls_loss_setup)
 
     def box_loss_setup(ctx, inputs, output):
         regression, anchors, gt_boxes, matched, weights = inputs
@@ -234,21 +240,7 @@ def register() -> None:
     def _(grad, bbox_regression, anchors, gt_boxes, matched_idxs, weights, num_foreground):
         return bbox_regression.new_empty(bbox_regression.shape)
 
-    # ---- FCOS head losses: cls_logits, bbox_regression and bbox_ctrness are the only differentiable inputs; the count is
-    # not.  The box op's two losses share one backward, which takes both incoming gradients ----
-    def fcos_cls_setup(ctx, inputs, output):
-        logits, matched, labels = inputs
-        ctx.mark_non_differentiable(output[1])
-        ctx.save_for_backward(logits, output[1])
-        ctx.lists = (list(matched), list(labels))
-
-    def fcos_cls_backward(ctx, grad, _grad_count):
-        logits, count = ctx.saved_tensors
-        matched, labels = ctx.lists
-        return ops.fcos_cls_loss_backward(grad, logits, matched, labels, count), [None] * len(matched), [None] * len(labels)
-
-    lib.register_autograd("vision_b200::fcos_cls_loss", fcos_cls_backward, setup_context=fcos_cls_setup)
-
+    # the FCOS box op's two losses share one backward, which takes both incoming gradients
     def fcos_box_setup(ctx, inputs, output):
         regression, ctrness, anchors, gt_boxes, labels, matched, normalize = inputs
         ctx.mark_non_differentiable(output[2])

@@ -71,22 +71,18 @@ def load_ops() -> None:
 
 # every symbol include/vision_b200.h declares (checked by tests/test_abi.py)
 ABI_SYMBOLS = (
-    "vb200_abi_version", "vb200_last_error", "vb200_launch_count", "vb200_reload_env", "vb200_env_generation",
+    "vb200_abi_version", "vb200_last_error", "vb200_launch_count", "vb200_reload_env",
     "vb200_roi_align_workspace_bytes", "vb200_roi_align_forward", "vb200_roi_align_forward_gather", "vb200_roi_pool_forward",
     "vb200_ps_roi_align_forward", "vb200_nms_workspace_bytes", "vb200_nms",
     "vb200_batched_nms_workspace_bytes", "vb200_batched_nms", "vb200_deform_conv2d_workspace_bytes",
-    "vb200_deform_conv2d_forward", "vb200_deform_conv2d_forward_gather", "vb200_resize", "vb200_resize_gather",
-    "vb200_deform_conv2d_packed_weight_bytes", "vb200_deform_conv2d_pack_weight", "vb200_deform_conv2d_forward_ex",
+    "vb200_deform_conv2d_forward", "vb200_resize", "vb200_resize_gather",
+    "vb200_deform_conv2d_packed_weight_bytes", "vb200_deform_conv2d_pack_weight",
     "vb200_deform_conv2d_sample_columns", "vb200_deform_conv2d_backward_inputs", "vb200_ps_roi_pool_forward", "vb200_ps_roi_pool_backward", "vb200_box_iou_rotated", "vb200_resize_crop_normalize", "vb200_detection_postprocess_workspace_bytes", "vb200_detection_postprocess",
     "vb200_multiscale_roi_align_workspace_bytes", "vb200_multiscale_roi_align_supported", "vb200_multiscale_roi_align_forward",
     "vb200_roi_backward_workspace_bytes", "vb200_roi_align_backward", "vb200_roi_pool_backward", "vb200_ps_roi_align_backward",
     "vb200_single_stage_postprocess_workspace_bytes", "vb200_single_stage_postprocess",
-    "vb200_deform_conv2d_backward_inputs_workspace_bytes", "vb200_deform_conv2d_backward_inputs_ex",
-    "vb200_ps_roi_pool_backward_ex", "vb200_roi_backward_deterministic_supported",
+    "vb200_deform_conv2d_backward_inputs_workspace_bytes", "vb200_roi_backward_deterministic_supported",
     "vb200_heatmaps_to_keypoints_workspace_bytes", "vb200_heatmaps_to_keypoints",
     "vb200_rcnn_batch_images", "vb200_rcnn_rescale", "vb200_match_boxes_workspace_bytes", "vb200_match_boxes",
-    "vb200_fcos_level_bounds", "vb200_fcos_match", "vb200_retinanet_cls_loss_workspace_bytes", "vb200_retinanet_cls_loss",
-    "vb200_retinanet_cls_loss_backward", "vb200_retinanet_box_loss_workspace_bytes", "vb200_retinanet_box_loss",
-    "vb200_retinanet_box_loss_backward", "vb200_fcos_cls_loss_workspace_bytes", "vb200_fcos_cls_loss", "vb200_fcos_cls_loss_backward",
-    "vb200_fcos_box_loss_workspace_bytes", "vb200_fcos_box_loss", "vb200_fcos_box_loss_backward",
+    "vb200_fcos_level_bounds", "vb200_fcos_match", "vb200_head_loss_workspace_bytes", "vb200_head_loss", "vb200_head_loss_backward",
 )

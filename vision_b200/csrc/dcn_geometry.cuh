@@ -15,7 +15,7 @@ namespace vb200 {
 struct DcnParams {
   int batch, c_in, in_h, in_w, c_out, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w;
   int groups, offset_groups, use_mask, out_h, out_w;
-  // fused all-gather (vb200_deform_conv2d_forward_gather): the epilogue also stores every output element to the same slot of
+  // fused all-gather (vb200_deform_conv2d_forward): the epilogue also stores every output element to the same slot of
   // the peers' gathered buffers (peer-mapped device pointers; NVLink stores)
   void* peer_out[7];
   int n_peer;

@@ -260,41 +260,16 @@ static int dcn_forward_impl(const void* input, const void* weight, const void* o
   });
 }
 
-extern "C" int vb200_deform_conv2d_forward(const void* input, const void* weight, const void* offset,
-                                           const void* mask, const void* bias, void* out, int dtype, int batch,
-                                           int c_in, int in_h, int in_w, int c_out, int kh, int kw, int stride_h,
-                                           int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int groups,
-                                           int offset_groups, int use_mask, void* workspace,
-                                           size_t workspace_bytes, vb200_stream stream) {
-  return vb200_deform_conv2d_forward_ex(input, weight, nullptr, 0, offset, mask, bias, out, dtype, batch, c_in, in_h, in_w, c_out, kh, kw,
-                                        stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, groups, offset_groups, use_mask, workspace,
-                                        workspace_bytes, stream);
-}
-
-extern "C" int vb200_deform_conv2d_forward_ex(const void* input, const void* weight, const void* packed_weight, int input_is_nhwc,
-                                              const void* offset, const void* mask, const void* bias, void* out, int dtype, int batch,
-                                              int c_in, int in_h, int in_w, int c_out, int kh, int kw, int stride_h, int stride_w, int pad_h,
-                                              int pad_w, int dil_h, int dil_w, int groups, int offset_groups, int use_mask, void* workspace,
-                                              size_t workspace_bytes, vb200_stream stream) {
-  DcnParams p;
-  if (const int rc = dcn_params(p, batch, c_in, in_h, in_w, c_out, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, groups,
-                                offset_groups, use_mask))
-    return rc;
-  return dcn_forward_impl(input, weight, offset, mask, bias, out, dtype, p, workspace, workspace_bytes, stream,
-                          DcnHints{packed_weight, input_is_nhwc, nullptr, 0, nullptr});
-}
-
-// deform_conv2d fused with the all-gather of its output: outs[0] is the caller's slot of its own gathered buffer, outs[1..n) the
-// same slot of the peers' buffers (peer-mapped).  The wgmma kernel's epilogue stores each element to all of them; shapes that
-// take another kernel are computed into outs[0] and copied to the peers on the same stream.
-extern "C" int vb200_deform_conv2d_forward_gather(const void* input, const void* weight, const void* packed_weight, int input_is_nhwc,
-                                                  const void* offset, const void* mask, const void* bias, void* const* outs, int n_outs,
-                                                  int dtype, int batch, int c_in, int in_h, int in_w, int c_out, int kh, int kw,
-                                                  int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int groups,
-                                                  int offset_groups, int use_mask, void* workspace, size_t workspace_bytes,
-                                                  vb200_stream stream) {
-  VB200_REQUIRE(outs && n_outs >= 1 && n_outs <= 8, "deform_conv2d_gather: 1..8 destinations");
-  for (int d = 0; d < n_outs; ++d) VB200_REQUIRE(outs[d] != nullptr, "deform_conv2d_gather: null destination");
+// outs[0] is the output (the caller's slot of its own gathered buffer when fused with an all-gather), outs[1..n) the same slot
+// of the peers' buffers (peer-mapped).  The wgmma kernel's epilogue stores each element to all of them; shapes that take another
+// kernel are computed into outs[0] and copied to the peers on the same stream.
+extern "C" int vb200_deform_conv2d_forward(const void* input, const void* weight, const void* packed_weight, int input_is_nhwc,
+                                           const void* offset, const void* mask, const void* bias, void* const* outs, int n_outs,
+                                           int dtype, int batch, int c_in, int in_h, int in_w, int c_out, int kh, int kw, int stride_h,
+                                           int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int groups, int offset_groups,
+                                           int use_mask, void* workspace, size_t workspace_bytes, vb200_stream stream) {
+  VB200_REQUIRE(outs && n_outs >= 1 && n_outs <= 8, "deform_conv2d_forward: 1..8 destinations");
+  for (int d = 0; d < n_outs; ++d) VB200_REQUIRE(outs[d] != nullptr, "deform_conv2d_forward: null destination");
   DcnParams p;
   int rc = dcn_params(p, batch, c_in, in_h, in_w, c_out, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, groups, offset_groups,
                       use_mask);

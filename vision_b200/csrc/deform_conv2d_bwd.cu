@@ -397,11 +397,11 @@ extern "C" size_t vb200_deform_conv2d_backward_inputs_workspace_bytes(int dtype,
   return carve_det(nullptr, p, pass, dtype == VB200_F64 ? sizeof(double) : sizeof(float)).total;
 }
 
-extern "C" int vb200_deform_conv2d_backward_inputs_ex(const void* dcol, const void* input, const void* offset, const void* mask,
-                                                      void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs,
-                                                      int c_in, int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h,
-                                                      int pad_w, int dil_h, int dil_w, int offset_groups, int use_mask, int deterministic,
-                                                      void* workspace, size_t workspace_bytes, vb200_stream stream) {
+extern "C" int vb200_deform_conv2d_backward_inputs(const void* dcol, const void* input, const void* offset, const void* mask,
+                                                   void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs, int c_in,
+                                                   int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w,
+                                                   int dil_h, int dil_w, int offset_groups, int use_mask, int deterministic, void* workspace,
+                                                   size_t workspace_bytes, vb200_stream stream) {
   DcnParams p;
   if (const int rc = dcn_params(p, n_imgs, c_in, in_h, in_w, 0, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, 1, offset_groups,
                                 use_mask))
@@ -423,13 +423,4 @@ extern "C" int vb200_deform_conv2d_backward_inputs_ex(const void* dcol, const vo
       return launch_bwd_inputs_det<T>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, workspace, workspace_bytes, st);
     return launch_bwd_inputs<T>(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, p, n_imgs, st);
   });
-}
-
-extern "C" int vb200_deform_conv2d_backward_inputs(const void* dcol, const void* input, const void* offset, const void* mask,
-                                                   void* grad_input, void* grad_offset, void* grad_mask, int dtype, int n_imgs, int c_in,
-                                                   int in_h, int in_w, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w,
-                                                   int dil_h, int dil_w, int offset_groups, int use_mask, vb200_stream stream) {
-  return vb200_deform_conv2d_backward_inputs_ex(dcol, input, offset, mask, grad_input, grad_offset, grad_mask, dtype, n_imgs, c_in, in_h,
-                                                in_w, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, offset_groups, use_mask, 0,
-                                                nullptr, 0, stream);
 }

@@ -35,8 +35,8 @@ constexpr int kBackground = -1;   // every class's target is 0
 //   kBatchRecip  once for the batch, the product with fl(1 / max(1, n)), n from .item()
 enum class Norm { kImageDiv, kImageRecip, kBatchRecip };
 
-template <class Image> struct LossPlan {
-  Image img[VB200_LOSS_MAX_IMAGES];
+struct LossPlan {
+  vb200_loss_image img[VB200_LOSS_MAX_IMAGES];
   int64_t num_anchors;
   int num_classes, tiles, first_image, num_images;     // img[0] is image first_image of the call's num_images
   double* partial;                                      // forward: [num_images, tiles]
@@ -51,9 +51,8 @@ template <class Image> struct LossPlan {
 
 // RetinaNet: the Matcher's -2 is ignored; a label in [-C, 0) wraps as advanced indexing does.
 struct RetinaNetCls {
-  using Image = vb200_retinanet_loss_image;
   static constexpr Norm kNorm = Norm::kImageDiv;
-  __device__ static __forceinline__ int code(const Image& d, int64_t a, int C, bool& fg) {
+  __device__ static __forceinline__ int code(const vb200_loss_image& d, int64_t a, int C, bool& fg) {
     const int64_t m = d.matched[a * d.matched_stride];
     fg = m >= 0;                                        // num_foreground counts matched >= 0, bad indices included
     if (m == -2) return kIgnored;
@@ -68,7 +67,7 @@ struct RetinaNetCls {
 // FCOS (fcos.py:64-90): every negative match is background; an image without gt gives a match the class 0 of new_zeros; a
 // negative label is background (the mask is >= 0, nothing wraps).  `C` bounds the class: the box call passes INT64_MAX, as
 // its reference reads no class.  m is the match, for the box call's gt row.
-__device__ __forceinline__ int fcos_code(const vb200_fcos_loss_image& d, int64_t a, int64_t C, int64_t& m) {
+__device__ __forceinline__ int fcos_code(const vb200_loss_image& d, int64_t a, int64_t C, int64_t& m) {
   m = d.matched[a * d.matched_stride];
   if (m < 0) return kBackground;
   if (d.num_gt == 0) return 0;
@@ -79,9 +78,8 @@ __device__ __forceinline__ int fcos_code(const vb200_fcos_loss_image& d, int64_t
 }
 
 struct FcosCls {
-  using Image = vb200_fcos_loss_image;
   static constexpr Norm kNorm = Norm::kBatchRecip;
-  __device__ static __forceinline__ int code(const Image& d, int64_t a, int C, bool& fg) {
+  __device__ static __forceinline__ int code(const vb200_loss_image& d, int64_t a, int C, bool& fg) {
     int64_t m;
     const int c = fcos_code(d, a, C, m);
     fg = c >= 0 || c == kBad;                           // the reference's mask is label >= 0, bad indices included
@@ -148,13 +146,23 @@ template <Norm kNorm> __device__ __forceinline__ float loss_scale(const float* g
   return kNorm == Norm::kImageRecip ? __fmul_rn(g, reciprocal(d)) : __fdiv_rn(g, d);
 }
 
+// A forward CTA's results in its per-(image, tile) slots, stored by thread 0 (which holds the block sums); sum2 only for the
+// FCOS box loss.
+__device__ __forceinline__ void store_tile(const LossPlan& plan, int image, int tile_fg, double sum, const double* sum2 = nullptr) {
+  if (threadIdx.x != 0) return;
+  const int64_t slot = (int64_t)image * plan.tiles + blockIdx.x;
+  plan.partial[slot] = sum;
+  if (sum2) plan.partial2[slot] = *sum2;
+  plan.tile_fg[slot] = tile_fg;
+}
+
 // One CTA: kLossTile anchors of image blockIdx.y, all C classes.  The tile's elements [e0, e1) of the image's [A, C] block are
 // taken in 16-byte groups aligned on the streamed array (the logits forward, the gradient backward); the first and last groups
 // may be partial, since C need not be a multiple of 4.  Rule gives each anchor its code and the head's division.
 template <class Rule, bool kBackward>
 __global__ void __launch_bounds__(kLossThreads)
-focal_loss_kernel(const __grid_constant__ LossPlan<typename Rule::Image> plan) {
-  const typename Rule::Image& d = plan.img[blockIdx.y];
+focal_loss_kernel(const __grid_constant__ LossPlan plan) {
+  const vb200_loss_image& d = plan.img[blockIdx.y];
   const int image = plan.first_image + (int)blockIdx.y;
   const int C = plan.num_classes;
   const int64_t a0 = (int64_t)blockIdx.x * kLossTile;
@@ -215,13 +223,7 @@ focal_loss_kernel(const __grid_constant__ LossPlan<typename Rule::Image> plan) {
       }
     }
   }
-  if (!kBackward) {
-    const double sum = block_sum(acc, scratch);
-    if (threadIdx.x == 0) {
-      plan.partial[(int64_t)image * plan.tiles + blockIdx.x] = sum;
-      plan.tile_fg[(int64_t)image * plan.tiles + blockIdx.x] = tile_fg;
-    }
-  }
+  if (!kBackward) store_tile(plan, image, tile_fg, block_sum(acc, scratch));
 }
 
 // encode_boxes (models/detection/_utils.py:103-118) for one anchor and its matched gt box, one rounding per tensor op and
@@ -347,8 +349,8 @@ __device__ __forceinline__ float sign_of(float v) { return (float)((0.f < v) - (
 // One CTA: kLossTile anchors of image blockIdx.y, one per thread.  Only foreground anchors read their regression row.
 template <bool kBackward>
 __global__ void __launch_bounds__(kLossThreads)
-box_loss_kernel(const __grid_constant__ LossPlan<vb200_retinanet_loss_image> plan) {
-  const vb200_retinanet_loss_image& d = plan.img[blockIdx.y];
+box_loss_kernel(const __grid_constant__ LossPlan plan) {
+  const vb200_loss_image& d = plan.img[blockIdx.y];
   const int image = plan.first_image + (int)blockIdx.y;
   const int64_t a = (int64_t)blockIdx.x * kLossTile + threadIdx.x;
   const bool valid = a < plan.num_anchors;
@@ -383,11 +385,7 @@ box_loss_kernel(const __grid_constant__ LossPlan<vb200_retinanet_loss_image> pla
     if (valid) *reinterpret_cast<float4*>(d.grad + a * 4) = make_float4(gout[0], gout[1], gout[2], gout[3]);
   } else {
     const int tile_fg = __syncthreads_count(fg);
-    const double sum = block_sum(acc, scratch);
-    if (threadIdx.x == 0) {
-      plan.partial[(int64_t)image * plan.tiles + blockIdx.x] = sum;
-      plan.tile_fg[(int64_t)image * plan.tiles + blockIdx.x] = tile_fg;
-    }
+    store_tile(plan, image, tile_fg, block_sum(acc, scratch));
   }
 }
 
@@ -397,8 +395,8 @@ box_loss_kernel(const __grid_constant__ LossPlan<vb200_retinanet_loss_image> pla
 // loss's stable form; its derivative σ(x) - t.
 template <bool kBackward>
 __global__ void __launch_bounds__(kLossThreads)
-fcos_box_loss_kernel(const __grid_constant__ LossPlan<vb200_fcos_loss_image> plan) {
-  const vb200_fcos_loss_image& d = plan.img[blockIdx.y];
+fcos_box_loss_kernel(const __grid_constant__ LossPlan plan) {
+  const vb200_loss_image& d = plan.img[blockIdx.y];
   const int image = plan.first_image + (int)blockIdx.y;
   const int64_t a = (int64_t)blockIdx.x * kLossTile + threadIdx.x;
   const bool valid = a < plan.num_anchors;
@@ -449,11 +447,7 @@ fcos_box_loss_kernel(const __grid_constant__ LossPlan<vb200_fcos_loss_image> pla
     const int tile_fg = __syncthreads_count(fg);
     const double sum = block_sum(giou, scratch);
     const double sum2 = block_sum(bce, scratch);
-    if (threadIdx.x == 0) {
-      plan.partial[(int64_t)image * plan.tiles + blockIdx.x] = sum;
-      plan.partial2[(int64_t)image * plan.tiles + blockIdx.x] = sum2;
-      plan.tile_fg[(int64_t)image * plan.tiles + blockIdx.x] = tile_fg;
-    }
+    store_tile(plan, image, tile_fg, sum, &sum2);
   }
 }
 
@@ -494,40 +488,49 @@ loss_finalize_kernel(const double* __restrict__ partial, const double* __restric
   if (kNorm != Norm::kBatchRecip && threadIdx.x == 0) *loss = __fmul_rn(total, reciprocal((float)num_images));
 }
 
-int check_sizes(const void* images, int num_images, int64_t num_anchors, int width, const char* op) {
+// What each kind runs: its kernels, the division its finalize applies, its number of losses and its names in errors.
+struct Head {
+  void (*forward)(const LossPlan);
+  void (*backward)(const LossPlan);
+  const char* kernel;
+  Norm norm;
+  int terms;                                            // 2: FCOS's GIoU and centre-ness losses from one call
+  const char *op, *op_backward;
+};
+
+Head head_of(int kind) {
+  switch (kind) {
+    case VB200_LOSS_RETINANET_CLS:
+      return {focal_loss_kernel<RetinaNetCls, false>, focal_loss_kernel<RetinaNetCls, true>, "focal_loss_kernel", RetinaNetCls::kNorm, 1,
+              "retinanet_cls_loss", "retinanet_cls_loss_backward"};
+    case VB200_LOSS_RETINANET_BOX:
+      return {box_loss_kernel<false>, box_loss_kernel<true>, "box_loss_kernel", Norm::kImageRecip, 1, "retinanet_box_loss",
+              "retinanet_box_loss_backward"};
+    case VB200_LOSS_FCOS_CLS:
+      return {focal_loss_kernel<FcosCls, false>, focal_loss_kernel<FcosCls, true>, "focal_loss_kernel", FcosCls::kNorm, 1,
+              "fcos_cls_loss", "fcos_cls_loss_backward"};
+    case VB200_LOSS_FCOS_BOX:
+      return {fcos_box_loss_kernel<false>, fcos_box_loss_kernel<true>, "fcos_box_loss_kernel", Norm::kBatchRecip, 2, "fcos_box_loss",
+              "fcos_box_loss_backward"};
+  }
+  return {};                                            // forward null: an unknown kind
+}
+
+// The sizes, and every pointer of the descriptors that the kind reads.
+int check_call(int kind, const vb200_loss_image* images, int num_images, int64_t num_anchors, int width, bool backward, const char* op) {
+  const bool box = kind == VB200_LOSS_RETINANET_BOX || kind == VB200_LOSS_FCOS_BOX, ctrness = kind == VB200_LOSS_FCOS_BOX,
+             labels = kind != VB200_LOSS_RETINANET_BOX;
   VB200_REQUIRE(num_images >= 1 && images, "%s: at least one image", op);
   VB200_REQUIRE(num_anchors >= 0 && width >= 1 && num_anchors * width < ((int64_t)1 << 31), "%s: bad sizes (%lld anchors, width %d)", op,
                 (long long)num_anchors, width);
-  return 0;
-}
-
-int check_call(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors, int width, bool box, bool backward,
-               const char* op) {
-  const int rc = check_sizes(images, num_images, num_anchors, width, op);
-  if (rc) return rc;
+  VB200_REQUIRE(!box || width == 4, "%s: width %d, the box losses take 4", op, width);
   for (int i = 0; i < num_images; ++i) {
-    const vb200_retinanet_loss_image& d = images[i];
+    const vb200_loss_image& d = images[i];
     VB200_REQUIRE(d.num_gt >= 0, "%s: image %d: bad gt count", op, i);
     if (num_anchors == 0) continue;
-    VB200_REQUIRE(d.pred && d.matched && (!backward || d.grad) && (!box || d.anchors), "%s: image %d: null pointer", op, i);
-    VB200_REQUIRE(d.num_gt == 0 || (box ? d.gt != nullptr : d.labels != nullptr), "%s: image %d: null gt pointer", op, i);
-    VB200_REQUIRE(!box || !backward || (reinterpret_cast<uintptr_t>(d.grad) & 15) == 0, "%s: image %d: gradient rows must be 16-byte aligned",
-                  op, i);
-  }
-  return 0;
-}
-
-int check_call(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int width, bool box, bool backward,
-               const char* op) {
-  const int rc = check_sizes(images, num_images, num_anchors, width, op);
-  if (rc) return rc;
-  for (int i = 0; i < num_images; ++i) {
-    const vb200_fcos_loss_image& d = images[i];
-    VB200_REQUIRE(d.num_gt >= 0, "%s: image %d: bad gt count", op, i);
-    if (num_anchors == 0) continue;
-    VB200_REQUIRE(d.pred && d.matched && (!backward || d.grad) && (!box || (d.anchors && d.ctrness && (!backward || d.grad_ctrness))),
+    VB200_REQUIRE(d.pred && d.matched && (!backward || d.grad) && (!box || d.anchors) && (!ctrness || (d.ctrness && (!backward || d.grad_ctrness))),
                   "%s: image %d: null pointer", op, i);
-    VB200_REQUIRE(d.num_gt == 0 || (d.labels && (!box || d.gt)), "%s: image %d: null gt pointer", op, i);
+    VB200_REQUIRE(d.num_gt == 0 || ((!labels || d.labels) && (!box || d.gt)), "%s: image %d: null gt pointer", op, i);
     VB200_REQUIRE(!box || !backward || (reinterpret_cast<uintptr_t>(d.grad) & 15) == 0, "%s: image %d: gradient rows must be 16-byte aligned",
                   op, i);
   }
@@ -535,8 +538,7 @@ int check_call(const vb200_fcos_loss_image* images, int num_images, int64_t num_
 }
 
 // One launch of `kernel` per VB200_LOSS_MAX_IMAGES images, each with its images' descriptors in the plan.
-template <class Image>
-int launch_loss(void (*kernel)(const LossPlan<Image>), const char* name, LossPlan<Image>& plan, const Image* images, int num_images,
+int launch_loss(void (*kernel)(const LossPlan), const char* name, LossPlan& plan, const vb200_loss_image* images, int num_images,
                 cudaStream_t st) {
   if (plan.tiles == 0) return 0;
   for (int done = 0; done < num_images; done += VB200_LOSS_MAX_IMAGES) {
@@ -560,9 +562,8 @@ size_t loss_workspace_bytes(int num_images, int64_t num_anchors, int terms) {
   return terms * align256(slots * sizeof(double)) + align256(slots * sizeof(int));
 }
 
-template <class Image>
-LossPlan<Image> make_plan(int num_images, int64_t num_anchors, int width, const float* weights, bool normalize) {
-  LossPlan<Image> plan;
+LossPlan make_plan(int kind, int num_images, int64_t num_anchors, int width, const float* weights_host, int normalize_by_size) {
+  LossPlan plan;
   plan.num_anchors = num_anchors;
   plan.num_classes = width;
   plan.tiles = tiles_of(num_anchors);
@@ -572,138 +573,69 @@ LossPlan<Image> make_plan(int num_images, int64_t num_anchors, int width, const 
   plan.tile_fg = nullptr;
   plan.grad_loss = plan.grad_loss2 = nullptr;
   plan.num_fg = nullptr;
-  for (int j = 0; j < 4; ++j) plan.weights[j] = weights ? weights[j] : 0.f;
-  plan.normalize = normalize;
+  for (int j = 0; j < 4; ++j) plan.weights[j] = kind == VB200_LOSS_RETINANET_BOX ? weights_host[j] : 0.f;
+  plan.normalize = kind == VB200_LOSS_FCOS_BOX && normalize_by_size != 0;
   return plan;
 }
-
-// The forward of one loss call: the partials of one loss (loss2 null) or two, then the finalize.
-template <Norm kNorm, class Image>
-int loss_forward(void (*kernel)(const LossPlan<Image>), const char* name, LossPlan<Image>& plan, const Image* images, int num_images,
-                 bool box, float* loss, float* loss2, int64_t* num_fg, void* workspace, size_t workspace_bytes, cudaStream_t st,
-                 const char* op) {
-  const int rc = check_call(images, num_images, plan.num_anchors, plan.num_classes, box, false, op);
-  if (rc) return rc;
-  VB200_REQUIRE(loss && num_fg, "%s: null outputs", op);
-  const int terms = loss2 ? 2 : 1;
-  const size_t need = loss_workspace_bytes(num_images, plan.num_anchors, terms);
-  if (need && (!workspace || workspace_bytes < need)) {
-    set_error("%s: workspace of %zu bytes, %zu needed", op, workspace_bytes, need);
-    return VB200_EWORKSPACE;
-  }
-  Carver ws(workspace);
-  plan.partial = ws.take<double>((size_t)num_images * plan.tiles);
-  if (loss2) plan.partial2 = ws.take<double>((size_t)num_images * plan.tiles);
-  plan.tile_fg = ws.take<int>((size_t)num_images * plan.tiles);
-  const int lrc = launch_loss<Image>(kernel, name, plan, images, num_images, st);
-  if (lrc) return lrc;
-  const bool batch = kNorm == Norm::kBatchRecip;      // the [num_images, tiles] slots as one image's
-  loss_finalize_kernel<kNorm><<<1, kFinalizeThreads, 0, st>>>(plan.partial, plan.partial2, plan.tile_fg,
-                                                              batch ? num_images * plan.tiles : plan.tiles, batch ? 1 : num_images,
-                                                              loss, loss2, num_fg);
-  return check_launch("loss_finalize_kernel");
-}
-
-template <class Image>
-int loss_backward(void (*kernel)(const LossPlan<Image>), const char* name, LossPlan<Image>& plan, const Image* images, int num_images,
-                  bool box, const int64_t* num_fg, cudaStream_t st, const char* op) {
-  const int rc = check_call(images, num_images, plan.num_anchors, plan.num_classes, box, true, op);
-  if (rc) return rc;
-  VB200_REQUIRE(num_fg && (plan.grad_loss || plan.grad_loss2), "%s: null gradient or counts", op);
-  plan.num_fg = num_fg;
-  return launch_loss<Image>(kernel, name, plan, images, num_images, st);
-}
-
-using RetinaPlan = LossPlan<vb200_retinanet_loss_image>;
-using FcosPlan = LossPlan<vb200_fcos_loss_image>;
 
 }  // namespace
 }  // namespace vb200
 
 using namespace vb200;
 
-extern "C" size_t vb200_retinanet_cls_loss_workspace_bytes(int num_images, int64_t num_anchors) {
-  return loss_workspace_bytes(num_images, num_anchors, 1);
+extern "C" size_t vb200_head_loss_workspace_bytes(int kind, int num_images, int64_t num_anchors) {
+  const Head h = head_of(kind);
+  return h.forward ? loss_workspace_bytes(num_images, num_anchors, h.terms) : 0;
 }
 
-extern "C" int vb200_retinanet_cls_loss(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors, int num_classes,
-                                        float* loss, int64_t* num_foreground, void* workspace, size_t workspace_bytes,
-                                        vb200_stream stream) {
-  RetinaPlan plan = make_plan<vb200_retinanet_loss_image>(num_images, num_anchors, num_classes, nullptr, false);
-  return loss_forward<Norm::kImageDiv>(focal_loss_kernel<RetinaNetCls, false>, "focal_loss_kernel", plan, images, num_images, false, loss,
-                                       nullptr, num_foreground, workspace, workspace_bytes, (cudaStream_t)stream, "retinanet_cls_loss");
+// The partials of one loss (loss2 null) or two, then the finalize.
+extern "C" int vb200_head_loss(int kind, const vb200_loss_image* images, int num_images, int64_t num_anchors, int width,
+                               const float* weights_host, int normalize_by_size, float* loss, float* loss2, int64_t* num_foreground,
+                               void* workspace, size_t workspace_bytes, vb200_stream stream) {
+  const Head h = head_of(kind);
+  VB200_REQUIRE(h.forward, "head_loss: unknown kind %d", kind);
+  const char* op = h.op;
+  VB200_REQUIRE(kind != VB200_LOSS_RETINANET_BOX || weights_host, "%s: null weights", op);
+  VB200_REQUIRE(h.terms == 1 || loss2, "%s: null outputs", op);
+  VB200_REQUIRE(h.terms == 2 || !loss2, "%s: loss2 is for the FCOS box loss only", op);
+  int rc = check_call(kind, images, num_images, num_anchors, width, false, op);
+  if (rc) return rc;
+  VB200_REQUIRE(loss && num_foreground, "%s: null outputs", op);
+  const size_t need = loss_workspace_bytes(num_images, num_anchors, h.terms);
+  if (need && (!workspace || workspace_bytes < need)) {
+    set_error("%s: workspace of %zu bytes, %zu needed", op, workspace_bytes, need);
+    return VB200_EWORKSPACE;
+  }
+  LossPlan plan = make_plan(kind, num_images, num_anchors, width, weights_host, normalize_by_size);
+  Carver ws(workspace);
+  plan.partial = ws.take<double>((size_t)num_images * plan.tiles);
+  if (loss2) plan.partial2 = ws.take<double>((size_t)num_images * plan.tiles);
+  plan.tile_fg = ws.take<int>((size_t)num_images * plan.tiles);
+  const cudaStream_t st = (cudaStream_t)stream;
+  rc = launch_loss(h.forward, h.kernel, plan, images, num_images, st);
+  if (rc) return rc;
+  const bool batch = h.norm == Norm::kBatchRecip;     // the [num_images, tiles] slots as one image's
+  const auto finalize = batch ? loss_finalize_kernel<Norm::kBatchRecip>
+                        : h.norm == Norm::kImageRecip ? loss_finalize_kernel<Norm::kImageRecip> : loss_finalize_kernel<Norm::kImageDiv>;
+  finalize<<<1, kFinalizeThreads, 0, st>>>(plan.partial, plan.partial2, plan.tile_fg, batch ? num_images * plan.tiles : plan.tiles,
+                                          batch ? 1 : num_images, loss, loss2, num_foreground);
+  return check_launch("loss_finalize_kernel");
 }
 
-extern "C" int vb200_retinanet_cls_loss_backward(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
-                                                 int num_classes, const float* grad_loss, const int64_t* num_foreground,
-                                                 vb200_stream stream) {
-  RetinaPlan plan = make_plan<vb200_retinanet_loss_image>(num_images, num_anchors, num_classes, nullptr, false);
+extern "C" int vb200_head_loss_backward(int kind, const vb200_loss_image* images, int num_images, int64_t num_anchors, int width,
+                                        const float* weights_host, int normalize_by_size, const float* grad_loss,
+                                        const float* grad_loss2, const int64_t* num_foreground, vb200_stream stream) {
+  const Head h = head_of(kind);
+  VB200_REQUIRE(h.forward, "head_loss_backward: unknown kind %d", kind);
+  const char* op = h.op_backward;
+  VB200_REQUIRE(kind != VB200_LOSS_RETINANET_BOX || weights_host, "%s: null weights", op);
+  VB200_REQUIRE(h.terms == 2 || !grad_loss2, "%s: grad_loss2 is for the FCOS box loss only", op);
+  const int rc = check_call(kind, images, num_images, num_anchors, width, true, op);
+  if (rc) return rc;
+  VB200_REQUIRE(num_foreground && (grad_loss || grad_loss2), "%s: null gradient or counts", op);
+  LossPlan plan = make_plan(kind, num_images, num_anchors, width, weights_host, normalize_by_size);
   plan.grad_loss = grad_loss;
-  return loss_backward(focal_loss_kernel<RetinaNetCls, true>, "focal_loss_kernel", plan, images, num_images, false, num_foreground,
-                       (cudaStream_t)stream, "retinanet_cls_loss_backward");
-}
-
-extern "C" size_t vb200_retinanet_box_loss_workspace_bytes(int num_images, int64_t num_anchors) {
-  return loss_workspace_bytes(num_images, num_anchors, 1);
-}
-
-extern "C" int vb200_retinanet_box_loss(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
-                                        const float* weights_host, float* loss, int64_t* num_foreground, void* workspace,
-                                        size_t workspace_bytes, vb200_stream stream) {
-  VB200_REQUIRE(weights_host, "retinanet_box_loss: null weights");
-  RetinaPlan plan = make_plan<vb200_retinanet_loss_image>(num_images, num_anchors, 4, weights_host, false);
-  return loss_forward<Norm::kImageRecip>(box_loss_kernel<false>, "box_loss_kernel", plan, images, num_images, true, loss, nullptr,
-                                         num_foreground, workspace, workspace_bytes, (cudaStream_t)stream, "retinanet_box_loss");
-}
-
-extern "C" int vb200_retinanet_box_loss_backward(const vb200_retinanet_loss_image* images, int num_images, int64_t num_anchors,
-                                                 const float* weights_host, const float* grad_loss, const int64_t* num_foreground,
-                                                 vb200_stream stream) {
-  VB200_REQUIRE(weights_host, "retinanet_box_loss_backward: null weights");
-  RetinaPlan plan = make_plan<vb200_retinanet_loss_image>(num_images, num_anchors, 4, weights_host, false);
-  plan.grad_loss = grad_loss;
-  return loss_backward(box_loss_kernel<true>, "box_loss_kernel", plan, images, num_images, true, num_foreground, (cudaStream_t)stream,
-                       "retinanet_box_loss_backward");
-}
-
-extern "C" size_t vb200_fcos_cls_loss_workspace_bytes(int num_images, int64_t num_anchors) {
-  return loss_workspace_bytes(num_images, num_anchors, 1);
-}
-
-extern "C" int vb200_fcos_cls_loss(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int num_classes, float* loss,
-                                   int64_t* num_foreground, void* workspace, size_t workspace_bytes, vb200_stream stream) {
-  FcosPlan plan = make_plan<vb200_fcos_loss_image>(num_images, num_anchors, num_classes, nullptr, false);
-  return loss_forward<Norm::kBatchRecip>(focal_loss_kernel<FcosCls, false>, "focal_loss_kernel", plan, images, num_images, false, loss,
-                                         nullptr, num_foreground, workspace, workspace_bytes, (cudaStream_t)stream, "fcos_cls_loss");
-}
-
-extern "C" int vb200_fcos_cls_loss_backward(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int num_classes,
-                                            const float* grad_loss, const int64_t* num_foreground, vb200_stream stream) {
-  FcosPlan plan = make_plan<vb200_fcos_loss_image>(num_images, num_anchors, num_classes, nullptr, false);
-  plan.grad_loss = grad_loss;
-  return loss_backward(focal_loss_kernel<FcosCls, true>, "focal_loss_kernel", plan, images, num_images, false, num_foreground,
-                       (cudaStream_t)stream, "fcos_cls_loss_backward");
-}
-
-extern "C" size_t vb200_fcos_box_loss_workspace_bytes(int num_images, int64_t num_anchors) {
-  return loss_workspace_bytes(num_images, num_anchors, 2);
-}
-
-extern "C" int vb200_fcos_box_loss(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors, int normalize_by_size,
-                                   float* loss_box, float* loss_ctrness, int64_t* num_foreground, void* workspace, size_t workspace_bytes,
-                                   vb200_stream stream) {
-  VB200_REQUIRE(loss_ctrness, "fcos_box_loss: null outputs");
-  FcosPlan plan = make_plan<vb200_fcos_loss_image>(num_images, num_anchors, 4, nullptr, normalize_by_size != 0);
-  return loss_forward<Norm::kBatchRecip>(fcos_box_loss_kernel<false>, "fcos_box_loss_kernel", plan, images, num_images, true, loss_box,
-                                         loss_ctrness, num_foreground, workspace, workspace_bytes, (cudaStream_t)stream, "fcos_box_loss");
-}
-
-extern "C" int vb200_fcos_box_loss_backward(const vb200_fcos_loss_image* images, int num_images, int64_t num_anchors,
-                                            int normalize_by_size, const float* grad_box, const float* grad_ctrness,
-                                            const int64_t* num_foreground, vb200_stream stream) {
-  FcosPlan plan = make_plan<vb200_fcos_loss_image>(num_images, num_anchors, 4, nullptr, normalize_by_size != 0);
-  plan.grad_loss = grad_box;
-  plan.grad_loss2 = grad_ctrness;
-  return loss_backward(fcos_box_loss_kernel<true>, "fcos_box_loss_kernel", plan, images, num_images, true, num_foreground,
-                       (cudaStream_t)stream, "fcos_box_loss_backward");
+  plan.grad_loss2 = grad_loss2;
+  plan.num_fg = num_foreground;
+  return launch_loss(h.backward, h.kernel, plan, images, num_images, (cudaStream_t)stream);
 }

@@ -966,9 +966,9 @@ extern "C" int vb200_roi_pool_backward(const void* grad, const void* rois, const
   });
 }
 
-extern "C" int vb200_ps_roi_pool_backward_ex(const void* grad, const void* rois, void* grad_input, int dtype, int batch, int channels,
-                                             int height, int width, int num_rois, int pooled_h, int pooled_w, double spatial_scale,
-                                             int deterministic, void* workspace, size_t workspace_bytes, vb200_stream stream) {
+extern "C" int vb200_ps_roi_pool_backward(const void* grad, const void* rois, void* grad_input, int dtype, int batch, int channels,
+                                          int height, int width, int num_rois, int pooled_h, int pooled_w, double spatial_scale,
+                                          int deterministic, void* workspace, size_t workspace_bytes, vb200_stream stream) {
   size_t bytes;
   if (int rc = bwd_prologue("ps_roi_pool_backward", grad_input, dtype, batch, channels, height, width, num_rois, pooled_h, pooled_w,
                             bytes))
@@ -1001,13 +1001,6 @@ extern "C" int vb200_ps_roi_pool_backward_ex(const void* grad, const void* rois,
                                                    pooled_h, pooled_w, Cout, (typename Acc<T>::type)spatial_scale);
     return check_launch("ps_roi_pool_bwd_kernel");
   });
-}
-
-extern "C" int vb200_ps_roi_pool_backward(const void* grad, const void* rois, void* grad_input, int dtype, int batch, int channels,
-                                          int height, int width, int num_rois, int pooled_h, int pooled_w, double spatial_scale,
-                                          vb200_stream stream) {
-  return vb200_ps_roi_pool_backward_ex(grad, rois, grad_input, dtype, batch, channels, height, width, num_rois, pooled_h, pooled_w,
-                                       spatial_scale, 0, nullptr, 0, stream);
 }
 
 extern "C" int vb200_roi_backward_deterministic_supported(int dtype, int height, int width) {

@@ -80,7 +80,6 @@ int max_smem_optin() { return attr().smem_optin; }
 extern "C" int vb200_abi_version(void) { return VB200_ABI_VERSION; }
 extern "C" const char* vb200_last_error(void) { return vb200::last_error_buf(); }
 extern "C" uint64_t vb200_launch_count(void) { return vb200::g_launch_count.load(); }
-extern "C" int vb200_env_generation(void) { return vb200::env_generation(); }
 extern "C" void vb200_reload_env(void) {
   std::lock_guard<std::mutex> lk(vb200::g_env_mu);
   vb200::load_env_locked();

@@ -182,9 +182,9 @@ at::Tensor ps_roi_pool_backward(const at::Tensor& grad, const at::Tensor& rois, 
   const bool det = roi_backward_deterministic(dt, height, width, "ps_roi_pool_backward: a grad_input row too wide for shared memory");
   const size_t wsb = vb200_roi_backward_workspace_bytes((int)r.size(0), (int)pooled_height, (int)pooled_width, 1);
   at::Tensor ws = workspace(wsb, grad);
-  check_rc(vb200_ps_roi_pool_backward_ex(g.data_ptr(), r.data_ptr(), grad_input.data_ptr(), dt, (int)batch_size, (int)channels,
-                                         (int)height, (int)width, (int)r.size(0), (int)pooled_height, (int)pooled_width, spatial_scale,
-                                         det ? 1 : 0, wsb ? ws.data_ptr() : nullptr, wsb, cur_stream()),
+  check_rc(vb200_ps_roi_pool_backward(g.data_ptr(), r.data_ptr(), grad_input.data_ptr(), dt, (int)batch_size, (int)channels,
+                                      (int)height, (int)width, (int)r.size(0), (int)pooled_height, (int)pooled_width, spatial_scale,
+                                      det ? 1 : 0, wsb ? ws.data_ptr() : nullptr, wsb, cur_stream()),
            "ps_roi_pool_backward");
   return grad_input;
 }
@@ -625,12 +625,12 @@ at::Tensor deform_conv2d_impl(const at::Tensor& input, const at::Tensor& weight,
   } else {
     outs[0] = out.data_ptr();
   }
-  check_rc(vb200_deform_conv2d_forward_gather(input_c.data_ptr(), weight_c.data_ptr(), packed.defined() ? packed.data_ptr() : nullptr,
-                                              nhwc_ok ? 1 : 0, offset_c.data_ptr(), use_mask ? mask_c.data_ptr() : nullptr,
-                                              bias_c.data_ptr(), outs, n_outs, dt, (int)batch, (int)c_in, (int)in_h, (int)in_w, (int)c_out,
-                                              (int)kh, (int)kw, (int)stride_h, (int)stride_w, (int)pad_h, (int)pad_w, (int)dilation_h,
-                                              (int)dilation_w, (int)n_weight_grps, (int)n_offset_grps, use_mask ? 1 : 0,
-                                              wsb ? ws.data_ptr() : nullptr, wsb, cur_stream()),
+  check_rc(vb200_deform_conv2d_forward(input_c.data_ptr(), weight_c.data_ptr(), packed.defined() ? packed.data_ptr() : nullptr,
+                                       nhwc_ok ? 1 : 0, offset_c.data_ptr(), use_mask ? mask_c.data_ptr() : nullptr,
+                                       bias_c.data_ptr(), outs, n_outs, dt, (int)batch, (int)c_in, (int)in_h, (int)in_w, (int)c_out,
+                                       (int)kh, (int)kw, (int)stride_h, (int)stride_w, (int)pad_h, (int)pad_w, (int)dilation_h,
+                                       (int)dilation_w, (int)n_weight_grps, (int)n_offset_grps, use_mask ? 1 : 0,
+                                       wsb ? ws.data_ptr() : nullptr, wsb, cur_stream()),
            "deform_conv2d");
   return out;
 }
@@ -725,10 +725,10 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> deform_co
                                                                                     (int)dilation_h, (int)dilation_w, (int)n_offset_grps)
                               : 0;
     at::Tensor ws = gather ? workspace(wsb, input_c) : at::Tensor();
-    check_rc(vb200_deform_conv2d_backward_inputs_ex(buf.data_ptr(), in_b.data_ptr(), off_b.data_ptr(), mk, gi_b.data_ptr(), go_b.data_ptr(), gm,
-                                                    dt, (int)nb, (int)C_in, (int)H, (int)W, (int)kh, (int)kw, (int)stride_h, (int)stride_w,
-                                                    (int)pad_h, (int)pad_w, (int)dilation_h, (int)dilation_w, (int)n_offset_grps,
-                                                    use_mask ? 1 : 0, gather ? 1 : 0, gather ? ws.data_ptr() : nullptr, wsb, cur_stream()),
+    check_rc(vb200_deform_conv2d_backward_inputs(buf.data_ptr(), in_b.data_ptr(), off_b.data_ptr(), mk, gi_b.data_ptr(), go_b.data_ptr(), gm,
+                                                 dt, (int)nb, (int)C_in, (int)H, (int)W, (int)kh, (int)kw, (int)stride_h, (int)stride_w,
+                                                 (int)pad_h, (int)pad_w, (int)dilation_h, (int)dilation_w, (int)n_offset_grps,
+                                                 use_mask ? 1 : 0, gather ? 1 : 0, gather ? ws.data_ptr() : nullptr, wsb, cur_stream()),
              "deform_conv2d_backward");
     // columns for grad_weight (the buffer is reused)
     check_rc(vb200_deform_conv2d_sample_columns(in_b.data_ptr(), off_b.data_ptr(), mk, buf.data_ptr(), dt, (int)nb, (int)C_in, (int)H, (int)W,
@@ -1002,13 +1002,17 @@ std::vector<at::Tensor> fcos_match(at::TensorList gt_boxes, at::TensorList ancho
   return out;
 }
 
-// ---- RetinaNet head losses (retinanet.py:158-189, 272-302) --------------------------------------------------------------
+// ---- single-stage detector head losses (retinanet.py:158-189, 272-302; fcos.py:52-125) ----------------------------------
 // pred: cls_logits [B, A, C] or bbox_regression [B, A, 4], fp32 on one GPU with dense rows (unit stride in the last dimension,
-// rows of its width).  matched_idxs: one int64 [A] per image; labels: one int64 [M_i] per image (classification); gt_boxes /
-// anchors: one fp32 [M_i, 4] / [A, 4] per image (regression).  Returns the 0-dim loss and the int64 [B] foreground counts the
-// backward takes; the backward returns the dense gradient of pred.
-std::vector<vb200_retinanet_loss_image> loss_images(const at::Tensor& pred, int64_t width, at::TensorList matched_idxs, at::TensorList labels,
-                                                    at::TensorList anchors, at::TensorList gt_boxes, bool box, const char* op) {
+// rows of its width).  matched_idxs: one int64 [A] per image; labels: one int64 [M_i] per image on that GPU (not RetinaNet's
+// box loss; as many rows as the image's gt boxes in FCOS's); gt_boxes / anchors: one fp32 [M_i, 4] / [A, 4] per image (box
+// losses); ctrness (FCOS's box loss) fp32 [B, A, 1] on the same GPU, any strides.
+std::vector<vb200_loss_image> loss_images(int kind, const at::Tensor& pred, const at::Tensor* ctrness, at::TensorList matched_idxs,
+                                          at::TensorList labels, at::TensorList anchors, at::TensorList gt_boxes, const char* op) {
+  const bool box = kind == VB200_LOSS_RETINANET_BOX || kind == VB200_LOSS_FCOS_BOX;
+  if (!box) TORCH_CHECK(pred.dim() == 3, op, ": cls_logits must be [B, A, C]");
+  if (kind == VB200_LOSS_FCOS_CLS || kind == VB200_LOSS_FCOS_BOX) TORCH_CHECK(labels.size() == matched_idxs.size(), op, ": one labels tensor per image");
+  const int64_t width = box ? 4 : pred.size(2);
   TORCH_CHECK(pred.is_cuda() && pred.scalar_type() == at::kFloat && pred.dim() == 3 && pred.size(0) >= 1, op,
               ": the predictions must be a CUDA float32 [B, A, ", box ? "4" : "C", "] tensor with B >= 1");
   const int64_t B = pred.size(0), A = pred.size(1);
@@ -1019,9 +1023,13 @@ std::vector<vb200_retinanet_loss_image> loss_images(const at::Tensor& pred, int6
                   (!box || (int64_t)anchors.size() == B),
               op, ": one matched_idxs and one target per image");
   const auto same_gpu = [&](const at::Tensor& t) { return t.is_cuda() && t.get_device() == pred.get_device(); };
-  std::vector<vb200_retinanet_loss_image> desc((size_t)B);
+  if (ctrness)
+    TORCH_CHECK(same_gpu(*ctrness) && ctrness->scalar_type() == at::kFloat && ctrness->dim() == 3 && ctrness->size(0) == B &&
+                    ctrness->size(1) == A && ctrness->size(2) == 1,
+                op, ": bbox_ctrness must be a float32 [B, A, 1] tensor on the predictions' GPU");
+  std::vector<vb200_loss_image> desc((size_t)B);
   for (int64_t i = 0; i < B; ++i) {
-    vb200_retinanet_loss_image& d = desc[(size_t)i];
+    vb200_loss_image& d = desc[(size_t)i];
     d = {};
     d.pred = pred.data_ptr<float>() + i * pred.stride(0);
     const at::Tensor& m = matched_idxs[i];
@@ -1042,225 +1050,146 @@ std::vector<vb200_retinanet_loss_image> loss_images(const at::Tensor& pred, int6
       d.anchors = a.data_ptr<float>();
       d.anchor_stride[0] = a.stride(0);
       d.anchor_stride[1] = a.stride(1);
-    } else {
+    }
+    if (kind != VB200_LOSS_RETINANET_BOX) {
       const at::Tensor& l = labels[i];
-      TORCH_CHECK(same_gpu(l) && l.scalar_type() == at::kLong && l.dim() == 1, op, ": labels must be int64 [M] tensors on the predictions' GPU");
+      TORCH_CHECK(same_gpu(l) && l.scalar_type() == at::kLong && l.dim() == 1 && (!box || l.size(0) == d.num_gt), op,
+                  ": labels must be int64 [M] tensors on the predictions' GPU", box ? ", one per gt box" : "");
       d.labels = l.data_ptr<int64_t>();
       d.label_stride = l.stride(0);
       d.num_gt = l.size(0);
     }
-  }
-  return desc;
-}
-
-std::array<float, 4> coder_weights(at::ArrayRef<double> weights, const char* op) {
-  TORCH_CHECK(weights.size() == 4, op, ": four box coder weights");
-  return {(float)weights[0], (float)weights[1], (float)weights[2], (float)weights[3]};
-}
-
-std::tuple<at::Tensor, at::Tensor> retinanet_cls_loss(const at::Tensor& cls_logits, at::TensorList matched_idxs, at::TensorList labels) {
-  TORCH_CHECK(cls_logits.dim() == 3, "retinanet_cls_loss: cls_logits must be [B, A, C]");
-  auto desc = loss_images(cls_logits, cls_logits.size(2), matched_idxs, labels, {}, {}, false, "retinanet_cls_loss");
-  at::cuda::CUDAGuard guard(cls_logits.device());
-  const int B = (int)desc.size();
-  const int64_t A = cls_logits.size(1);
-  at::Tensor loss = at::empty({}, cls_logits.options());
-  at::Tensor counts = at::empty({B}, cls_logits.options().dtype(at::kLong));
-  const size_t wsb = vb200_retinanet_cls_loss_workspace_bytes(B, A);
-  at::Tensor ws = workspace(wsb, cls_logits);
-  check_rc(vb200_retinanet_cls_loss(desc.data(), B, A, (int)cls_logits.size(2), loss.data_ptr<float>(), counts.data_ptr<int64_t>(),
-                                    ws.data_ptr(), wsb, cur_stream()),
-           "retinanet_cls_loss");
-  return std::make_tuple(loss, counts);
-}
-
-at::Tensor retinanet_cls_loss_backward(const at::Tensor& grad, const at::Tensor& cls_logits, at::TensorList matched_idxs, at::TensorList labels,
-                                       const at::Tensor& num_foreground) {
-  TORCH_CHECK(cls_logits.dim() == 3, "retinanet_cls_loss_backward: cls_logits must be [B, A, C]");
-  auto desc = loss_images(cls_logits, cls_logits.size(2), matched_idxs, labels, {}, {}, false, "retinanet_cls_loss_backward");
-  const int B = (int)desc.size();
-  TORCH_CHECK(grad.is_cuda() && grad.get_device() == cls_logits.get_device() && grad.scalar_type() == at::kFloat && grad.numel() == 1,
-              "retinanet_cls_loss_backward: the gradient must be one float32 value on the logits' GPU");
-  TORCH_CHECK(num_foreground.is_cuda() && num_foreground.get_device() == cls_logits.get_device() && num_foreground.scalar_type() == at::kLong &&
-                  num_foreground.dim() == 1 && num_foreground.size(0) == B,
-              "retinanet_cls_loss_backward: num_foreground must be the forward's int64 [B] counts");
-  at::cuda::CUDAGuard guard(cls_logits.device());
-  at::Tensor g = grad.contiguous(), n = num_foreground.contiguous();
-  at::Tensor out = at::empty(cls_logits.sizes(), cls_logits.options());
-  for (int i = 0; i < B; ++i) desc[(size_t)i].grad = out.data_ptr<float>() + (int64_t)i * out.stride(0);
-  check_rc(vb200_retinanet_cls_loss_backward(desc.data(), B, cls_logits.size(1), (int)cls_logits.size(2), g.data_ptr<float>(),
-                                             n.data_ptr<int64_t>(), cur_stream()),
-           "retinanet_cls_loss_backward");
-  return out;
-}
-
-std::tuple<at::Tensor, at::Tensor> retinanet_box_loss(const at::Tensor& bbox_regression, at::TensorList anchors, at::TensorList gt_boxes,
-                                                      at::TensorList matched_idxs, at::ArrayRef<double> weights) {
-  auto desc = loss_images(bbox_regression, 4, matched_idxs, {}, anchors, gt_boxes, true, "retinanet_box_loss");
-  const auto w = coder_weights(weights, "retinanet_box_loss");
-  at::cuda::CUDAGuard guard(bbox_regression.device());
-  const int B = (int)desc.size();
-  const int64_t A = bbox_regression.size(1);
-  at::Tensor loss = at::empty({}, bbox_regression.options());
-  at::Tensor counts = at::empty({B}, bbox_regression.options().dtype(at::kLong));
-  const size_t wsb = vb200_retinanet_box_loss_workspace_bytes(B, A);
-  at::Tensor ws = workspace(wsb, bbox_regression);
-  check_rc(vb200_retinanet_box_loss(desc.data(), B, A, w.data(), loss.data_ptr<float>(), counts.data_ptr<int64_t>(), ws.data_ptr(), wsb,
-                                    cur_stream()),
-           "retinanet_box_loss");
-  return std::make_tuple(loss, counts);
-}
-
-at::Tensor retinanet_box_loss_backward(const at::Tensor& grad, const at::Tensor& bbox_regression, at::TensorList anchors, at::TensorList gt_boxes,
-                                       at::TensorList matched_idxs, at::ArrayRef<double> weights, const at::Tensor& num_foreground) {
-  auto desc = loss_images(bbox_regression, 4, matched_idxs, {}, anchors, gt_boxes, true, "retinanet_box_loss_backward");
-  const auto w = coder_weights(weights, "retinanet_box_loss_backward");
-  const int B = (int)desc.size();
-  TORCH_CHECK(grad.is_cuda() && grad.get_device() == bbox_regression.get_device() && grad.scalar_type() == at::kFloat && grad.numel() == 1,
-              "retinanet_box_loss_backward: the gradient must be one float32 value on the regression's GPU");
-  TORCH_CHECK(num_foreground.is_cuda() && num_foreground.get_device() == bbox_regression.get_device() &&
-                  num_foreground.scalar_type() == at::kLong && num_foreground.dim() == 1 && num_foreground.size(0) == B,
-              "retinanet_box_loss_backward: num_foreground must be the forward's int64 [B] counts");
-  at::cuda::CUDAGuard guard(bbox_regression.device());
-  at::Tensor g = grad.contiguous(), n = num_foreground.contiguous();
-  at::Tensor out = at::empty(bbox_regression.sizes(), bbox_regression.options());
-  for (int i = 0; i < B; ++i) desc[(size_t)i].grad = out.data_ptr<float>() + (int64_t)i * out.stride(0);
-  check_rc(vb200_retinanet_box_loss_backward(desc.data(), B, bbox_regression.size(1), w.data(), g.data_ptr<float>(), n.data_ptr<int64_t>(),
-                                             cur_stream()),
-           "retinanet_box_loss_backward");
-  return out;
-}
-
-// ---- FCOS head losses (fcos.py:52-125) ----------------------------------------------------------------------------------
-// cls_logits [B, A, C] / bbox_regression [B, A, 4] as loss_images takes them; bbox_ctrness (box call) fp32 [B, A, 1] on the
-// same GPU, any strides; labels one int64 [M_i] per image on that GPU (as many rows as the image's gt boxes in the box call).
-// Each forward returns its 0-dim losses and the batch's foreground count (int64, 0-dim) that its backward takes.
-std::vector<vb200_fcos_loss_image> fcos_loss_images(const at::Tensor& pred, int64_t width, const at::Tensor* ctrness, at::TensorList matched_idxs,
-                                                    at::TensorList labels, at::TensorList anchors, at::TensorList gt_boxes, const char* op) {
-  const bool box = ctrness != nullptr;
-  TORCH_CHECK(labels.size() == matched_idxs.size(), op, ": one labels tensor per image");
-  const auto base = loss_images(pred, width, matched_idxs, labels, anchors, gt_boxes, box, op);
-  const int64_t A = pred.size(1);
-  if (box)
-    TORCH_CHECK(ctrness->is_cuda() && ctrness->get_device() == pred.get_device() && ctrness->scalar_type() == at::kFloat && ctrness->dim() == 3 &&
-                    ctrness->size(0) == pred.size(0) && ctrness->size(1) == A && ctrness->size(2) == 1,
-                op, ": bbox_ctrness must be a float32 [B, A, 1] tensor on the predictions' GPU");
-  std::vector<vb200_fcos_loss_image> desc(base.size());
-  for (size_t i = 0; i < base.size(); ++i) {
-    const vb200_retinanet_loss_image& r = base[i];
-    vb200_fcos_loss_image& d = desc[i];
-    d = {};
-    d.pred = r.pred;
-    d.matched = r.matched;
-    d.matched_stride = r.matched_stride;
-    const at::Tensor& l = labels[i];
-    TORCH_CHECK(l.is_cuda() && l.get_device() == pred.get_device() && l.scalar_type() == at::kLong && l.dim() == 1 && (!box || l.size(0) == r.num_gt),
-                op, ": labels must be int64 [M] tensors on the predictions' GPU, one per gt box");
-    d.labels = l.data_ptr<int64_t>();
-    d.label_stride = l.stride(0);
-    d.num_gt = l.size(0);
-    if (box) {
-      d.ctrness = ctrness->data_ptr<float>() + (int64_t)i * ctrness->stride(0);
+    if (ctrness) {
+      d.ctrness = ctrness->data_ptr<float>() + i * ctrness->stride(0);
       d.ctrness_stride = ctrness->stride(1);
-      d.gt = r.gt;
-      d.anchors = r.anchors;
-      for (int k = 0; k < 2; ++k) {
-        d.gt_stride[k] = r.gt_stride[k];
-        d.anchor_stride[k] = r.anchor_stride[k];
-      }
     }
   }
   return desc;
 }
 
-void check_fcos_backward(const at::Tensor& grad, const at::Tensor& pred, const at::Tensor& num_foreground, const char* op) {
+std::array<float, 4> coder_weights(int kind, at::ArrayRef<double> weights, const char* op) {
+  if (kind != VB200_LOSS_RETINANET_BOX) return {};
+  TORCH_CHECK(weights.size() == 4, op, ": four box coder weights");
+  return {(float)weights[0], (float)weights[1], (float)weights[2], (float)weights[3]};
+}
+
+// The forward of one head loss: its 0-dim loss (and FCOS box's 0-dim centre-ness loss, else undefined) and the foreground
+// counts the backward takes, int64 [B] per image for RetinaNet, int64 0-dim for the batch for FCOS.
+std::tuple<at::Tensor, at::Tensor, at::Tensor> head_loss(int kind, const at::Tensor& pred, const at::Tensor* ctrness, at::TensorList matched_idxs,
+                                                         at::TensorList labels, at::TensorList anchors, at::TensorList gt_boxes,
+                                                         at::ArrayRef<double> weights, bool normalize_by_size, const char* op) {
+  auto desc = loss_images(kind, pred, ctrness, matched_idxs, labels, anchors, gt_boxes, op);
+  const auto w = coder_weights(kind, weights, op);
+  at::cuda::CUDAGuard guard(pred.device());
+  const int B = (int)desc.size();
+  const int64_t A = pred.size(1);
+  const bool fcos = kind == VB200_LOSS_FCOS_CLS || kind == VB200_LOSS_FCOS_BOX;
+  at::Tensor loss = at::empty({}, pred.options()), loss2 = ctrness ? at::empty({}, pred.options()) : at::Tensor();
+  at::Tensor counts = fcos ? at::empty({}, pred.options().dtype(at::kLong)) : at::empty({B}, pred.options().dtype(at::kLong));
+  const size_t wsb = vb200_head_loss_workspace_bytes(kind, B, A);
+  at::Tensor ws = workspace(wsb, pred);
+  check_rc(vb200_head_loss(kind, desc.data(), B, A, (int)pred.size(2), w.data(), normalize_by_size ? 1 : 0, loss.data_ptr<float>(),
+                           ctrness ? loss2.data_ptr<float>() : nullptr, counts.data_ptr<int64_t>(), ws.data_ptr(), wsb, cur_stream()),
+           op);
+  return std::make_tuple(loss, loss2, counts);
+}
+
+void check_loss_grad(int kind, const at::Tensor& grad, const at::Tensor& pred, const at::Tensor& num_foreground, const char* op) {
+  const bool fcos = kind == VB200_LOSS_FCOS_CLS || kind == VB200_LOSS_FCOS_BOX;
   TORCH_CHECK(grad.is_cuda() && grad.get_device() == pred.get_device() && grad.scalar_type() == at::kFloat && grad.numel() == 1, op,
-              ": each incoming gradient must be one float32 value on the predictions' GPU");
+              fcos                                ? ": each incoming gradient must be one float32 value on the predictions' GPU"
+              : kind == VB200_LOSS_RETINANET_CLS ? ": the gradient must be one float32 value on the logits' GPU"
+                                                  : ": the gradient must be one float32 value on the regression's GPU");
   TORCH_CHECK(num_foreground.is_cuda() && num_foreground.get_device() == pred.get_device() && num_foreground.scalar_type() == at::kLong &&
-                  num_foreground.numel() == 1,
-              op, ": num_foreground must be the forward's int64 count");
+                  (fcos ? num_foreground.numel() == 1 : num_foreground.dim() == 1 && num_foreground.size(0) == pred.size(0)),
+              op, fcos ? ": num_foreground must be the forward's int64 count" : ": num_foreground must be the forward's int64 [B] counts");
+}
+
+// The backward of one head loss: the dense gradient of pred (and of ctrness for FCOS's box loss, else undefined).  An
+// undefined incoming gradient counts as zero: its rows are 0 (both undefined: no launch).
+std::tuple<at::Tensor, at::Tensor> head_loss_backward(int kind, const std::optional<at::Tensor>& grad, const std::optional<at::Tensor>& grad2,
+                                                      const at::Tensor& pred, const at::Tensor* ctrness, at::TensorList matched_idxs,
+                                                      at::TensorList labels, at::TensorList anchors, at::TensorList gt_boxes,
+                                                      at::ArrayRef<double> weights, bool normalize_by_size, const at::Tensor& num_foreground,
+                                                      const char* op) {
+  auto desc = loss_images(kind, pred, ctrness, matched_idxs, labels, anchors, gt_boxes, op);
+  const auto w = coder_weights(kind, weights, op);
+  const bool has = grad.has_value() && grad->defined(), has2 = grad2.has_value() && grad2->defined();
+  at::cuda::CUDAGuard guard(pred.device());
+  if (!has && !has2)
+    return std::make_tuple(at::zeros(pred.sizes(), pred.options()), ctrness ? at::zeros(ctrness->sizes(), ctrness->options()) : at::Tensor());
+  at::Tensor g, g2;
+  if (has) {
+    check_loss_grad(kind, *grad, pred, num_foreground, op);
+    g = grad->contiguous();
+  }
+  if (has2) {
+    check_loss_grad(kind, *grad2, pred, num_foreground, op);
+    g2 = grad2->contiguous();
+  }
+  const int B = (int)desc.size();
+  at::Tensor n = num_foreground.contiguous();
+  at::Tensor out = at::empty(pred.sizes(), pred.options());
+  at::Tensor out2 = ctrness ? at::empty(ctrness->sizes(), ctrness->options()) : at::Tensor();
+  for (int i = 0; i < B; ++i) {
+    desc[(size_t)i].grad = out.data_ptr<float>() + (int64_t)i * out.stride(0);
+    if (ctrness) desc[(size_t)i].grad_ctrness = out2.data_ptr<float>() + (int64_t)i * out2.stride(0);
+  }
+  check_rc(vb200_head_loss_backward(kind, desc.data(), B, pred.size(1), (int)pred.size(2), w.data(), normalize_by_size ? 1 : 0,
+                                    has ? g.data_ptr<float>() : nullptr, has2 ? g2.data_ptr<float>() : nullptr, n.data_ptr<int64_t>(),
+                                    cur_stream()),
+           op);
+  return std::make_tuple(out, out2);
+}
+
+std::tuple<at::Tensor, at::Tensor> retinanet_cls_loss(const at::Tensor& cls_logits, at::TensorList matched_idxs, at::TensorList labels) {
+  const auto r = head_loss(VB200_LOSS_RETINANET_CLS, cls_logits, nullptr, matched_idxs, labels, {}, {}, {}, false, "retinanet_cls_loss");
+  return std::make_tuple(std::get<0>(r), std::get<2>(r));
+}
+
+at::Tensor retinanet_cls_loss_backward(const at::Tensor& grad, const at::Tensor& cls_logits, at::TensorList matched_idxs, at::TensorList labels,
+                                       const at::Tensor& num_foreground) {
+  return std::get<0>(head_loss_backward(VB200_LOSS_RETINANET_CLS, grad, std::nullopt, cls_logits, nullptr, matched_idxs, labels, {}, {}, {},
+                                        false, num_foreground, "retinanet_cls_loss_backward"));
+}
+
+std::tuple<at::Tensor, at::Tensor> retinanet_box_loss(const at::Tensor& bbox_regression, at::TensorList anchors, at::TensorList gt_boxes,
+                                                      at::TensorList matched_idxs, at::ArrayRef<double> weights) {
+  const auto r = head_loss(VB200_LOSS_RETINANET_BOX, bbox_regression, nullptr, matched_idxs, {}, anchors, gt_boxes, weights, false,
+                           "retinanet_box_loss");
+  return std::make_tuple(std::get<0>(r), std::get<2>(r));
+}
+
+at::Tensor retinanet_box_loss_backward(const at::Tensor& grad, const at::Tensor& bbox_regression, at::TensorList anchors, at::TensorList gt_boxes,
+                                       at::TensorList matched_idxs, at::ArrayRef<double> weights, const at::Tensor& num_foreground) {
+  return std::get<0>(head_loss_backward(VB200_LOSS_RETINANET_BOX, grad, std::nullopt, bbox_regression, nullptr, matched_idxs, {}, anchors,
+                                        gt_boxes, weights, false, num_foreground, "retinanet_box_loss_backward"));
 }
 
 std::tuple<at::Tensor, at::Tensor> fcos_cls_loss(const at::Tensor& cls_logits, at::TensorList matched_idxs, at::TensorList labels) {
-  TORCH_CHECK(cls_logits.dim() == 3, "fcos_cls_loss: cls_logits must be [B, A, C]");
-  auto desc = fcos_loss_images(cls_logits, cls_logits.size(2), nullptr, matched_idxs, labels, {}, {}, "fcos_cls_loss");
-  at::cuda::CUDAGuard guard(cls_logits.device());
-  const int B = (int)desc.size();
-  const int64_t A = cls_logits.size(1);
-  at::Tensor loss = at::empty({}, cls_logits.options());
-  at::Tensor count = at::empty({}, cls_logits.options().dtype(at::kLong));
-  const size_t wsb = vb200_fcos_cls_loss_workspace_bytes(B, A);
-  at::Tensor ws = workspace(wsb, cls_logits);
-  check_rc(vb200_fcos_cls_loss(desc.data(), B, A, (int)cls_logits.size(2), loss.data_ptr<float>(), count.data_ptr<int64_t>(), ws.data_ptr(),
-                               wsb, cur_stream()),
-           "fcos_cls_loss");
-  return std::make_tuple(loss, count);
+  const auto r = head_loss(VB200_LOSS_FCOS_CLS, cls_logits, nullptr, matched_idxs, labels, {}, {}, {}, false, "fcos_cls_loss");
+  return std::make_tuple(std::get<0>(r), std::get<2>(r));
 }
 
 at::Tensor fcos_cls_loss_backward(const at::Tensor& grad, const at::Tensor& cls_logits, at::TensorList matched_idxs, at::TensorList labels,
                                   const at::Tensor& num_foreground) {
-  TORCH_CHECK(cls_logits.dim() == 3, "fcos_cls_loss_backward: cls_logits must be [B, A, C]");
-  auto desc = fcos_loss_images(cls_logits, cls_logits.size(2), nullptr, matched_idxs, labels, {}, {}, "fcos_cls_loss_backward");
-  check_fcos_backward(grad, cls_logits, num_foreground, "fcos_cls_loss_backward");
-  at::cuda::CUDAGuard guard(cls_logits.device());
-  const int B = (int)desc.size();
-  at::Tensor g = grad.contiguous(), n = num_foreground.contiguous();
-  at::Tensor out = at::empty(cls_logits.sizes(), cls_logits.options());
-  for (int i = 0; i < B; ++i) desc[(size_t)i].grad = out.data_ptr<float>() + (int64_t)i * out.stride(0);
-  check_rc(vb200_fcos_cls_loss_backward(desc.data(), B, cls_logits.size(1), (int)cls_logits.size(2), g.data_ptr<float>(), n.data_ptr<int64_t>(),
-                                        cur_stream()),
-           "fcos_cls_loss_backward");
-  return out;
+  return std::get<0>(head_loss_backward(VB200_LOSS_FCOS_CLS, grad, std::nullopt, cls_logits, nullptr, matched_idxs, labels, {}, {}, {}, false,
+                                        num_foreground, "fcos_cls_loss_backward"));
 }
 
 std::tuple<at::Tensor, at::Tensor, at::Tensor> fcos_box_loss(const at::Tensor& bbox_regression, const at::Tensor& bbox_ctrness, at::TensorList anchors,
                                                              at::TensorList gt_boxes, at::TensorList labels, at::TensorList matched_idxs,
                                                              bool normalize_by_size) {
-  auto desc = fcos_loss_images(bbox_regression, 4, &bbox_ctrness, matched_idxs, labels, anchors, gt_boxes, "fcos_box_loss");
-  at::cuda::CUDAGuard guard(bbox_regression.device());
-  const int B = (int)desc.size();
-  const int64_t A = bbox_regression.size(1);
-  at::Tensor loss_box = at::empty({}, bbox_regression.options()), loss_ctr = at::empty({}, bbox_regression.options());
-  at::Tensor count = at::empty({}, bbox_regression.options().dtype(at::kLong));
-  const size_t wsb = vb200_fcos_box_loss_workspace_bytes(B, A);
-  at::Tensor ws = workspace(wsb, bbox_regression);
-  check_rc(vb200_fcos_box_loss(desc.data(), B, A, normalize_by_size ? 1 : 0, loss_box.data_ptr<float>(), loss_ctr.data_ptr<float>(),
-                               count.data_ptr<int64_t>(), ws.data_ptr(), wsb, cur_stream()),
-           "fcos_box_loss");
-  return std::make_tuple(loss_box, loss_ctr, count);
+  return head_loss(VB200_LOSS_FCOS_BOX, bbox_regression, &bbox_ctrness, matched_idxs, labels, anchors, gt_boxes, {}, normalize_by_size,
+                   "fcos_box_loss");
 }
 
-// An undefined incoming gradient counts as zero: its rows are 0 (both undefined: no launch).
 std::tuple<at::Tensor, at::Tensor> fcos_box_loss_backward(const std::optional<at::Tensor>& grad_box, const std::optional<at::Tensor>& grad_ctrness,
                                                           const at::Tensor& bbox_regression, const at::Tensor& bbox_ctrness, at::TensorList anchors,
                                                           at::TensorList gt_boxes, at::TensorList labels, at::TensorList matched_idxs,
                                                           bool normalize_by_size, const at::Tensor& num_foreground) {
-  auto desc = fcos_loss_images(bbox_regression, 4, &bbox_ctrness, matched_idxs, labels, anchors, gt_boxes, "fcos_box_loss_backward");
-  const bool has_box = grad_box.has_value() && grad_box->defined(), has_ctr = grad_ctrness.has_value() && grad_ctrness->defined();
-  at::cuda::CUDAGuard guard(bbox_regression.device());
-  if (!has_box && !has_ctr)
-    return std::make_tuple(at::zeros(bbox_regression.sizes(), bbox_regression.options()), at::zeros(bbox_ctrness.sizes(), bbox_ctrness.options()));
-  at::Tensor gb, gc;
-  if (has_box) {
-    check_fcos_backward(*grad_box, bbox_regression, num_foreground, "fcos_box_loss_backward");
-    gb = grad_box->contiguous();
-  }
-  if (has_ctr) {
-    check_fcos_backward(*grad_ctrness, bbox_regression, num_foreground, "fcos_box_loss_backward");
-    gc = grad_ctrness->contiguous();
-  }
-  const int B = (int)desc.size();
-  at::Tensor n = num_foreground.contiguous();
-  at::Tensor out = at::empty(bbox_regression.sizes(), bbox_regression.options());
-  at::Tensor out_ctr = at::empty(bbox_ctrness.sizes(), bbox_ctrness.options());
-  for (int i = 0; i < B; ++i) {
-    desc[(size_t)i].grad = out.data_ptr<float>() + (int64_t)i * out.stride(0);
-    desc[(size_t)i].grad_ctrness = out_ctr.data_ptr<float>() + (int64_t)i * out_ctr.stride(0);
-  }
-  check_rc(vb200_fcos_box_loss_backward(desc.data(), B, bbox_regression.size(1), normalize_by_size ? 1 : 0, has_box ? gb.data_ptr<float>() : nullptr,
-                                        has_ctr ? gc.data_ptr<float>() : nullptr, n.data_ptr<int64_t>(), cur_stream()),
-           "fcos_box_loss_backward");
-  return std::make_tuple(out, out_ctr);
+  return head_loss_backward(VB200_LOSS_FCOS_BOX, grad_box, grad_ctrness, bbox_regression, &bbox_ctrness, matched_idxs, labels, anchors,
+                            gt_boxes, {}, normalize_by_size, num_foreground, "fcos_box_loss_backward");
 }
 
 // ---- box_iou_rotated (csrc/ops/box_iou_rotated.cpp; checks as cuda/box_iou_rotated_kernel.cu:92-118) ----------------
