@@ -460,6 +460,46 @@ VB200_API int vb200_head_loss_backward(int kind, const vb200_loss_image* images,
                                        const float* weights_host, int normalize_by_size, const float* grad_loss,
                                        const float* grad_loss2, const int64_t* num_foreground, vb200_stream stream);
 
+/* ---- Mask R-CNN mask loss ------------------------------------------------------------------------------------------------
+ * Replaces, forward and backward, for all images of a call, maskrcnn_loss (torchvision/models/detection/roi_heads.py:100-129)
+ * with project_masks_on_boxes (:85-97): the fp32 copy of every image's whole gt-mask stack, roi_align over it, the label
+ * gather, the two torch.cat, the [P, C, M, M] advanced-index gather, binary_cross_entropy_with_logits as a chain of
+ * elementwise kernels and a mean, and in the backward the zeros_like + index_put of the dense gradient.
+ * Image i: masks its gt masks [num_gt, height, width] (element strides mask_stride; mask_dtype VB200_U8, bool masks passed
+ * as their 0 / 1 bytes with VB200_U8), read in place, never copied; proposals its positive RoIs fp32 [num_rois, 4] (x1, y1,
+ * x2, y2; element strides (row, column)); matched int64 [num_rois] (stride matched_stride), the gt index of each RoI; labels
+ * int64 [num_gt] (stride label_stride).  The images' RoIs are the rows of mask_logits in order: mask_logits fp32 [P, C, M, M]
+ * dense, P = sum of num_rois, C = num_classes, M = size; targets fp32 [P, M, M] dense; P * C * M * M below 2^31.
+ * Arithmetic: RoI p of image i with m = matched[p] has target t[p, bin] = roi_align(float(masks[m]), proposals[p], (M, M),
+ * spatial_scale 1, sampling_ratio -1, aligned false) -- the reference's RoI geometry, sample order and roundings, bit-exact
+ * with its CPU kernel -- and logit x = mask_logits[p, l, bin] with l = labels[m], a label in [-C, 0) wrapping as indexing
+ * does.  Each element's BCE term (1 - t) x + softplus(-x) is formed in fp64 from fp32 exp / log1p (the stable forms of the
+ * head losses).  Forward: *loss = fl(S) * fl(1 / N), N = P * M * M (ATen's mean: the sum, then the product with the fp32
+ * reciprocal), S the sum of every term: per CTA of 256 (RoI, bin) threads a fixed-order tree, the CTA partials added in
+ * order by one finalize CTA.  targets are written (the backward reads them).  Backward: grad_logits [P, C, M, M] dense,
+ * written exactly once: the label plane of RoI p gets fl(s * (sigmoid(x) - t)) with s = fl(g * fl(1 / N)), g = *grad_loss
+ * read from device memory; every other plane +0; a null grad_loss is a zero gradient (every element +0).
+ * Bad indices, where the reference raises a device-side assert: m < 0, m >= num_gt or a label outside [-C, C) makes the loss
+ * NaN, the RoI's targets NaN and its whole [C, M, M] gradient block NaN; nothing outside masks, labels, proposals, matched
+ * and the RoI's logits is read.  No floating-point atomics and nothing from the SM count: bit-reproducible in every mode.
+ * Launches: per VB200_LOSS_MAX_IMAGES images one forward kernel (none for images without RoIs) plus one finalize per forward;
+ * one backward kernel per VB200_LOSS_MAX_IMAGES images.  workspace: the query's bytes, a function of (num_images, P, M) only.
+ * P = 0 writes NaN (0 / 0) and launches only the finalize.  Asynchronous. */
+typedef struct vb200_mask_image {
+  const void* masks;
+  const float* proposals;
+  const int64_t* matched;
+  const int64_t* labels;
+  int64_t mask_stride[3], proposal_stride[2], matched_stride, label_stride;
+  int64_t num_gt, height, width, num_rois;
+  int mask_dtype;
+} vb200_mask_image;
+VB200_API size_t vb200_mask_loss_workspace_bytes(int num_images, int64_t total_rois, int size);
+VB200_API int vb200_mask_loss(const vb200_mask_image* images, int num_images, const float* mask_logits, int num_classes, int size,
+                              float* loss, float* targets, void* workspace, size_t workspace_bytes, vb200_stream stream);
+VB200_API int vb200_mask_loss_backward(const vb200_mask_image* images, int num_images, const float* mask_logits, const float* targets,
+                                       int num_classes, int size, const float* grad_loss, float* grad_logits, vb200_stream stream);
+
 /* ---- deform_conv2d -----------------------------------------------------
  * Replaces deform_conv2d_forward_kernel, csrc/ops/cuda/deform_conv2d_kernel.cu:1035-1255
  * (schema torchvision::deform_conv2d, csrc/ops/deform_conv2d.cpp:101-102).

@@ -14,7 +14,9 @@
     python tools/prof_ops.py retinanet_loss [iters]     fused vs. reference RetinaNet head losses, forward + backward,
                              batch 2 and 8, 7 and 50 gt boxes per image
     python tools/prof_ops.py fcos_loss [iters]     fused vs. reference FCOSHead.compute_loss, forward + backward, batch 2,
-                             8 and 16, 7 and 50 gt boxes per image"""
+                             8 and 16, 7 and 50 gt boxes per image
+    python tools/prof_ops.py mask_loss [iters]     fused vs. reference Mask R-CNN maskrcnn_loss, forward + backward,
+                             batch 2 and 8, 128 positives per image, 7 and 50 uint8 gt masks of 800 x 1088 per image"""
 import os
 import sys
 
@@ -613,6 +615,106 @@ def fcos_loss(iters: int) -> None:
                 print(f"    {name:9s} wall {wall:.3f} ms per step, kernels {kern:.3f} ms ({top}), peak +{peak:.0f} MiB")
 
 
+def mask_loss(iters: int) -> None:
+    """roi_heads.maskrcnn_loss, forward + backward, with C = 91, M = 28, batch 2 and 8, 128 positive RoIs per image jittered
+    around their gt boxes, M_gt in {7, 50} uint8 gt masks of 800 x 1088 per image: the fused op against the reference body on
+    the same inputs.  Wall time per step ending in a synchronize (median), GPU kernel time per step from torch.profiler (a
+    separate run), the peak-memory delta over the step and the HBM bound of the fused step computed from the shapes (the
+    label planes of the logits read forward and backward, the targets written and read back, the [P, C, M, M] gradient
+    written once; the mask taps are not counted, so the bound is a lower one; at the data-sheet 3.35 TB/s)."""
+    import re
+    import subprocess
+    import time
+
+    from torch.profiler import ProfilerActivity, profile
+    from torchvision.models.detection import roi_heads
+
+    from vision_b200 import detection as det
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+    print(f"mask_loss: {gpu.strip().splitlines()[0] if gpu.strip() else 'unknown GPU'}")
+    C, M, P, H, W = 91, 28, 128, 800, 1088
+
+    def timed(fn, n):
+        for _ in range(2):
+            fn()
+        torch.cuda.synchronize()
+        wall = []
+        for _ in range(n):
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            wall.append(time.perf_counter() - t0)
+        return sorted(wall)[n // 2] * 1e3
+
+    def kernel_ms(fn, n):
+        fn()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(n):
+                fn()
+            torch.cuda.synchronize()
+        events = [e for e in prof.key_averages() if e.device_type == torch.autograd.DeviceType.CUDA]
+        total = sum(e.self_device_time_total for e in events) / n / 1e3
+        top = sorted(events, key=lambda e: -e.self_device_time_total)[:4]
+        short = lambda k: re.sub(r"^void |vb200::|\(anonymous namespace\)::|at::native::|\(.*$", "", k)[:48]  # noqa: E731
+        return total, ", ".join(f"{short(e.key)} {e.self_device_time_total / n / 1e3:.3f}" for e in top)
+
+    def peak_mb(fn, clear):
+        clear()
+        torch.cuda.synchronize()
+        base = torch.cuda.memory_allocated()
+        torch.cuda.reset_peak_memory_stats()
+        fn()
+        torch.cuda.synchronize()
+        return (torch.cuda.max_memory_allocated() - base) / 2**20
+
+    for batch in (2, 8):
+        for G in (7, 50):
+            g = torch.Generator(device=dev).manual_seed(G)
+            proposals, masks, labels, matched = [], [], [], []
+            for _ in range(batch):
+                xy = torch.rand(G, 2, generator=g, device=dev) * torch.tensor([W * 0.7, H * 0.7], device=dev)
+                gt = torch.cat([xy, xy + 32 + torch.rand(G, 2, generator=g, device=dev) * 300], 1)
+                mk = torch.zeros(G, H, W, dtype=torch.uint8, device=dev)
+                for j, b in enumerate(gt.round().int().tolist()):
+                    mk[j, b[1]:b[3], b[0]:b[2]] = 1
+                m = torch.randint(0, G, (P,), generator=g, device=dev)
+                size = (gt[m, 2:] - gt[m, :2]).repeat(1, 2)
+                proposals.append(gt[m] + (torch.rand(P, 4, generator=g, device=dev) - 0.5) * 0.3 * size)
+                masks.append(mk)
+                labels.append(torch.randint(1, C, (G,), generator=g, device=dev))
+                matched.append(m)
+            logits = (torch.randn(batch * P, C, M, M, generator=g, device=dev)).requires_grad_(True)
+
+            def clear():
+                logits.grad = None
+
+            bodies = {"reference": lambda: roi_heads.maskrcnn_loss(logits, proposals, masks, labels, matched),
+                      "fused": lambda: det.maskrcnn_loss_op(logits, proposals, masks, labels, matched)[0]}
+            rows = {}
+            for name, body in bodies.items():
+                def step(body=body):
+                    clear()
+                    loss = body()
+                    loss.backward()
+                    return loss.detach()
+
+                loss = step()
+                rows[name] = (loss, logits.grad.clone(), timed(step, iters), kernel_ms(step, 5), peak_mb(step, clear))
+            n = batch * P
+            bound_us = (n * M * M * 4 * 4 + n * C * M * M * 4) / 3.35e12 * 1e6
+            (l0, g0, *_), (l1, g1, *_) = rows["reference"], rows["fused"]
+            print(f"  batch {batch}, M_gt {G} ({n} positives): HBM bound of the fused step {bound_us:.0f} us; loss rel. diff "
+                  f"{abs(l1.item() - l0.item()) / abs(l0.item()):.1e}, max |d grad| / max |grad| "
+                  f"{((g1 - g0).abs().max() / g0.abs().max()).item():.1e}")
+            for name, (_, _, wall, (kern, top), peak) in rows.items():
+                print(f"    {name:9s} wall {wall:.3f} ms per step, kernels {kern:.3f} ms ({top}), peak +{peak:.0f} MiB")
+
+
+if op == "mask_loss":
+    mask_loss(iters)
+    raise SystemExit(0)
 if op == "fcos_loss":
     fcos_loss(iters)
     raise SystemExit(0)

@@ -4,6 +4,8 @@
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py fcos         (the FCOS matching kernel: memcheck only)
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py retinanet_loss   (the RetinaNet and FCOS head-loss
                                                                                        kernels: memcheck only)
+    compute-sanitizer --tool memcheck python tools/sanitize_smoke.py mask_loss    (the Mask R-CNN mask-loss kernels: memcheck
+                                                                                   only)
 No numerics are checked here (tests/ does that); the point is out-of-bounds / hazard reports."""
 import os
 import sys
@@ -204,8 +206,38 @@ def retinanet_loss():
             (det.fcos_cls_loss_op(logits, matched, labels) + loss_box + loss_ctr).backward()
 
 
+def mask_loss():
+    """the mask-loss kernels forward and backward, memcheck only: logits not 16-byte aligned, transposed and sliced bool and
+    uint8 masks, RoIs past the image edge, an image without positives, bad match and label indices (which must read nothing
+    outside the masks, labels or logits), and more images than one launch's descriptors"""
+    from vision_b200 import detection as det
+
+    for B, C, M in ((3, 91, 28), (70, 3, 7)):
+        ps = [5 if i % 3 != 1 else 0 for i in range(B)]
+        gs = [4 if i % 5 != 4 else 1 for i in range(B)]
+        hw = [(40 + i % 3, 52 + i % 4) for i in range(B)]
+        masks = []
+        for i, (g, (H, W)) in enumerate(zip(gs, hw)):
+            m = torch.rand(g, W, H, device=dev) > 0.5
+            masks.append(m.transpose(1, 2) if i % 2 else torch.cat([m, m], 1)[:, ::2].transpose(1, 2).to(torch.uint8))
+        proposals = []
+        for p, (H, W) in zip(ps, hw):
+            xy = torch.rand(p, 2, device=dev) * torch.tensor([W, H], device=dev)
+            box = torch.cat([xy, xy + torch.rand(p, 2, device=dev) * 60], 1)
+            if p:
+                box[0] = torch.tensor([W - 3.0, H - 2.0, W + 40.0, H + 30.0])    # past the image edge
+            proposals.append(box)
+        labels = [torch.randint(-C, C, (g,), device=dev) for g in gs]
+        matched = [torch.randint(0, g, (p,), device=dev) for p, g in zip(ps, gs)]
+        matched[0][1], matched[0][2], labels[0][0] = gs[0] + 100, -7, C + 5
+        P = sum(ps)
+        logits = torch.randn(P * C * M * M + 1, device=dev)[1:].view(P, C, M, M).requires_grad_(True)
+        det.maskrcnn_loss_op(logits, proposals, masks, labels, matched)[0].backward()
+
+
 for name, fn in (("roi", roi), ("bwd", bwd), ("nms", nms), ("resize", resize), ("dcn", dcn), ("gather", gather), ("matching", matching),
-                 ("fcos", fcos), ("retinanet_loss", retinanet_loss)):
+                 ("fcos", fcos), ("retinanet_loss", retinanet_loss),
+                 ("mask_loss", mask_loss)):
     if only in ("all", name):
         fn()
         torch.cuda.synchronize()

@@ -274,6 +274,31 @@ def register() -> None:
           num_foreground):
         return bbox_regression.new_empty(bbox_regression.shape), bbox_ctrness.new_empty(bbox_ctrness.shape)
 
+    # ---- Mask R-CNN mask loss: mask_logits is the only differentiable input; the targets are saved for the backward ----
+    def mask_loss_setup(ctx, inputs, output):
+        logits, proposals, gt_masks, gt_labels, matched = inputs
+        ctx.mark_non_differentiable(output[1])
+        ctx.save_for_backward(logits, output[1])
+        ctx.lists = (list(gt_labels), list(matched))
+        ctx.num_images = len(proposals)
+
+    def mask_loss_backward(ctx, grad, _grad_targets):
+        logits, targets = ctx.saved_tensors
+        gt_labels, matched = ctx.lists
+        n = ctx.num_images
+        return ops.maskrcnn_loss_backward(grad, logits, targets, gt_labels, matched), [None] * n, [None] * n, [None] * n, [None] * n
+
+    lib.register_autograd("vision_b200::maskrcnn_loss", mask_loss_backward, setup_context=mask_loss_setup)
+
+    @lib.register_fake("vision_b200::maskrcnn_loss")
+    def _(mask_logits, proposals, gt_masks, gt_labels, matched_idxs):
+        P, _, M, _ = mask_logits.shape
+        return mask_logits.new_empty(()), mask_logits.new_empty((P, M, M))
+
+    @lib.register_fake("vision_b200::maskrcnn_loss_backward")
+    def _(grad, mask_logits, targets, gt_labels, matched_idxs):
+        return mask_logits.new_empty(mask_logits.shape)
+
     # ---- deform_conv2d ----
     def dcn_setup(ctx, inputs, output):
         inp, weight, offset, mask, bias = inputs[:5]

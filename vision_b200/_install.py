@@ -23,7 +23,8 @@
    ``FCOS.compute_loss`` likewise: its per-image centre-sampling loop becomes one call.
    Head losses: ``RetinaNetClassificationHead.compute_loss`` and ``RetinaNetRegressionHead.compute_loss`` are rebound on
    their classes; each per-image loss loop becomes one call with a fused backward.  ``FCOSHead.compute_loss`` likewise:
-   its three losses become two calls, each with a fused backward.
+   its three losses become two calls, each with a fused backward.  The module global ``roi_heads.maskrcnn_loss`` (Mask
+   R-CNN) is rebound to one mask-loss call for all images with a fused backward.
 5. ``resize`` has no torchvision kernel (transforms/v2/functional/_geometry.py:283-362 calls
    F.interpolate): the entries of ``_KERNEL_REGISTRY[resize]`` for Tensor / Image / Video are swapped.
 CPU tensors and unsupported dtypes/modes keep flowing to the reference implementation.
@@ -180,6 +181,15 @@ def install() -> None:
     tv_fcos.FCOSHead.compute_loss = fcos_head_loss
     fcos_losses = {(tv_fcos.FCOSHead, "compute_loss"): orig_fcos_head_loss}
 
+    # ---- Mask R-CNN mask loss (roi_heads.py:100-129): RoIHeads.forward looks up maskrcnn_loss at call time ----
+    orig_mask_loss = tv_roi_heads.maskrcnn_loss
+
+    @functools.wraps(orig_mask_loss)
+    def maskrcnn_loss(mask_logits, proposals, gt_masks, gt_labels, mask_matched_idxs):
+        return _det.maskrcnn_loss(mask_logits, proposals, gt_masks, gt_labels, mask_matched_idxs, _orig=orig_mask_loss)
+
+    tv_roi_heads.maskrcnn_loss = maskrcnn_loss
+
     # ---- detection model inputs and outputs (transform.py:119-158, 257-277): bound on the class, so every model's
     # self.transform (Faster / Mask / Keypoint R-CNN, RetinaNet, FCOS, SSD, SSDLite) picks them up ----
     from torchvision.models.detection import transform as tv_transform
@@ -248,7 +258,7 @@ def install() -> None:
                        tv_roi_align_mod=tv_roi_align_mod, orig_det_roi_align=orig_det_roi_align,
                        tv_roi_heads=tv_roi_heads, tv_rpn=tv_rpn, orig_pp=orig_pp, orig_fp=orig_fp, orig_kri=orig_kri, orig_h2k=orig_h2k,
                        tv_presets=tv_presets, orig_preset_forward=orig_preset_forward, single_stage=single_stage, matching=matching, losses=losses,
-                       fcos_losses=fcos_losses, rcnn_transform=rcnn_transform, orig_tf_forward=orig_tf_forward, orig_tf_post=orig_tf_post))
+                       fcos_losses=fcos_losses, orig_mask_loss=orig_mask_loss, rcnn_transform=rcnn_transform, orig_tf_forward=orig_tf_forward, orig_tf_post=orig_tf_post))
 
 
 def uninstall() -> None:
@@ -264,6 +274,7 @@ def uninstall() -> None:
     _state["tv_rpn"].RegionProposalNetwork.filter_proposals = _state["orig_fp"]
     _state["tv_roi_heads"].keypointrcnn_inference = _state["orig_kri"]
     _state["tv_roi_heads"].heatmaps_to_keypoints = _state["orig_h2k"]
+    _state["tv_roi_heads"].maskrcnn_loss = _state["orig_mask_loss"]
     _state["rcnn_transform"].forward = _state["orig_tf_forward"]
     _state["rcnn_transform"].postprocess = _state["orig_tf_post"]
     for cls, orig in _state["single_stage"].items():

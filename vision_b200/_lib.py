@@ -85,4 +85,5 @@ ABI_SYMBOLS = (
     "vb200_heatmaps_to_keypoints_workspace_bytes", "vb200_heatmaps_to_keypoints",
     "vb200_rcnn_batch_images", "vb200_rcnn_rescale", "vb200_match_boxes_workspace_bytes", "vb200_match_boxes",
     "vb200_fcos_level_bounds", "vb200_fcos_match", "vb200_head_loss_workspace_bytes", "vb200_head_loss", "vb200_head_loss_backward",
+    "vb200_mask_loss_workspace_bytes", "vb200_mask_loss", "vb200_mask_loss_backward",
 )

@@ -14,7 +14,13 @@
 //   backward  the dense gradient written exactly once: the analytic derivative times the head's scale, 0 where the
 //             reference's indexing leaves it 0.
 // No floating-point atomics and no launch parameter depends on the SM count, so every result is bit-reproducible run to run.
+//
+// Mask R-CNN's mask loss (roi_heads.py:85-129) follows the same plan over (RoI, bin) instead of (anchor, class): the
+// forward projects each positive RoI's gt mask on its box with the generic roi_align kernel's own per-bin routine
+// (roi_geometry.cuh), reading the uint8 / bool masks in place, and adds the BCE term of the RoI's label plane; the backward
+// writes the dense [P, C, M, M] gradient once from the saved targets.
 #include "common.cuh"
+#include "roi_geometry.cuh"
 
 namespace vb200 {
 namespace {
@@ -578,6 +584,211 @@ LossPlan make_plan(int kind, int num_images, int64_t num_anchors, int width, con
   return plan;
 }
 
+// ---- Mask R-CNN mask loss ------------------------------------------------------------------------------------------------
+constexpr int kMaskThreads = 256;
+
+struct MaskPlan {
+  vb200_mask_image img[VB200_LOSS_MAX_IMAGES];
+  int64_t roi_begin[VB200_LOSS_MAX_IMAGES];             // img[i]'s first RoI, counted from the chunk's first
+  int images;                                           // in this chunk
+  int num_classes, size;
+  int64_t first_roi, num_rois;                          // the chunk's RoIs, counted in the call
+  int64_t total_rois;                                   // the call's P
+  int64_t first_partial;                                // forward: the chunk's first CTA slot
+  const float* logits;
+  float* targets;                                       // forward: written; backward: read
+  double* partial;                                      // forward
+  const float* grad_loss;                               // backward (null: a zero gradient)
+  float* grad;                                          // backward
+};
+
+// A chunk RoI's gt index and class plane; bad as the loss's bad-index rule says.
+struct MaskRoi {
+  int image;
+  int64_t row, m;
+  int label;
+  bool bad;
+};
+
+__device__ __forceinline__ MaskRoi mask_roi(const MaskPlan& plan, int64_t p) {
+  int lo = 0, hi = plan.images - 1;                     // the last image starting at or before p holds it
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (plan.roi_begin[mid] <= p) lo = mid;
+    else hi = mid - 1;
+  }
+  const vb200_mask_image& d = plan.img[lo];
+  MaskRoi q;
+  q.image = lo;
+  q.row = p - plan.roi_begin[lo];
+  q.m = d.matched[q.row * d.matched_stride];
+  q.label = 0;
+  q.bad = q.m < 0 || q.m >= d.num_gt;
+  if (!q.bad) {
+    const int64_t l = d.labels[q.m * d.label_stride];
+    q.bad = l < -plan.num_classes || l >= plan.num_classes;
+    q.label = (int)(l < 0 ? l + plan.num_classes : l);
+  }
+  return q;
+}
+
+// One thread per (RoI, bin) of the chunk: the bin's target, written, and its BCE term; one partial sum per CTA.
+__global__ void __launch_bounds__(kMaskThreads)
+mask_loss_kernel(const __grid_constant__ MaskPlan plan) {
+  __shared__ double scratch[kMaskThreads / 32];
+  const int M = plan.size, MM = M * M;
+  const int64_t e = (int64_t)blockIdx.x * kMaskThreads + threadIdx.x;
+  double term = 0.0;
+  if (e < plan.num_rois * MM) {
+    const int64_t pl = e / MM;
+    const int bin = (int)(e - pl * MM);
+    const MaskRoi q = mask_roi(plan, pl);
+    const int64_t p = plan.first_roi + pl;
+    float t = NAN;
+    if (q.bad) {
+      term = (double)NAN;
+    } else {
+      const vb200_mask_image& d = plan.img[q.image];
+      float r[5];
+      r[0] = 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) r[1 + j] = d.proposals[q.row * d.proposal_stride[0] + j * d.proposal_stride[1]];
+      const RoiGeom<float> g = roi_geometry<float, float>(r, 1.f, M, M, -1, false, false);
+      const StridedPlane<uint8_t> mask{static_cast<const uint8_t*>(d.masks) + q.m * d.mask_stride[0], d.mask_stride[1], d.mask_stride[2]};
+      t = roi_align_bin<float>(mask, (int)d.height, (int)d.width, g, bin / M, bin % M, false, nullptr, nullptr);
+      const float x = __ldg(plan.logits + ((p * plan.num_classes + q.label) * MM + bin));
+      term = (1.0 - (double)t) * (double)x + sig(x).sp_neg;
+    }
+    plan.targets[p * MM + bin] = t;
+  }
+  const double sum = block_sum(term, scratch);
+  if (threadIdx.x == 0) plan.partial[plan.first_partial + blockIdx.x] = sum;
+}
+
+// The CTA partials in order; *loss = fl(S) * fl(1 / N).
+__global__ void __launch_bounds__(kFinalizeThreads)
+mask_loss_finalize_kernel(const double* __restrict__ partial, int64_t count, int64_t n, float* loss) {
+  __shared__ double scratch[kFinalizeThreads / 32];
+  double s = 0.0;
+  for (int64_t j = threadIdx.x; j < count; j += kFinalizeThreads) s += partial[j];
+  s = block_sum(s, scratch);
+  if (threadIdx.x == 0) *loss = __fmul_rn((float)s, reciprocal((float)n));
+}
+
+// One thread per 16-byte group of the chunk's [P_chunk, C, M, M] gradient, groups aligned on the gradient's address (the
+// first and last may be partial).  Flat element offsets are below 2^31, so the index arithmetic is 32-bit.
+__global__ void __launch_bounds__(kMaskThreads)
+mask_loss_backward_kernel(const __grid_constant__ MaskPlan plan) {
+  const uint32_t MM = (uint32_t)(plan.size * plan.size), block = (uint32_t)plan.num_classes * MM;
+  const int64_t e0 = plan.first_roi * block, e1 = (plan.first_roi + plan.num_rois) * block;
+  float* __restrict__ out = plan.grad;
+  const int pad = (int)((reinterpret_cast<uintptr_t>(out + e0) >> 2) & 3);
+  const int64_t eb = e0 - pad + 4 * ((int64_t)blockIdx.x * kMaskThreads + threadIdx.x);
+  if (eb >= e1) return;
+  const float s = plan.grad_loss ? __fmul_rn(*plan.grad_loss, reciprocal((float)(plan.total_rois * MM))) : 0.f;
+  // (RoI, class, bin) of the group's first element inside the chunk, then stepped element by element
+  const uint32_t u = (uint32_t)(eb < e0 ? e0 : eb);
+  uint32_t p = u / block, c = (u - p * block) / MM, bin = u - p * block - c * MM;
+  MaskRoi q = mask_roi(plan, (int64_t)p - plan.first_roi);
+  float gout[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    gout[k] = 0.f;
+    const int64_t e = eb + k;
+    if (e < e0 || e >= e1 || !plan.grad_loss) continue;
+    if (q.bad) {
+      gout[k] = NAN;
+    } else if ((int)c == q.label) {
+      const float x = __ldg(plan.logits + e), t = __ldg(plan.targets + (int64_t)p * MM + bin);
+      gout[k] = (float)((double)s * (sig(x).p - (double)t));
+    }
+    if (++bin == MM) {
+      bin = 0;
+      if (++c == (uint32_t)plan.num_classes && k < 3 && e + 1 < e1) {
+        c = 0;
+        q = mask_roi(plan, (int64_t)++p - plan.first_roi);
+      }
+    }
+  }
+  if (eb >= e0 && eb + 4 <= e1) {
+    __stcs(reinterpret_cast<float4*>(out + eb), make_float4(gout[0], gout[1], gout[2], gout[3]));
+  } else {
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (eb + k >= e0 && eb + k < e1) out[eb + k] = gout[k];
+  }
+}
+
+// The sizes, and every pointer an image with RoIs reads (the backward reads neither masks nor proposals).
+int check_mask_call(const vb200_mask_image* images, int num_images, int num_classes, int size, bool backward, int64_t& total_rois,
+                    const char* op) {
+  VB200_REQUIRE(num_images >= 1 && images, "%s: at least one image", op);
+  VB200_REQUIRE(num_classes >= 1 && size >= 1 && size <= 4096, "%s: bad sizes (%d classes, size %d)", op, num_classes, size);
+  total_rois = 0;
+  for (int i = 0; i < num_images; ++i) {
+    const vb200_mask_image& d = images[i];
+    VB200_REQUIRE(d.num_rois >= 0 && d.num_gt >= 0 && d.height >= 0 && d.width >= 0 && d.height < ((int64_t)1 << 31) &&
+                      d.width < ((int64_t)1 << 31),
+                  "%s: image %d: bad sizes", op, i);
+    VB200_REQUIRE(backward || d.mask_dtype == VB200_U8, "%s: image %d: masks must be uint8 (or bool as uint8), dtype %d given", op, i,
+                  d.mask_dtype);
+    total_rois += d.num_rois;
+    VB200_REQUIRE(total_rois * num_classes * size * size < ((int64_t)1 << 31), "%s: 2^31 or more logits", op);
+    if (d.num_rois == 0) continue;
+    VB200_REQUIRE(d.matched && (backward || d.proposals), "%s: image %d: null pointer", op, i);
+    VB200_REQUIRE(d.num_gt == 0 || (d.labels && (backward || (d.masks && d.height >= 1 && d.width >= 1))), "%s: image %d: null or empty gt",
+                  op, i);
+  }
+  return 0;
+}
+
+// One launch of `kernel` per VB200_LOSS_MAX_IMAGES images holding RoIs; `grid(rois)` its CTA count for a chunk's RoIs, the
+// CTA slots of the forward's partials handed out in order.
+template <class Grid>
+int launch_mask(void (*kernel)(const MaskPlan), const char* name, MaskPlan& plan, const vb200_mask_image* images, int num_images,
+                Grid&& grid, cudaStream_t st) {
+  int64_t roi = 0, slot = 0;
+  for (int done = 0; done < num_images; done += VB200_LOSS_MAX_IMAGES) {
+    const int chunk = num_images - done < VB200_LOSS_MAX_IMAGES ? num_images - done : VB200_LOSS_MAX_IMAGES;
+    plan.images = chunk;
+    plan.first_roi = roi;
+    int64_t n = 0;
+    for (int i = 0; i < chunk; ++i) {
+      plan.img[i] = images[done + i];
+      plan.roi_begin[i] = n;
+      n += images[done + i].num_rois;
+    }
+    plan.num_rois = n;
+    plan.first_partial = slot;
+    roi += n;
+    if (n == 0) continue;
+    const int64_t ctas = grid(n);
+    slot += ctas;
+    kernel<<<(unsigned)ctas, kMaskThreads, 0, st>>>(plan);
+    const int rc = check_launch(name);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+// The forward's CTA slots: at most one partial CTA per chunk beyond the call's full ones.
+int64_t mask_partials(int num_images, int64_t total_rois, int size) {
+  return ceil_div64(total_rois * size * size, kMaskThreads) + ceil_div64(num_images, VB200_LOSS_MAX_IMAGES);
+}
+
+MaskPlan make_mask_plan(const float* logits, int num_classes, int size, int64_t total_rois) {
+  MaskPlan plan;
+  plan.num_classes = num_classes;
+  plan.size = size;
+  plan.total_rois = total_rois;
+  plan.logits = logits;
+  plan.targets = nullptr;
+  plan.partial = nullptr;
+  plan.grad_loss = nullptr;
+  plan.grad = nullptr;
+  return plan;
+}
+
 }  // namespace
 }  // namespace vb200
 
@@ -638,4 +849,60 @@ extern "C" int vb200_head_loss_backward(int kind, const vb200_loss_image* images
   plan.grad_loss2 = grad_loss2;
   plan.num_fg = num_foreground;
   return launch_loss(h.backward, h.kernel, plan, images, num_images, (cudaStream_t)stream);
+}
+
+extern "C" size_t vb200_mask_loss_workspace_bytes(int num_images, int64_t total_rois, int size) {
+  if (num_images < 1 || total_rois < 0 || size < 1) return 0;
+  return align256((size_t)mask_partials(num_images, total_rois, size) * sizeof(double));
+}
+
+extern "C" int vb200_mask_loss(const vb200_mask_image* images, int num_images, const float* mask_logits, int num_classes, int size,
+                               float* loss, float* targets, void* workspace, size_t workspace_bytes, vb200_stream stream) {
+  const char* op = "maskrcnn_loss";
+  int64_t total_rois = 0;
+  int rc = check_mask_call(images, num_images, num_classes, size, false, total_rois, op);
+  if (rc) return rc;
+  VB200_REQUIRE(loss && (total_rois == 0 || (mask_logits && targets)), "%s: null logits or outputs", op);
+  const size_t need = vb200_mask_loss_workspace_bytes(num_images, total_rois, size);
+  if (!workspace || workspace_bytes < need) {
+    set_error("%s: workspace of %zu bytes, %zu needed", op, workspace_bytes, need);
+    return VB200_EWORKSPACE;
+  }
+  MaskPlan plan = make_mask_plan(mask_logits, num_classes, size, total_rois);
+  plan.targets = targets;
+  plan.partial = static_cast<double*>(workspace);
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int64_t bins = (int64_t)size * size;
+  int64_t slots = 0;
+  rc = launch_mask(mask_loss_kernel, "mask_loss_kernel", plan, images, num_images,
+                   [&](int64_t rois) {
+                     const int64_t ctas = ceil_div64(rois * bins, kMaskThreads);
+                     slots += ctas;
+                     return ctas;
+                   },
+                   st);
+  if (rc) return rc;
+  mask_loss_finalize_kernel<<<1, kFinalizeThreads, 0, st>>>(plan.partial, slots, total_rois * bins, loss);
+  return check_launch("mask_loss_finalize_kernel");
+}
+
+extern "C" int vb200_mask_loss_backward(const vb200_mask_image* images, int num_images, const float* mask_logits, const float* targets,
+                                        int num_classes, int size, const float* grad_loss, float* grad_logits, vb200_stream stream) {
+  const char* op = "maskrcnn_loss_backward";
+  int64_t total_rois = 0;
+  const int rc = check_mask_call(images, num_images, num_classes, size, true, total_rois, op);
+  if (rc) return rc;
+  VB200_REQUIRE(total_rois == 0 || (mask_logits && targets && grad_logits), "%s: null logits, targets or gradient", op);
+  MaskPlan plan = make_mask_plan(mask_logits, num_classes, size, total_rois);
+  plan.targets = const_cast<float*>(targets);
+  plan.grad_loss = grad_loss;
+  plan.grad = grad_logits;
+  const int64_t block = (int64_t)num_classes * size * size;
+  return launch_mask(mask_loss_backward_kernel, "mask_loss_backward_kernel", plan, images, num_images,
+                     [&](int64_t rois) {
+                       const int64_t e0 = plan.first_roi * block;
+                       const int pad = (int)((reinterpret_cast<uintptr_t>(grad_logits + e0) >> 2) & 3);
+                       return ceil_div64(ceil_div64(rois * block + pad, 4), kMaskThreads);
+                     },
+                     (cudaStream_t)stream);
 }

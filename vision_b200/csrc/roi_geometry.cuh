@@ -1,7 +1,9 @@
 // roi_geometry.cuh — the reference's RoI arithmetic, shared by the RoI forward (roi_ops.cu) and backward
-// (roi_backward.cu) kernels.  Bit-exact parity with the reference rests on these few rules, so they live here only:
+// (roi_backward.cu) kernels and the Mask R-CNN mask-loss kernel (losses.cu).  Bit-exact parity with the reference rests on
+// these few rules, so they live here only:
 //   * RoI box -> sampling start / bin size / grid (roi_align_kernel.cu:86-121) and the sample coordinate;
 //   * the bilinear axis rule and four-tap blend of bilinear_interpolate (roi_align_kernel.cu:21-56);
+//   * one roi_align output bin, its samples in the reference's order (roi_align_generic_kernel and the mask loss);
 //   * the packed (offset, weight) axis encoding of the plane-resident roi_align kernels;
 //   * the integer box and bin windows of roi_pool / ps_roi_pool (roi_pool_kernel.cu:31-58, ps_roi_pool_kernel.cu:30-58).
 #pragma once
@@ -85,15 +87,61 @@ __device__ __forceinline__ A sample_coord(A start, A bin, int p, int i, int grid
   return add_rn(a, b);
 }
 
-// bilinear_interpolate's value at (ey, ex) of an H x W plane with row length W: w1 v1 + w2 v2 + w3 v3 + w4 v4 in the
-// reference's order, one rounding per operation; 0 outside.
+// bilinear_interpolate's blend of the four taps v1..v4 at (ey, ex): w1 v1 + w2 v2 + w3 v3 + w4 v4 in the reference's
+// order, one rounding per operation.
+template <typename A>
+__device__ __forceinline__ A blend_taps(A v1, A v2, A v3, A v4, const AxisEnt<A>& ey, const AxisEnt<A>& ex) {
+  const A w1 = mul_rn(ey.h, ex.h), w2 = mul_rn(ey.h, ex.l), w3 = mul_rn(ey.l, ex.h), w4 = mul_rn(ey.l, ex.l);
+  return add_rn(add_rn(add_rn(mul_rn(w1, v1), mul_rn(w2, v2)), mul_rn(w3, v3)), mul_rn(w4, v4));
+}
+
+// bilinear_interpolate's value at (ey, ex) of an H x W plane with row length W; 0 outside.
 template <typename T, typename A>
 __device__ __forceinline__ A bilinear_blend(const T* __restrict__ plane, int W, const AxisEnt<A>& ey, const AxisEnt<A>& ex) {
   if (ey.lo < 0 || ex.lo < 0) return 0;
   const A v1 = to_acc(plane[ey.lo * W + ex.lo]), v2 = to_acc(plane[ey.lo * W + ex.hi]);
   const A v3 = to_acc(plane[ey.hi * W + ex.lo]), v4 = to_acc(plane[ey.hi * W + ex.hi]);
-  const A w1 = mul_rn(ey.h, ex.h), w2 = mul_rn(ey.h, ex.l), w3 = mul_rn(ey.l, ex.h), w4 = mul_rn(ey.l, ex.l);
-  return add_rn(add_rn(add_rn(mul_rn(w1, v1), mul_rn(w2, v2)), mul_rn(w3, v3)), mul_rn(w4, v4));
+  return blend_taps<A>(v1, v2, v3, v4, ey, ex);
+}
+
+// The planes roi_align_bin reads: a dense H x W plane with row length W, or one with any element strides (Mask R-CNN's
+// gt masks, read in place as uint8 / bool bytes).  blend() is bilinear_blend's value at (ey, ex).
+template <typename T>
+struct DensePlane {
+  const T* __restrict__ p;
+  int W;
+  template <typename A>
+  __device__ __forceinline__ A blend(const AxisEnt<A>& ey, const AxisEnt<A>& ex) const { return bilinear_blend<T, A>(p, W, ey, ex); }
+};
+
+template <typename T>
+struct StridedPlane {
+  const T* __restrict__ p;
+  int64_t sy, sx;
+  template <typename A>
+  __device__ __forceinline__ A blend(const AxisEnt<A>& ey, const AxisEnt<A>& ex) const {
+    if (ey.lo < 0 || ex.lo < 0) return 0;
+    const A v1 = to_acc(p[ey.lo * sy + ex.lo * sx]), v2 = to_acc(p[ey.lo * sy + ex.hi * sx]);
+    const A v3 = to_acc(p[ey.hi * sy + ex.lo * sx]), v4 = to_acc(p[ey.hi * sy + ex.hi * sx]);
+    return blend_taps<A>(v1, v2, v3, v4, ey, ex);
+  }
+};
+
+// One roi_align output bin (ph, pw) of an H x W plane: the gh x gw samples in the reference's order (roi_align_kernel.cu:
+// 124-140), added one rounding at a time, over max(gh * gw, 1).  With `tab` the axis entries come from rowtab / coltab
+// (PH * gh row and PW * gw column entries, as the generic kernel stages them), else they are derived per sample.
+template <typename A, typename Plane>
+__device__ __forceinline__ A roi_align_bin(const Plane& plane, int H, int W, const RoiGeom<A>& g, int ph, int pw, bool tab,
+                                           const AxisEnt<A>* rowtab, const AxisEnt<A>* coltab) {
+  A sum = 0;
+  for (int iy = 0; iy < g.gh; ++iy) {
+    const AxisEnt<A> ey = tab ? rowtab[ph * g.gh + iy] : axis_entry<A>(sample_coord<A>(g.start_h, g.bin_h, ph, iy, g.gh), H);
+    for (int ix = 0; ix < g.gw; ++ix) {
+      const AxisEnt<A> ex = tab ? coltab[pw * g.gw + ix] : axis_entry<A>(sample_coord<A>(g.start_w, g.bin_w, pw, ix, g.gw), W);
+      sum = add_rn(sum, plane.template blend<A>(ey, ex));
+    }
+  }
+  return div_rn(sum, (A)max(g.gh * g.gw, 1));
 }
 
 // Packed (lo, l) of one axis sample for the plane-resident kernels, whose planes carry zero pad columns and rows:

@@ -58,18 +58,8 @@ roi_align_generic_kernel(const T* __restrict__ input, const T* __restrict__ rois
   for (int i = threadIdx.x; i < nch * nbins; i += blockDim.x) {
     const int cl = i / nbins, bin = i - cl * nbins;
     const int ph = bin / PW, pw = bin - ph * PW;
-    const T* __restrict__ in = input + ((int64_t)g.batch * C + (c0 + cl)) * plane;
-    A sum = 0;
-    for (int iy = 0; iy < g.gh; ++iy) {
-      const AxisEnt<A> ey = tab ? rowtab[ph * g.gh + iy]
-                                : axis_entry<A>(sample_coord<A>(g.start_h, g.bin_h, ph, iy, g.gh), H);
-      for (int ix = 0; ix < g.gw; ++ix) {
-        const AxisEnt<A> ex = tab ? coltab[pw * g.gw + ix]
-                                  : axis_entry<A>(sample_coord<A>(g.start_w, g.bin_w, pw, ix, g.gw), W);
-        sum = add_rn(sum, bilinear_blend<T, A>(in, W, ey, ex));
-      }
-    }
-    sum = div_rn(sum, (A)max(g.gh * g.gw, 1));
+    const DensePlane<T> in{input + ((int64_t)g.batch * C + (c0 + cl)) * plane, W};
+    const A sum = roi_align_bin<A>(in, H, W, g, ph, pw, tab, rowtab, coltab);
     output[((int64_t)n * C + (c0 + cl)) * nbins + bin] = from_acc<T, A>(sum);
   }
 }

@@ -1192,6 +1192,96 @@ std::tuple<at::Tensor, at::Tensor> fcos_box_loss_backward(const std::optional<at
                             gt_boxes, {}, normalize_by_size, num_foreground, "fcos_box_loss_backward");
 }
 
+// ---- Mask R-CNN mask loss (roi_heads.py:85-129) ---------------------------------------------------------------------------
+// mask_logits: fp32 [P, C, M, M] dense on one GPU; per image: gt_masks uint8 / bool [M_i, H_i, W_i] (any strides), proposals
+// fp32 [P_i, 4], matched_idxs int64 [P_i], gt_labels int64 [M_i], all on that GPU, sum P_i = P.  proposals and gt_masks are
+// null in the backward, which reads neither.
+std::vector<vb200_mask_image> mask_images(const at::Tensor& mask_logits, at::TensorList proposals, at::TensorList gt_masks,
+                                          at::TensorList gt_labels, at::TensorList matched_idxs, bool backward, const char* op) {
+  TORCH_CHECK(mask_logits.is_cuda() && mask_logits.scalar_type() == at::kFloat && mask_logits.dim() == 4 &&
+                  mask_logits.size(2) == mask_logits.size(3) && mask_logits.size(1) >= 1 && mask_logits.size(2) >= 1 &&
+                  mask_logits.is_contiguous(),
+              op, ": mask_logits must be a dense CUDA float32 [P, C, M, M] tensor");
+  TORCH_CHECK(mask_logits.numel() < ((int64_t)1 << 31), op, ": 2^31 or more mask logits");
+  const size_t B = matched_idxs.size();
+  TORCH_CHECK(B >= 1 && gt_labels.size() == B && (backward || (proposals.size() == B && gt_masks.size() == B)), op,
+              ": one proposals, gt_masks, gt_labels and matched_idxs tensor per image");
+  const auto same_gpu = [&](const at::Tensor& t) { return t.is_cuda() && t.get_device() == mask_logits.get_device(); };
+  std::vector<vb200_mask_image> desc(B);
+  int64_t total = 0;
+  for (size_t i = 0; i < B; ++i) {
+    vb200_mask_image& d = desc[i];
+    d = {};
+    d.mask_dtype = VB200_U8;
+    const at::Tensor &m = matched_idxs[i], &l = gt_labels[i];
+    TORCH_CHECK(same_gpu(m) && m.scalar_type() == at::kLong && m.dim() == 1, op,
+                ": matched_idxs must be int64 [P_i] tensors on the logits' GPU");
+    TORCH_CHECK(same_gpu(l) && l.scalar_type() == at::kLong && l.dim() == 1, op, ": gt_labels must be int64 [M_i] tensors on the logits' GPU");
+    d.matched = m.data_ptr<int64_t>();
+    d.matched_stride = m.stride(0);
+    d.labels = l.data_ptr<int64_t>();
+    d.label_stride = l.stride(0);
+    d.num_rois = m.size(0);
+    d.num_gt = l.size(0);
+    total += d.num_rois;
+    if (backward) continue;
+    const at::Tensor &p = proposals[i], &g = gt_masks[i];
+    TORCH_CHECK(same_gpu(p) && p.scalar_type() == at::kFloat && p.dim() == 2 && p.size(0) == d.num_rois && p.size(1) == 4, op,
+                ": proposals must be float32 [P_i, 4] tensors on the logits' GPU, one row per matched index");
+    TORCH_CHECK(same_gpu(g) && (g.scalar_type() == at::kByte || g.scalar_type() == at::kBool) && g.dim() == 3 && g.size(0) == d.num_gt, op,
+                ": gt_masks must be uint8 or bool [M_i, H, W] tensors on the logits' GPU, one mask per label");
+    d.masks = g.data_ptr();
+    for (int k = 0; k < 3; ++k) d.mask_stride[k] = g.stride(k);
+    d.height = g.size(1);
+    d.width = g.size(2);
+    d.proposals = p.data_ptr<float>();
+    d.proposal_stride[0] = p.stride(0);
+    d.proposal_stride[1] = p.stride(1);
+  }
+  TORCH_CHECK(total == mask_logits.size(0), op, ": mask_logits has ", mask_logits.size(0), " rows, the images ", total, " RoIs");
+  return desc;
+}
+
+std::tuple<at::Tensor, at::Tensor> maskrcnn_loss(const at::Tensor& mask_logits, at::TensorList proposals, at::TensorList gt_masks,
+                                                 at::TensorList gt_labels, at::TensorList matched_idxs) {
+  const char* op = "maskrcnn_loss";
+  auto desc = mask_images(mask_logits, proposals, gt_masks, gt_labels, matched_idxs, false, op);
+  at::cuda::CUDAGuard guard(mask_logits.device());
+  const int64_t P = mask_logits.size(0), M = mask_logits.size(2);
+  at::Tensor loss = at::empty({}, mask_logits.options());
+  at::Tensor targets = at::empty({P, M, M}, mask_logits.options());
+  const size_t wsb = vb200_mask_loss_workspace_bytes((int)desc.size(), P, (int)M);
+  at::Tensor ws = workspace(wsb, mask_logits);
+  check_rc(vb200_mask_loss(desc.data(), (int)desc.size(), mask_logits.data_ptr<float>(), (int)mask_logits.size(1), (int)M,
+                           loss.data_ptr<float>(), targets.data_ptr<float>(), ws.data_ptr(), wsb, cur_stream()),
+           op);
+  return std::make_tuple(loss, targets);
+}
+
+// An undefined incoming gradient counts as zero.
+at::Tensor maskrcnn_loss_backward(const std::optional<at::Tensor>& grad, const at::Tensor& mask_logits, const at::Tensor& targets,
+                                  at::TensorList gt_labels, at::TensorList matched_idxs) {
+  const char* op = "maskrcnn_loss_backward";
+  auto desc = mask_images(mask_logits, {}, {}, gt_labels, matched_idxs, true, op);
+  const int64_t P = mask_logits.size(0), M = mask_logits.size(2);
+  TORCH_CHECK(targets.is_cuda() && targets.get_device() == mask_logits.get_device() && targets.scalar_type() == at::kFloat &&
+                  targets.dim() == 3 && targets.size(0) == P && targets.size(1) == M && targets.size(2) == M && targets.is_contiguous(),
+              op, ": targets must be the forward's dense float32 [P, M, M] tensor");
+  const bool has = grad.has_value() && grad->defined();
+  at::cuda::CUDAGuard guard(mask_logits.device());
+  at::Tensor g;
+  if (has) {
+    TORCH_CHECK(grad->is_cuda() && grad->get_device() == mask_logits.get_device() && grad->scalar_type() == at::kFloat && grad->numel() == 1,
+                op, ": the gradient must be one float32 value on the logits' GPU");
+    g = grad->contiguous();
+  }
+  at::Tensor out = at::empty(mask_logits.sizes(), mask_logits.options());
+  check_rc(vb200_mask_loss_backward(desc.data(), (int)desc.size(), mask_logits.data_ptr<float>(), targets.data_ptr<float>(),
+                                    (int)mask_logits.size(1), (int)M, has ? g.data_ptr<float>() : nullptr, out.data_ptr<float>(), cur_stream()),
+           op);
+  return out;
+}
+
 // ---- box_iou_rotated (csrc/ops/box_iou_rotated.cpp; checks as cuda/box_iou_rotated_kernel.cu:92-118) ----------------
 at::Tensor box_iou_rotated(const at::Tensor& boxes1, const at::Tensor& boxes2) {
   TORCH_CHECK(boxes1.is_cuda() && boxes2.is_cuda(), "boxes1 and boxes2 must be CUDA tensors");
@@ -1270,6 +1360,8 @@ TORCH_LIBRARY(vision_b200, m) {
   m.def("fcos_cls_loss_backward(Tensor grad, Tensor cls_logits, Tensor[] matched_idxs, Tensor[] labels, Tensor num_foreground) -> Tensor");
   m.def("fcos_box_loss(Tensor bbox_regression, Tensor bbox_ctrness, Tensor[] anchors, Tensor[] gt_boxes, Tensor[] labels, Tensor[] matched_idxs, bool normalize_by_size) -> (Tensor, Tensor, Tensor)");
   m.def("fcos_box_loss_backward(Tensor? grad_box, Tensor? grad_ctrness, Tensor bbox_regression, Tensor bbox_ctrness, Tensor[] anchors, Tensor[] gt_boxes, Tensor[] labels, Tensor[] matched_idxs, bool normalize_by_size, Tensor num_foreground) -> (Tensor, Tensor)");
+  m.def("maskrcnn_loss(Tensor mask_logits, Tensor[] proposals, Tensor[] gt_masks, Tensor[] gt_labels, Tensor[] matched_idxs) -> (Tensor loss, Tensor targets)");
+  m.def("maskrcnn_loss_backward(Tensor? grad, Tensor mask_logits, Tensor targets, Tensor[] gt_labels, Tensor[] matched_idxs) -> Tensor");
   m.def("multiscale_roi_align(Tensor[] features, Tensor rois, float[] scales, int pooled_height, int pooled_width, int sampling_ratio, int k_min, int k_max, float canonical_scale, float canonical_level, float eps) -> (Tensor, Tensor)");
   m.def("_roi_align_backward(Tensor grad, Tensor rois, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width, int sampling_ratio, bool aligned) -> Tensor");
   m.def("_roi_pool_backward(Tensor grad, Tensor rois, Tensor argmax, float spatial_scale, SymInt pooled_height, SymInt pooled_width, SymInt batch_size, SymInt channels, SymInt height, SymInt width) -> Tensor");
@@ -1315,6 +1407,8 @@ TORCH_LIBRARY_IMPL(vision_b200, CUDA, m) {
   m.impl("fcos_cls_loss_backward", TORCH_FN(fcos_cls_loss_backward));
   m.impl("fcos_box_loss", TORCH_FN(fcos_box_loss));
   m.impl("fcos_box_loss_backward", TORCH_FN(fcos_box_loss_backward));
+  m.impl("maskrcnn_loss", TORCH_FN(maskrcnn_loss));
+  m.impl("maskrcnn_loss_backward", TORCH_FN(maskrcnn_loss_backward));
   m.impl("resize_crop_normalize", TORCH_FN(resize_crop_normalize));
   m.impl("box_iou_rotated", TORCH_FN(box_iou_rotated));
   m.impl("_deform_conv2d_backward", TORCH_FN(deform_conv2d_backward));

@@ -25,7 +25,10 @@ RetinaNet's head losses, ``RetinaNetClassificationHead.compute_loss`` (retinanet
 elementwise chains, are ONE call each of ``vision_b200::retinanet_cls_loss`` / ``retinanet_box_loss`` for all images, with
 a fused backward (_autograd.py).  FCOS's, ``FCOSHead.compute_loss`` (fcos.py:52-125: the focal, GIoU and centre-ness
 losses after a per-image gather loop and a ``.item()``), is ONE call of ``vision_b200::fcos_cls_loss`` and one of
-``fcos_box_loss``, each with a fused backward."""
+``fcos_box_loss``, each with a fused backward.
+
+Mask R-CNN's ``maskrcnn_loss`` (roi_heads.py:100-129: an fp32 copy of every image's gt masks, roi_align, gathers and a
+BCE chain) is ONE call of ``vision_b200::maskrcnn_loss`` for all images, with a fused backward."""
 from __future__ import annotations
 
 import math
@@ -602,3 +605,40 @@ def fcos_head_compute_loss(self, targets, head_outputs, anchors, matched_idxs, _
                                               [t["boxes"] for t in targets], labels, matched_idxs, self.box_coder.normalize_by_size)
     return {"classification": fcos_cls_loss_op(head_outputs["cls_logits"], matched_idxs, labels), "bbox_regression": loss_box,
             "bbox_ctrness": loss_ctrness}
+
+
+def maskrcnn_loss_supported(mask_logits, proposals, gt_masks, gt_labels, mask_matched_idxs) -> bool:
+    """Inputs the mask-loss kernels reproduce roi_heads.maskrcnn_loss on, decided from shapes alone (no host sync): outside
+    scripting and tracing, a dense CUDA fp32 [P, C, M, M] mask_logits (so autocast's fp16 / bf16 logits keep the reference)
+    with P the proposals' total rows, P > 0 and P * C * M * M below 2^31; per image, on the logits' GPU, fp32 [P_i, 4]
+    proposals, an int64 [P_i] matched_idxs, uint8 or bool [M_i, H, W] gt masks and int64 [M_i] gt labels."""
+    if _traced() or not isinstance(mask_logits, Tensor) or not mask_logits.is_cuda or mask_logits.dtype != torch.float32:
+        return False
+    if mask_logits.dim() != 4 or mask_logits.shape[2] != mask_logits.shape[3] or not mask_logits.is_contiguous():
+        return False
+    lists = (proposals, gt_masks, gt_labels, mask_matched_idxs)
+    if not all(isinstance(v, (list, tuple)) for v in lists) or not proposals or len({len(v) for v in lists}) != 1:
+        return False
+    P, C, M, _ = mask_logits.shape
+    device, total = mask_logits.device, 0
+    for p, g, l, m in zip(*lists):
+        if not (_same_gpu(p, device, torch.float32, 2) and p.shape[1] == 4 and _same_gpu(m, device, torch.int64, 1)
+                and m.shape[0] == p.shape[0] and _same_gpu(l, device, torch.int64, 1) and isinstance(g, Tensor) and g.is_cuda
+                and g.device == device and g.dtype in (torch.uint8, torch.bool) and g.dim() == 3 and g.shape[0] == l.shape[0]):
+            return False
+        total += p.shape[0]
+    return total == P > 0 and C >= 1 and M >= 1 and P * C * M * M < 2**31
+
+
+def maskrcnn_loss_op(mask_logits, proposals, gt_masks, gt_labels, mask_matched_idxs):
+    """The mask loss and the [P, M, M] fp32 targets (each positive RoI's gt mask projected on its box) of one fused call."""
+    _lib.load_ops()
+    return torch.ops.vision_b200.maskrcnn_loss(mask_logits, list(proposals), list(gt_masks), list(gt_labels), list(mask_matched_idxs))
+
+
+def maskrcnn_loss(mask_logits, proposals, gt_masks, gt_labels, mask_matched_idxs, _orig=None):
+    """roi_heads.maskrcnn_loss as one fused call for all images: the masks projected on the boxes straight from their uint8 /
+    bool bytes, the BCE of each RoI's label plane, and a dense gradient of mask_logits written in one pass."""
+    if not maskrcnn_loss_supported(mask_logits, proposals, gt_masks, gt_labels, mask_matched_idxs):
+        return _orig(mask_logits, proposals, gt_masks, gt_labels, mask_matched_idxs)
+    return maskrcnn_loss_op(mask_logits, proposals, gt_masks, gt_labels, mask_matched_idxs)[0]
